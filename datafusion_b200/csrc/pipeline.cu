@@ -29,7 +29,9 @@
 #include "expr_dev.cuh"
 #include "expr_dec.cuh"
 #include "bloom.cuh"
+#include "tma.cuh"
 #include <climits>
+#include <algorithm>
 #include <array>
 
 namespace dfgpu {
@@ -44,6 +46,14 @@ enum SinkKind : int { SINK_NONE = 0, SINK_COUNT = 1, SINK_BUILD = 2, SINK_AGG = 
                       SINK_PACK = 6 /* build sink, table size unknown: {key, payload} records to a staging buffer, inserted afterwards */ };
 constexpr int kStageMaybe = 3;   // DFGPU_STAGE_MAYBE
 constexpr int kPipeVarDefault = 11;   // pipe_kernel's VAR when DFGPU_PIPE_VAR is not set (H100 SXM at 400 W, Q3 SF100 lineitem pass: 17.5 ms; 43 20.4-20.9 ms)
+// ring-fed phase A: at most kMaxRing streamed columns, kMaxRingStages tiles per warp ring, the mbarriers in the first kRingBarBytes of the
+// dynamic shared memory; kGather gathered argument columns
+constexpr int kMaxRing = 4, kMaxRingStages = 4, kRingBarBytes = 256, kGather = 2;
+constexpr int kErrRingAgg = 8;   // error bit (next to ErrBits): the ring kernel met an aggregate that fill_ring should not have admitted
+// bytes of rings per block.  The aggregate sink runs three blocks per SM with 2-tile rings: its phase B lookups need the warps (Q3 SF100
+// lineitem pass on an H100 SXM at 700 W: 15.0 ms, against 18.5 ms with two blocks and 4-tile rings).  The pack sink runs two blocks with
+// 4-tile rings (orders pass: 1.71 ms, against 1.78 ms with 3-tile rings).
+constexpr int ring_smem(int sink) { return sink == SINK_AGG ? 48 * 1024 : 96 * 1024; }
 
 struct LookupDev {
   int mode, stride /* 8-byte words per record */, has_payload, pad;
@@ -69,6 +79,9 @@ struct PipeParams {
   // unordered output sink
   int n_out, out_src[kMaxPipeCols], out_width[kMaxPipeCols]; void* out_dst[kMaxPipeCols]; unsigned long long* out_counter;
   ENode pool[kPoolNodes];
+  // ring-fed phase A (pipe_kernel VAR bit 64): ring_stages > 0 when this batch qualifies (fill_params)
+  int ring_stages, ring_bytes /* one stage: a 256-row warp tile of every ring column */, ring_n, ring_col[kMaxRing], ring_off[kMaxPipeCols] /* byte offset in a stage */;
+  int n_gather, gather_node[kGather];   // pool nodes of agg[0]'s column operands, loaded for all survivors of a round before evaluating
 };
 
 // ---- cache-policy loads: the table scan is read-once (evict first), the lookup structures should stay in L2 ----
@@ -202,6 +215,29 @@ __device__ __forceinline__ uint64_t eval_int_fast(const ENode* __restrict__ node
   }
   return s0;
 }
+// the same program with its first `ng` column operands already loaded (g0 first): the loads of a round were all issued before the first
+// evaluation instead of one dependent access per node; same operations in the same order
+__device__ __forceinline__ uint64_t eval_int_gathered(const ENode* __restrict__ nodes, int n, int64_t row, const uint64_t* ext, int ng, uint64_t g0, uint64_t g1) {
+  uint64_t s0 = 0, s1 = 0, s2 = 0, s3 = 0;
+#pragma unroll 1
+  for (int i = 0; i < n; ++i) {
+    const ENode& nd = nodes[i];
+    if (nd.kind == DFGPU_EXPR_BINARY) {
+      uint64_t r = nd.op == DFGPU_OP_PLUS ? s1 + s0 : (nd.op == DFGPU_OP_MINUS ? s1 - s0 : s1 * s0);
+      if (type_width_prim(nd.out_type) < 8) r = wrap_to_type(r, nd.out_type);
+      s0 = r; s1 = s2; s2 = s3;
+    } else {
+      uint64_t v;
+      if (nd.kind == DFGPU_EXPR_COLUMN) {
+        if (ng > 0) { v = g0; g0 = g1; --ng; }
+        else v = load_col_value(nd, row);
+      } else if (nd.kind == DFGPU_EXPR_LITERAL) v = nd.lit;
+      else { v = ext[nd.voff] >> (int)nd.lit; const int w = type_width_prim(nd.out_type); if (w < 8) { v &= (1ull << (8 * w)) - 1ull; if (type_is_signed_int(nd.out_type)) v = (uint64_t)(((int64_t)(v << (64 - 8 * w))) >> (64 - 8 * w)); } }
+      s3 = s2; s2 = s1; s1 = s0; s0 = v;
+    }
+  }
+  return s0;
+}
 
 // programs that touch Decimal128 values (small == 3): the 128-bit interpreter; returns the low word, *hi the high word
 __device__ __noinline__ uint64_t pipe_eval_dec(const ENode* nodes, int n, int64_t row, const uint64_t* ext, int* err_ok, unsigned long long* hi) {
@@ -307,6 +343,40 @@ __device__ __forceinline__ void load8(const ColRef& c, int64_t row0, int64_t n, 
     }
   }
 }
+// ring-fed phase A: the lane's 8 rows are row0 + 32 j (row0 = tile start + lane), so every shared-memory load of the warp reads
+// consecutive elements (no bank conflicts).  `src` is the column's slice of the ring stage; a tile that is not full was not streamed
+// and is read from global memory.
+__device__ __forceinline__ void ring_load8(const ColRef& c, const unsigned char* src, bool full, int64_t row0, int64_t n, uint64_t v[kWarpRows], uint64_t pol) {
+  if (full) {
+    const int lane = (int)(row0 & 31);
+    switch (c.width) {
+      case 8:
+#pragma unroll
+        for (int j = 0; j < kWarpRows; ++j) v[j] = ((const uint64_t*)src)[32 * j + lane];
+        break;
+      case 4:
+#pragma unroll
+        for (int j = 0; j < kWarpRows; ++j) v[j] = ext32(((const uint32_t*)src)[32 * j + lane], c.sgn);
+        break;
+      case 2:
+#pragma unroll
+        for (int j = 0; j < kWarpRows; ++j) v[j] = ext16(((const uint16_t*)src)[32 * j + lane], c.sgn);
+        break;
+      default:
+#pragma unroll
+        for (int j = 0; j < kWarpRows; ++j) v[j] = ext8(((const uint8_t*)src)[32 * j + lane], c.sgn);
+        break;
+    }
+  } else {
+#pragma unroll 1
+    for (int j = 0; j < kWarpRows; ++j) {
+      const int64_t r = row0 + 32 * j;
+      const uint64_t x = r < n ? ld_stream_int(c.ptr, c.width, c.sgn, r, pol) : 0ull;
+#pragma unroll
+      for (int k = 0; k < kWarpRows; ++k) if (k == j) v[k] = x;
+    }
+  }
+}
 // validity bits of the same 8 rows (bit j = row0 + j is non-NULL)
 __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_t n) {
   if (!c.valid) return 0xFFu;
@@ -323,21 +393,33 @@ __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_
 //              while its odd neighbour adds the same row's value (then the roles swap) — one reduction request per row instead of two;
 //   bit 5 (32) sector-aligned column loads in phase A: a lane's 8 rows are read as one or two whole 32-byte sectors (each as two
 //              back-to-back 128-bit loads, the widest sm_90 has: the same requests as without the bit) when the column base is 32-byte aligned.
+//   bit 6 (64) ring-fed phase A: the columns phase A reads for every row (predicate terms, keys of the filter / bitmap stages) arrive by
+//              TMA bulk copies in a ring of ring_stages warp tiles per warp in dynamic shared memory; lane 0 refills the ring S - 1 tiles
+//              ahead, so a warp in phase B keeps its next tiles in flight.  Phase B loads agg[0]'s column operands of the whole round
+//              before evaluating (replaces bit 0).  Blocks per SM and ring sizes: ring_smem.  Chosen by launch_pipe, not by DFGPU_PIPE_VAR.
 // DFGPU_PIPE_VAR selects the instantiation (aggregate sink; bits 1 and 5 also for the pack sink, bit 1 for the unordered-output sink); 0 is the
 // kernel without any of them, 11 the default.  Tried and removed: four instead of two survivors per lane and phase-B round; prefetching the
 // table record and the argument sectors already when a row passes the membership filter in phase A (the prefetches of five tiles queue up
 // in front of the column stream).
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
 template <int SINK, bool DEC, int VAR = 0>
-__global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams* __restrict__ gp, int64_t n, unsigned long long* __restrict__ counters /* [alive, inserted, fail, err] */) {
+__global__ void __launch_bounds__(kPipeThreads, ((VAR & 64) && SINK == SINK_PACK) ? 2 : 3) pipe_kernel(const PipeParams* __restrict__ gp, int64_t n, unsigned long long* __restrict__ counters /* [alive, inserted, fail, err] */) {
   constexpr int PB = kPhaseB, PBG = kPhaseBGroup, QC = kQueueCap;
+  constexpr bool RING = (VAR & 64) != 0;
   __shared__ PipeParams sp;
   __shared__ uint32_t q_rows[kPipeWarps][QC];
+  extern __shared__ __align__(128) unsigned char dyn_smem[];   // RING: mbarriers [warp][stage], then the rings [warp][stage][ring_bytes]
   for (int i = threadIdx.x; i < (int)(sizeof(PipeParams) / 4); i += kPipeThreads) ((uint32_t*)&sp)[i] = ((const uint32_t*)gp)[i];
+  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  uint64_t* ring_bar = (uint64_t*)dyn_smem + wib * kMaxRingStages;
+  if (RING && lane == 0) {
+#pragma unroll 1
+    for (int s = 0; s < kMaxRingStages; ++s) mbar_init(&ring_bar[s], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
   __syncthreads();
   const uint64_t pol_stream = (sp.hints & 1) ? policy_evict_first() : policy_normal();
   const uint64_t pol_keep = (sp.hints & 2) ? policy_evict_last() : policy_normal();
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   uint32_t* q_row = q_rows[wib];
   unsigned int alive_cnt = 0, ins_cnt = 0;
   int err_ok[2] = {0, 0};
@@ -345,13 +427,46 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
   unsigned int qn = 0;   // queue length (warp-uniform)
   const int64_t ntiles = (n + kWarpTile - 1) / kWarpTile;
   const int64_t gwarp = (int64_t)blockIdx.x * kPipeWarps + wib, nwarps = (int64_t)gridDim.x * kPipeWarps;
+  // RING: the warp's i-th tile (gwarp + i nwarps) lives in stage i % S; only full tiles are streamed (bulk copies move multiples of 16 bytes)
+  const int S = sp.ring_stages;
+  auto ring_stage = [&](int s) { return dyn_smem + kRingBarBytes + (size_t)(wib * S + s) * sp.ring_bytes; };
+  auto ring_issue = [&](int64_t t, int s) {
+    if (t < ntiles && (t + 1) * kWarpTile <= n) {
+      mbar_expect_tx(&ring_bar[s], (uint32_t)sp.ring_bytes);
+      unsigned char* dst = ring_stage(s);
+#pragma unroll 1
+      for (int k = 0; k < sp.ring_n; ++k) {
+        const ColRef& c = sp.col[sp.ring_col[k]];
+        tma_load_1d_hint(dst + sp.ring_off[sp.ring_col[k]], (const char*)c.ptr + t * kWarpTile * c.width, (uint32_t)(kWarpTile * c.width), &ring_bar[s], pol_stream);
+      }
+    }
+  };
+  if (RING && lane == 0) {
+#pragma unroll 1
+    for (int k = 0; k + 1 < S; ++k) ring_issue(gwarp + k * nwarps, k);
+  }
+  unsigned int it = 0;     // RING: tiles of this warp so far: stage it % S, mbarrier phase parity (it / S) & 1
   for (int64_t tile = gwarp; tile < ntiles + nwarps; tile += nwarps) {   // one extra trip per warp drains its queue
     const bool draining = tile >= ntiles;
     if (!draining) {
       // =============================== phase A ===============================
-      const int64_t row0 = tile * kWarpTile + (int64_t)lane * kWarpRows;
-      uint32_t mask = row0 + kWarpRows <= n ? 0xFFu : (row0 < n ? (1u << (int)(n - row0)) - 1u : 0u);
-      if ((VAR & 2) && sp.n_stages > 0 && row0 < n) {
+      const int64_t row0 = RING ? tile * kWarpTile + lane : tile * kWarpTile + (int64_t)lane * kWarpRows;
+      uint32_t mask = 0;
+      const unsigned char* stage = nullptr;
+      bool full = false;
+      if (RING) {
+#pragma unroll
+        for (int j = 0; j < kWarpRows; ++j) mask |= (uint32_t)(row0 + 32 * j < n) << j;
+        const int rs = (int)(it % (unsigned)S);
+        if (lane == 0) ring_issue(tile + (int64_t)(S - 1) * nwarps, rs == 0 ? S - 1 : rs - 1);   // the stage the previous tile used: every lane has read it
+        full = (tile + 1) * kWarpTile <= n;
+        if (full) mbar_wait(&ring_bar[rs], (it / (unsigned)S) & 1u);
+        stage = ring_stage(rs);
+        ++it;
+      } else {
+        mask = row0 + kWarpRows <= n ? 0xFFu : (row0 < n ? (1u << (int)(n - row0)) - 1u : 0u);
+      }
+      if ((VAR & 2) && !RING && sp.n_stages > 0 && row0 < n) {
         const ColRef& kc0 = sp.col[sp.stage[0].key_col];
         prefetch_l2((const char*)kc0.ptr + row0 * kc0.width);
       }
@@ -360,7 +475,8 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
         for (int t = 0; t < sp.n_terms; ++t) {
           const ColRef c = sp.col[sp.term_col[t]];
           uint64_t v[kWarpRows];
-          load8<(VAR & 32) != 0>(c, row0, n, v, pol_stream);
+          if (RING) ring_load8(c, stage + sp.ring_off[sp.term_col[t]], full, row0, n, v, pol_stream);
+          else load8<(VAR & 32) != 0>(c, row0, n, v, pol_stream);
           mask &= valid8(c, row0, n);            // a NULL predicate drops the row
           const int op = sp.term_op[t];
           const long long lit = sp.term_lit[t];
@@ -383,7 +499,7 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
           }
           mask &= r;
         }
-      } else if (sp.pred_mode == 2) {   // FilterExec, general expression
+      } else if (!RING && sp.pred_mode == 2) {   // FilterExec, general expression
 #pragma unroll 1
         for (int j = 0; j < kWarpRows; ++j) {
           if (!((mask >> j) & 1u)) continue;
@@ -404,7 +520,8 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
         if (!__any_sync(0xffffffffu, mask != 0)) continue;
         const ColRef kc = sp.col[st.key_col];
         uint64_t key[kWarpRows];
-        load8<(VAR & 32) != 0>(kc, row0, n, key, pol_stream);
+        if (RING) ring_load8(kc, stage + sp.ring_off[st.key_col], full, row0, n, key, pol_stream);
+        else load8<(VAR & 32) != 0>(kc, row0, n, key, pol_stream);
         const uint32_t kvalid = valid8(kc, row0, n);
         if (bitmap) {
           uint32_t w[kWarpRows];
@@ -458,7 +575,7 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
       unsigned int pos = qn + incl - cnt;
 #pragma unroll
       for (int j = 0; j < kWarpRows; ++j)
-        if ((mask >> j) & 1u) { q_row[pos] = (uint32_t)(row0 + j); ++pos; }
+        if ((mask >> j) & 1u) { q_row[pos] = (uint32_t)(row0 + (RING ? 32 : 1) * j); ++pos; }
       qn += __shfl_sync(0xffffffffu, incl, 31);
       __syncwarp();
     }
@@ -488,6 +605,17 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
 #pragma unroll
             for (int u = 0; u < PB; ++u) if (live[u]) prefetch_l2((const char*)nd.col + row[u] * w);
           }
+        }
+      }
+      uint64_t g[kGather][PB];   // RING: agg[0]'s column operands, all issued before the stages' table lookups
+#pragma unroll
+      for (int k = 0; k < kGather; ++k) {
+#pragma unroll
+        for (int u = 0; u < PB; ++u) g[k][u] = 0;
+        if (RING && SINK == SINK_AGG && k < sp.n_gather) {
+          const ENode& nd = sp.pool[sp.gather_node[k]];
+#pragma unroll
+          for (int u = 0; u < PB; ++u) if (live[u]) g[k][u] = load_col_value(nd, row[u]);
         }
       }
 #pragma unroll
@@ -574,7 +702,11 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
 #pragma unroll
             for (int s = 0; s < kMaxStages; ++s) ext[s] = pay[s][u];
             unsigned long long v = 0;
-            if (live[u]) { alive_cnt++; v = eval_int_fast(sp.pool + ag0.start, ag0.n, row[u], ext); }
+            if (live[u]) {
+              alive_cnt++;
+              v = RING ? eval_int_gathered(sp.pool + ag0.start, ag0.n, row[u], ext, sp.n_gather, g[0][u], g[1][u])
+                       : eval_int_fast(sp.pool + ag0.start, ag0.n, row[u], ext);
+            }
             __syncwarp();
             const unsigned long long rp = (unsigned long long)arec[u];
             const unsigned long long prp = __shfl_xor_sync(0xffffffffu, rp, 1);
@@ -628,11 +760,13 @@ __global__ void __launch_bounds__(kPipeThreads, 3) pipe_kernel(const PipeParams*
             const AggDef ag = sp.agg[a];
             if (ag.func == DFGPU_AGG_COUNT_STAR) continue;   // = the row counter
             uint64_t v;
-            if (ag.small == 2) v = eval_int_fast(sp.pool + ag.start, ag.n, row[u], ext);
+            if (ag.small == 2) v = RING && a == 0 ? eval_int_gathered(sp.pool + ag.start, ag.n, row[u], ext, sp.n_gather, g[0][u], g[1][u])
+                                                  : eval_int_fast(sp.pool + ag.start, ag.n, row[u], ext);
             else if (DEC && ag.cls == C_DEC && ag.func == DFGPU_AGG_SUM) {
               pipe_sum_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, ag.nn_word >= 0 ? rec + ag.nn_word : nullptr);
               continue;
             } else {
+              if (RING) { atomicOr(&counters[3], (unsigned long long)kErrRingAgg); continue; }   // fill_ring admits integer programs and COUNT(*) only
               v = pipe_eval<DEC>(sp.pool + ag.start, ag.n, ag.small, row[u], ext, err_ok);
               if (!err_ok[1]) continue;                      // NULL inputs are skipped (accumulate.rs:373-470)
             }
@@ -1004,7 +1138,7 @@ struct dfgpu_pipeline {
   bool finished = false;
   DevBuf params_dev, counters;
   std::deque<BatchPtr> outq;
-  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0;
+  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0;
   std::string name;   // optional label: the kernel-timing family becomes "pipe:<name>" (dfgpu_kernel_time)
 };
 
@@ -1124,6 +1258,35 @@ static bool expr_can_be_null(const ExprPlan& plan, const std::vector<DCol>& cols
   return false;
 }
 
+// The ring-fed phase A (pipe_kernel VAR bit 64) serves batches whose phase A is a conjunction of `column <cmp> literal` terms (or no
+// predicate) plus filter / bitmap stage tests, over columns without validity bitmaps, and whose aggregates (if any) are COUNT(*) or
+// integer programs (eval_int_fast); the streamed columns need 16-byte-aligned bases and at least two 256-row tiles per warp ring must
+// fit ring_smem(sink).  Everything else keeps ring_stages = 0 and runs the other instantiations.
+static void fill_ring(PipeParams* pp, int ring_bytes_budget) {
+  if (pp->pred_mode == 2) return;
+  std::vector<int> ring;
+  auto add = [&](int c) { if (std::find(ring.begin(), ring.end(), c) == ring.end()) ring.push_back(c); };
+  if (pp->pred_mode == 1)
+    for (int t = 0; t < pp->n_terms; ++t) add(pp->term_col[t]);
+  for (int s = 0; s < pp->n_stages; ++s) {
+    const StageDev& st = pp->stage[s];
+    if (pp->col[st.key_col].valid) return;
+    if (st.lk.mode == LK_BITMAP || (st.lk.bloom && st.kind != DFGPU_STAGE_ANTI)) add(st.key_col);   // the keys phase A tests
+  }
+  for (int a = 0; a < pp->n_aggs; ++a) if (pp->agg[a].func != DFGPU_AGG_COUNT_STAR && pp->agg[a].small != 2) return;   // the general interpreters stay out of the ring kernel
+  if (ring.empty() || (int)ring.size() > kMaxRing) return;
+  int bytes = 0;
+  for (int c : ring) {
+    if (pp->col[c].valid || !pp->col[c].vec) return;
+    pp->ring_off[c] = bytes;
+    bytes += kWarpTile * pp->col[c].width;
+  }
+  const int stages = std::min(kMaxRingStages, ring_bytes_budget / (kPipeWarps * bytes));
+  if (stages < 2) return;
+  pp->ring_stages = stages; pp->ring_bytes = bytes; pp->ring_n = (int)ring.size();
+  for (size_t k = 0; k < ring.size(); ++k) pp->ring_col[k] = ring[k];
+}
+
 static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipeParams* pp) {
   memset(pp, 0, sizeof(*pp));
   pp->n_cols = (int)cols.size();
@@ -1193,23 +1356,50 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
           DF_CHECK(!expr_can_be_null(ag.plan, cols), DFGPU_ERR_UNSUPPORTED, "pipeline: nullable aggregate input needs one more accumulator word in the lookup (n_acc_words)");
       }
     }
+    if (pp->n_aggs > 0 && pp->agg[0].small == 2) {
+      const AggDef& d = pp->agg[0];
+      int ng = 0;
+      for (int i = 0; i < d.n; ++i) if (pp->pool[d.start + i].kind == DFGPU_EXPR_COLUMN) ng++;
+      if (ng <= kGather) {
+        for (int i = 0; i < d.n; ++i) if (pp->pool[d.start + i].kind == DFGPU_EXPR_COLUMN) pp->gather_node[pp->n_gather++] = d.start + i;
+      }
+    }
   }
+  fill_ring(pp, ring_smem(p->sink));
 }
 
 static void check_errors(unsigned long long err) {
   if (err & ERR_DIV_ZERO) throw Error(DFGPU_ERR_ARITH, "Arrow error: Divide by zero error");
   if (err & ERR_OVERFLOW) throw Error(DFGPU_ERR_ARITH, "Arrow error: Arithmetic overflow");
   if (err & ERR_CAST) throw Error(DFGPU_ERR_ARITH, "Arrow error: Cast error: Can't cast value to the target type (out of range)");
+  if (err & kErrRingAgg) throw Error(DFGPU_ERR_INVALID, "internal: the ring-fed pipeline kernel was given an aggregate it does not evaluate");
 }
 
 template <int SINK>
-static void launch_pipe(dfgpu_pipeline* p, int64_t n, const char* timer_name) {
+static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, const char* timer_name) {
   dfgpu_ctx* ctx = p->ctx;
   const int64_t ntiles = (n + kPipeTile - 1) / kPipeTile;
   // programs that touch Decimal128 values run a second instantiation of the kernel (128-bit interpreter linked in): the integer
   // instantiation stays byte for byte what it was
   bool dec = p->has_pred && p->pred.has_decimal;
   for (const auto& ag : p->aggs) dec = dec || (ag.has_expr && ag.plan.has_decimal);
+  const PipeParams* gp = (const PipeParams*)p->params_dev.ptr;
+  unsigned long long* cnt = p->counters.as<unsigned long long>();
+  const std::string tname = p->name.empty() ? std::string(timer_name) : "pipe:" + p->name;
+  if constexpr (SINK == SINK_AGG || SINK == SINK_PACK) if (!dec && pp.ring_stages > 0 && !getenv("DFGPU_PIPE_VAR")) {
+    constexpr int RV = SINK == SINK_AGG ? 64 | 8 : 64;   // ring + lane-paired REDs for the aggregate sink, ring alone for the pack sink
+    const int smem = kRingBarBytes + kPipeWarps * pp.ring_stages * pp.ring_bytes;
+    // the attribute belongs to the current device: set on every launch (a host-side call), so any device and thread may launch
+    DF_CUDA(cudaFuncSetAttribute(pipe_kernel<SINK, false, RV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingBarBytes + ring_smem(SINK)));
+    int blocks_per_sm = 0;
+    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, pipe_kernel<SINK, false, RV>, kPipeThreads, smem));
+    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
+    KernelTimer kt(ctx, tname.c_str());
+    pipe_kernel<SINK, false, RV><<<grid, kPipeThreads, smem, ctx->stream>>>(gp, n, cnt);
+    DF_LAUNCH_CHECK(ctx);
+    p->m_ring_launches++;
+    return;
+  }
   static const int blocks_env = getenv("DFGPU_PIPE_BLOCKS_PER_SM") ? atoi(getenv("DFGPU_PIPE_BLOCKS_PER_SM")) : 0;
   int blocks_per_sm = blocks_env;
   if (blocks_per_sm <= 0) {   // persistent blocks: exactly one resident wave (a second wave would start after the first finished)
@@ -1218,11 +1408,8 @@ static void launch_pipe(dfgpu_pipeline* p, int64_t n, const char* timer_name) {
     blocks_per_sm = std::max(1, blocks_per_sm);
   }
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * blocks_per_sm);
-  const std::string tname = p->name.empty() ? std::string(timer_name) : "pipe:" + p->name;
   KernelTimer kt(ctx, tname.c_str());
   const int var_env = getenv("DFGPU_PIPE_VAR") ? atoi(getenv("DFGPU_PIPE_VAR")) : kPipeVarDefault;
-  const PipeParams* gp = (const PipeParams*)p->params_dev.ptr;
-  unsigned long long* cnt = p->counters.as<unsigned long long>();
   if (dec) pipe_kernel<SINK, true><<<grid, kPipeThreads, 0, ctx->stream>>>(gp, n, cnt);
   else if (SINK == SINK_AGG && var_env == 1) pipe_kernel<SINK_AGG, false, 1><<<grid, kPipeThreads, 0, ctx->stream>>>(gp, n, cnt);
   else if (SINK == SINK_AGG && var_env == 2) pipe_kernel<SINK_AGG, false, 2><<<grid, kPipeThreads, 0, ctx->stream>>>(gp, n, cnt);
@@ -1296,7 +1483,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
       pp.out_dst[0] = recs.ptr;
       pp.out_counter = p->counters.as<unsigned long long>() + 4;
       upload_params(p, pp);
-      launch_pipe<SINK_PACK>(p, n, "pipeline_build");
+      launch_pipe<SINK_PACK>(p, pp, n, "pipeline_build");
       unsigned long long h8[8];
       DF_CUDA(cudaMemcpyAsync(h8, p->counters.ptr, 64, cudaMemcpyDeviceToHost, ctx->stream));
       DF_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1316,7 +1503,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
       fill_params(p, cols, &pp);
       upload_params(p, pp);
       p->counters.zero();
-      launch_pipe<SINK_BUILD>(p, n, "pipeline_build");
+      launch_pipe<SINK_BUILD>(p, pp, n, "pipeline_build");
       read_counters(p, h);
       check_errors(h[3]);
     }
@@ -1329,7 +1516,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     fill_params(p, cols, &pp);
     upload_params(p, pp);
     p->counters.zero();
-    launch_pipe<SINK_AGG>(p, n, "pipeline_agg");
+    launch_pipe<SINK_AGG>(p, pp, n, "pipeline_agg");
     read_counters(p, h);
     check_errors(h[3]);
     p->m_sink_rows += (int64_t)h[0];
@@ -1348,7 +1535,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     p->counters.zero();
     pp.out_counter = p->counters.as<unsigned long long>() + 4;
     upload_params(p, pp);
-    launch_pipe<SINK_OUTPUT_ANY>(p, n, "pipeline_output");
+    launch_pipe<SINK_OUTPUT_ANY>(p, pp, n, "pipeline_output");
     unsigned long long h8[8];
     DF_CUDA(cudaMemcpyAsync(h8, p->counters.ptr, 64, cudaMemcpyDeviceToHost, ctx->stream));
     DF_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -1835,6 +2022,7 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name) {
   if (s == "sink_rows") return p->m_sink_rows;
   if (s == "output_rows") return p->m_output_rows;
   if (s == "num_groups") return p->m_groups;
+  if (s == "ring_launches") return p->m_ring_launches;   // launches of the ring-fed pipeline kernel
   return -1;
 }
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p) {
