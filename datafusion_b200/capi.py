@@ -29,6 +29,7 @@ NULL_EQUALS_NOTHING, NULL_EQUALS_NULL = 0, 1
 AGG_PARTIAL, AGG_FINAL, AGG_FINAL_PARTITIONED, AGG_SINGLE, AGG_SINGLE_PARTITIONED, AGG_PARTIAL_REDUCE = range(6)
 AGG_SUM, AGG_COUNT, AGG_MIN, AGG_MAX, AGG_AVG, AGG_COUNT_STAR = range(1, 7)
 STAGE_INNER, STAGE_SEMI, STAGE_ANTI, STAGE_MAYBE = range(4)
+DENSE_MAX_GROUPS = 256   # DFGPU_DENSE_MAX_GROUPS: slots of a dense aggregate's key domain
 
 GEN_SEQ, GEN_UNIFORM, GEN_SPLITMIX, GEN_PERM, GEN_SPARSE_OF = range(5)
 
@@ -164,7 +165,7 @@ EXPORTS = [
     "dfgpu_comm_destroy", "dfgpu_exchange_create", "dfgpu_exchange_run", "dfgpu_exchange_columns", "dfgpu_exchange_destroy",
     "dfgpu_lookup_default_options", "dfgpu_lookup_create", "dfgpu_lookup_metric", "dfgpu_lookup_destroy", "dfgpu_lookup_clear",
     "dfgpu_lookup_filter_buffer", "dfgpu_lookup_filter_allreduce_peer", "dfgpu_pipeline_sink_output_unordered", "dfgpu_pipeline_set_name", "dfgpu_column_minmax_device", "dfgpu_column_sum_device",
-    "dfgpu_pipeline_create", "dfgpu_pipeline_sink_build", "dfgpu_pipeline_sink_aggregate", "dfgpu_pipeline_sink_output",
+    "dfgpu_pipeline_create", "dfgpu_pipeline_sink_build", "dfgpu_pipeline_sink_aggregate", "dfgpu_pipeline_sink_aggregate_dense", "dfgpu_pipeline_sink_output",
     "dfgpu_pipeline_push_host", "dfgpu_pipeline_push_device", "dfgpu_pipeline_push_arrow", "dfgpu_pipeline_finish",
     "dfgpu_pipeline_next", "dfgpu_pipeline_metric", "dfgpu_pipeline_destroy",
     "dfgpu_dictionary_create", "dfgpu_dictionary_unify", "dfgpu_dictionary_code", "dfgpu_dictionary_size", "dfgpu_dictionary_value",
@@ -289,6 +290,7 @@ def load_library() -> C.CDLL:
     sig("dfgpu_pipeline_create", C.c_int, [vp, P(i32), i32, P(ExprNode), i32, P(PipelineStage), i32, P(vp)])
     sig("dfgpu_pipeline_sink_build", C.c_int, [vp, vp, i32, P(i32), i32])
     sig("dfgpu_pipeline_sink_aggregate", C.c_int, [vp, P(i32), i32, P(PipelineAgg), i32, i32, i64])
+    sig("dfgpu_pipeline_sink_aggregate_dense", C.c_int, [vp, P(i32), P(i64), P(i64), i32, P(PipelineAgg), i32, i32, i64])
     sig("dfgpu_pipeline_sink_output", C.c_int, [vp, P(i32), i32, i64])
     sig("dfgpu_pipeline_set_name", C.c_int, [vp, C.c_char_p])
     sig("dfgpu_pipeline_push_host", C.c_int, [vp, P(Column), i32])
@@ -830,8 +832,7 @@ class Pipeline(_Operator):
         self._keep.append(target)
         self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_build(self.h, target.h, key_col, _i32arr(list(payload_cols)), len(payload_cols)))
 
-    def sink_aggregate(self, group_cols, aggs, mode=AGG_SINGLE, batch_size=0):
-        """aggs: [(func, nodes or None)]"""
+    def _agg_array(self, aggs):
         arr = (PipelineAgg * max(len(aggs), 1))()
         self._agg_nodes = []
         for i, (f, nodes) in enumerate(aggs):
@@ -842,7 +843,24 @@ class Pipeline(_Operator):
                 arr[i].n_nodes, arr[i].expr = len(nodes), C.addressof(na)
             else:
                 arr[i].n_nodes, arr[i].expr = 0, None
+        return arr
+
+    def sink_aggregate(self, group_cols, aggs, mode=AGG_SINGLE, batch_size=0):
+        """aggs: [(func, nodes or None)]"""
+        arr = self._agg_array(aggs)
         self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_aggregate(self.h, _i32arr(list(group_cols)), len(group_cols), arr, len(aggs), mode, batch_size))
+
+    def sink_aggregate_dense(self, group_cols, key_range, aggs, mode=AGG_SINGLE, batch_size=0):
+        """GROUP BY keys in small declared domains: key_range = [(min, max)] per group column (inclusive, NULL is a group of its
+        own), at most DENSE_MAX_GROUPS slots in all; no group columns = one output row.  aggs: [(func, nodes or None)]"""
+        group_cols, key_range = list(group_cols), list(key_range)
+        if len(key_range) != len(group_cols):
+            raise ValueError("sink_aggregate_dense: one (min, max) per group column")
+        arr = self._agg_array(aggs)
+        kmin = (C.c_int64 * max(len(key_range), 1))(*[int(lo) for lo, _ in key_range])
+        kmax = (C.c_int64 * max(len(key_range), 1))(*[int(hi) for _, hi in key_range])
+        self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_aggregate_dense(self.h, _i32arr(group_cols), kmin, kmax, len(group_cols), arr, len(aggs),
+                                                                        mode, batch_size))
 
     def sink_output(self, out_cols, batch_size=0, ordered=True):
         fn = self.ctx.lib.dfgpu_pipeline_sink_output if ordered else self.ctx.lib.dfgpu_pipeline_sink_output_unordered

@@ -43,7 +43,8 @@ constexpr int kMaxPipeCols = 16, kMaxStages = 3, kMaxPipeAggs = 4, kMaxExt = 8, 
 constexpr int kPipeThreads = 256, kPipeItems = 4, kPipeTile = kPipeThreads * kPipeItems;
 enum LookupMode : int { LK_HASH = 0, LK_BITMAP = 1 };
 enum SinkKind : int { SINK_NONE = 0, SINK_COUNT = 1, SINK_BUILD = 2, SINK_AGG = 3, SINK_OUTPUT = 4, SINK_OUTPUT_ANY = 5 /* row order unspecified */,
-                      SINK_PACK = 6 /* build sink, table size unknown: {key, payload} records to a staging buffer, inserted afterwards */ };
+                      SINK_PACK = 6 /* build sink, table size unknown: {key, payload} records to a staging buffer, inserted afterwards */,
+                      SINK_DENSE = 7 /* aggregate over group keys in small declared domains: slot arithmetic, shared-memory accumulators */ };
 constexpr int kStageMaybe = 3;   // DFGPU_STAGE_MAYBE
 constexpr int kPipeVarDefault = 11;   // pipe_kernel's VAR when DFGPU_PIPE_VAR is not set (H100 SXM at 400 W, Q3 SF100 lineitem pass: 17.5 ms; 43 20.4-20.9 ms)
 // ring-fed phase A: at most kMaxRing streamed columns, kMaxRingStages tiles per warp ring, the mbarriers in the first kRingBarBytes of the
@@ -402,8 +403,132 @@ __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_
 // table record and the argument sectors already when a row passes the membership filter in phase A (the prefetches of five tiles queue up
 // in front of the column stream).
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
+
+// ------------------------------------------------------------------------------------------
+// dense-group aggregate sink (SINK_DENSE): AggregateExec over a FilterExec (and probe stages) whose GROUP BY keys lie in small
+// declared domains (TPC-H Q1: l_returnflag x l_linestatus; Q4: o_orderpriority; Q6: no GROUP BY).  The group id is arithmetic:
+//   slot = sum_g stride_g * idx_g,  idx_g = key - min_g (a value) or max_g - min_g + 1 (NULL),  row-major strides,
+// at most kDenseMaxSlots slots, so no hash table.  The sink's parameters (DenseParams) sit right behind PipeParams in the same device
+// allocation; PipeParams and the other sinks' code are unchanged.  Accumulators are privatised per BLOCK in dynamic shared memory
+// (a 256-slot domain with 8 aggregates is up to 80 KB: per-warp copies do not fit); before touching them the lanes of a phase-B
+// round that share a slot are combined (__match_any_sync + a shuffle tree), so a warp issues one shared atomic per distinct slot
+// and aggregate instead of 32.  At kernel end every block adds its slots into the pipeline's global accumulator array (acc), which
+// persists across pushes; the row loop makes no global atomics.
+// ------------------------------------------------------------------------------------------
+constexpr int kDenseMaxSlots = 256, kDenseMaxKeys = 8, kDenseMaxAggs = 8, kDenseMaxWords = 40, kDenseMaxXTerms = 4;
+constexpr int kDenseWarpBytes = 48 * 1024;   // per-warp accumulator copies when all eight fit in this many bytes
+// how one aggregate's value combines: none (COUNT: only the non-null counter), add, min, max over u64 / i64 / f64 / i128 words
+enum DenseOp : int { DO_NONE = 0, DO_ADD_U64, DO_ADD_F64, DO_ADD_128, DO_MIN_S64, DO_MAX_S64, DO_MIN_U64, DO_MAX_U64, DO_MIN_F64, DO_MAX_F64, DO_MIN_128, DO_MAX_128 };
+struct DenseKey { int src /* virtual column */, pad; unsigned long long kmin, nvals /* max - min + 1: the index of NULL */, stride; };
+struct DenseAgg { int func, op, small, start, n, word /* value word(s) in a slot, -1 none */, nn_word /* non-null counter, -1 none */, pad; };
+struct DenseParams {
+  int n_keys, n_aggs, n_slots, n_words /* per slot, even: the 128-bit fields are 16-byte aligned; word 0 counts the rows */;
+  DenseKey key[kDenseMaxKeys];
+  DenseAgg agg[kDenseMaxAggs];
+  unsigned long long ident[kDenseMaxWords];   // initial value of each word of a slot (0, or the MIN / MAX identity)
+  unsigned long long* acc;                    // [n_slots][n_words] in global memory
+  int per_warp;                               // 1: one copy of the slots per warp, updated by plain loads and stores; 0: one per block, atomics
+  // `column <cmp> literal` terms of the predicate's conjunction beyond PipeParams' kMaxTerms (TPC-H Q6 has five), tested after them
+  int n_xterms, xterm_col[kDenseMaxXTerms], xterm_op[kDenseMaxXTerms], xterm_uns[kDenseMaxXTerms]; long long xterm_lit[kDenseMaxXTerms];
+};
+constexpr int kDenseParamsOff = (int)((sizeof(PipeParams) + 15) / 16 * 16);   // DenseParams behind PipeParams in the parameter buffer
+constexpr int kDenseAccOff = (int)((sizeof(DenseParams) + 15) / 16 * 16);     // dynamic shared memory: DenseParams, then the slots
+
+// 128-bit compare-and-swap on a generic address (shared memory in the row loop, global memory at the flush)
+__device__ __forceinline__ Rec128 cas128(void* addr, Rec128 cmp, Rec128 val) {
+  Rec128 old;
+  asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
+               : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
+  return old;
+}
+__device__ __forceinline__ bool lt128(unsigned long long alo, unsigned long long ahi, unsigned long long blo, unsigned long long bhi) {
+  return (long long)ahi < (long long)bhi || (ahi == bhi && alo < blo);   // signed 128-bit a < b
+}
+// true when value (lo, hi) replaces the current (clo, chi) under a MIN / MAX op
+__device__ __forceinline__ bool dense_better(int op, unsigned long long lo, unsigned long long hi, unsigned long long clo, unsigned long long chi) {
+  switch (op) {
+    case DO_MIN_S64: return (long long)lo < (long long)clo;
+    case DO_MAX_S64: return (long long)lo > (long long)clo;
+    case DO_MIN_U64: return lo < clo;
+    case DO_MAX_U64: return lo > clo;
+    case DO_MIN_F64: return __longlong_as_double((long long)lo) < __longlong_as_double((long long)clo);
+    case DO_MAX_F64: return __longlong_as_double((long long)lo) > __longlong_as_double((long long)clo);
+    case DO_MIN_128: return lt128(lo, hi, clo, chi);
+    case DO_MAX_128: return lt128(clo, chi, lo, hi);
+    default: return false;
+  }
+}
+__device__ __forceinline__ void dense_combine(int op, unsigned long long& lo, unsigned long long& hi, unsigned long long olo, unsigned long long ohi) {
+  if (op == DO_ADD_U64) lo += olo;   // add_wrapping
+  else if (op == DO_ADD_F64) lo = (unsigned long long)__double_as_longlong(__longlong_as_double((long long)lo) + __longlong_as_double((long long)olo));
+  else if (op == DO_ADD_128) { const unsigned long long s = lo + olo; hi += ohi + (s < lo ? 1ull : 0ull); lo = s; }   // i128 add_wrapping
+  else if (dense_better(op, olo, ohi, lo, hi)) { lo = olo; hi = ohi; }
+}
+// add / min / max (lo, hi) into the word(s) at w
+__device__ __forceinline__ void dense_update(int op, unsigned long long* w, unsigned long long lo, unsigned long long hi) {
+  switch (op) {
+    case DO_ADD_U64: atomicAdd(w, lo); break;
+    case DO_ADD_F64: atomicAdd((double*)w, __longlong_as_double((long long)lo)); break;
+    case DO_ADD_128: {   // the carry out of the low word is decided by this add alone
+      const unsigned long long old = atomicAdd(w, lo);
+      const unsigned long long add_hi = hi + ((old + lo) < old ? 1ull : 0ull);
+      if (add_hi) atomicAdd(w + 1, add_hi);
+      break;
+    }
+    case DO_MIN_S64: atomicMin((long long*)w, (long long)lo); break;
+    case DO_MAX_S64: atomicMax((long long*)w, (long long)lo); break;
+    case DO_MIN_U64: atomicMin(w, lo); break;
+    case DO_MAX_U64: atomicMax(w, lo); break;
+    case DO_MIN_F64: case DO_MAX_F64: {
+      unsigned long long old = *(volatile unsigned long long*)w;
+      while (dense_better(op, lo, 0, old, 0)) {
+        const unsigned long long prev = atomicCAS(w, old, lo);
+        if (prev == old) break;
+        old = prev;
+      }
+      break;
+    }
+    case DO_MIN_128: case DO_MAX_128: {
+      Rec128 cur = cas128(w, Rec128{lo, hi}, Rec128{lo, hi});   // an atomic read of both words (stores only what is already there)
+      while (dense_better(op, lo, hi, cur.lo, cur.hi)) {
+        const Rec128 prev = cas128(w, cur, Rec128{lo, hi});
+        if (prev.lo == cur.lo && prev.hi == cur.hi) break;
+        cur = prev;
+      }
+      break;
+    }
+    default: break;
+  }
+}
+// the same for a slot only this lane writes (per-warp copies): a plain read-modify-write
+__device__ __forceinline__ void dense_apply(int op, unsigned long long* w, unsigned long long lo, unsigned long long hi) {
+  const bool wide = op == DO_ADD_128 || op == DO_MIN_128 || op == DO_MAX_128;
+  unsigned long long clo = w[0], chi = wide ? w[1] : 0ull;
+  dense_combine(op, clo, chi, lo, hi);
+  w[0] = clo;
+  if (wide) w[1] = chi;
+}
+// combine (lo, hi) and the non-null counts over the lanes of each peer group (lanes with the same slot): a tree over the group's
+// lanes, log2(group size) shuffle steps; the group's lowest lane ends with the result
+__device__ __forceinline__ void dense_reduce_peers(unsigned peers, int op, unsigned long long& lo, unsigned long long& hi, unsigned& cnt) {
+  const int lane = threadIdx.x & 31;
+  const bool wide = op == DO_ADD_128 || op == DO_MIN_128 || op == DO_MAX_128;   // warp-uniform
+  unsigned rel = __popc(peers & ((1u << lane) - 1u));   // rank in the group
+  unsigned rest = peers & (0xfffffffeu << lane);          // the group's lanes above this one
+  while (__any_sync(0xffffffffu, rest != 0)) {
+    const int next = __ffs(rest);                         // the next one still in play (1-based, 0 = none)
+    const int src = next ? next - 1 : lane;
+    const unsigned long long tlo = __shfl_sync(0xffffffffu, lo, src);
+    const unsigned long long thi = wide ? __shfl_sync(0xffffffffu, hi, src) : 0ull;
+    const unsigned tc = __shfl_sync(0xffffffffu, cnt, src);
+    if (next) { if (op != DO_NONE) dense_combine(op, lo, hi, tlo, thi); cnt += tc; }
+    rest &= ~__ballot_sync(0xffffffffu, rel & 1u);        // odd ranks have been read: out of play
+    rel >>= 1;
+  }
+}
+
 template <int SINK, bool DEC, int VAR = 0>
-__global__ void __launch_bounds__(kPipeThreads, ((VAR & 64) && SINK == SINK_PACK) ? 2 : 3) pipe_kernel(const PipeParams* __restrict__ gp, int64_t n, unsigned long long* __restrict__ counters /* [alive, inserted, fail, err] */) {
+__global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PACK) || SINK == SINK_DENSE) ? 2 : 3) pipe_kernel(const PipeParams* __restrict__ gp, int64_t n, unsigned long long* __restrict__ counters /* [alive, inserted, fail, err] */) {
   constexpr int PB = kPhaseB, PBG = kPhaseBGroup, QC = kQueueCap;
   constexpr bool RING = (VAR & 64) != 0;
   __shared__ PipeParams sp;
@@ -417,7 +542,18 @@ __global__ void __launch_bounds__(kPipeThreads, ((VAR & 64) && SINK == SINK_PACK
     for (int s = 0; s < kMaxRingStages; ++s) mbar_init(&ring_bar[s], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
+  if constexpr (SINK == SINK_DENSE) {   // dynamic shared memory: DenseParams, then this block's slots
+    const uint32_t* src = (const uint32_t*)((const char*)gp + kDenseParamsOff);
+    for (int i = threadIdx.x; i < (int)(sizeof(DenseParams) / 4); i += kPipeThreads) ((uint32_t*)dyn_smem)[i] = src[i];
+  }
   __syncthreads();
+  if constexpr (SINK == SINK_DENSE) {
+    const DenseParams& dp = *(const DenseParams*)dyn_smem;
+    unsigned long long* sacc = (unsigned long long*)(dyn_smem + kDenseAccOff);
+    const int words = (dp.per_warp ? kPipeWarps : 1) * dp.n_slots * dp.n_words;
+    for (int i = threadIdx.x; i < words; i += kPipeThreads) sacc[i] = dp.ident[i % dp.n_words];
+    __syncthreads();
+  }
   const uint64_t pol_stream = (sp.hints & 1) ? policy_evict_first() : policy_normal();
   const uint64_t pol_keep = (sp.hints & 2) ? policy_evict_last() : policy_normal();
   uint32_t* q_row = q_rows[wib];
@@ -505,6 +641,34 @@ __global__ void __launch_bounds__(kPipeThreads, ((VAR & 64) && SINK == SINK_PACK
           if (!((mask >> j) & 1u)) continue;
           const uint64_t val = pipe_eval<DEC>(sp.pool + sp.pred_start, sp.pred_n, sp.pred_small, row0 + j, nullptr, err_ok);
           if (!(err_ok[1] && (val & 1))) mask &= ~(1u << j);
+        }
+      }
+      if constexpr (SINK == SINK_DENSE) {   // the conjunction's terms beyond kMaxTerms
+        const DenseParams& dp = *(const DenseParams*)dyn_smem;
+#pragma unroll 1
+        for (int t = 0; t < dp.n_xterms; ++t) {
+          const ColRef c = sp.col[dp.xterm_col[t]];
+          uint64_t v[kWarpRows];
+          load8<false>(c, row0, n, v, pol_stream);
+          const long long lit = dp.xterm_lit[t];
+          uint32_t lt = 0, eq = 0;
+          if (dp.xterm_uns[t]) {
+#pragma unroll
+            for (int j = 0; j < kWarpRows; ++j) { lt |= (uint32_t)(v[j] < (uint64_t)lit) << j; eq |= (uint32_t)(v[j] == (uint64_t)lit) << j; }
+          } else {
+#pragma unroll
+            for (int j = 0; j < kWarpRows; ++j) { lt |= (uint32_t)((long long)v[j] < lit) << j; eq |= (uint32_t)((long long)v[j] == lit) << j; }
+          }
+          uint32_t r;
+          switch (dp.xterm_op[t]) {
+            case DFGPU_OP_EQ: r = eq; break;
+            case DFGPU_OP_NEQ: r = ~eq; break;
+            case DFGPU_OP_LT: r = lt; break;
+            case DFGPU_OP_LTEQ: r = lt | eq; break;
+            case DFGPU_OP_GT: r = ~(lt | eq); break;
+            default: r = ~lt; break;
+          }
+          mask &= r & valid8(c, row0, n);
         }
       }
       // bitmap stages decide here; hash stages get their Bloom pre-test (the pushed-down membership filter)
@@ -719,9 +883,81 @@ __global__ void __launch_bounds__(kPipeThreads, ((VAR & 64) && SINK == SINK_PACK
           }
         }
       }
+      if constexpr (SINK == SINK_DENSE) {   // every lane takes part in each step: the combining is warp-collective
+        const DenseParams& dp = *(const DenseParams*)dyn_smem;
+        unsigned long long* sacc = (unsigned long long*)(dyn_smem + kDenseAccOff);
+#pragma unroll 1
+        for (int u = 0; u < PB; ++u) {
+          if (!__any_sync(0xffffffffu, live[u])) continue;
+          uint64_t ext[kMaxStages];
+#pragma unroll
+          for (int s = 0; s < kMaxStages; ++s) ext[s] = pay[s][u];
+          int slot = -1;
+          if (live[u]) {
+            alive_cnt++;
+            unsigned long long sl = 0;
+            bool inside = true;
+#pragma unroll 1
+            for (int k = 0; k < dp.n_keys; ++k) {
+              const DenseKey& dk = dp.key[k];
+              bool isnull = false;
+              uint64_t key;
+              if (dk.src < sp.n_cols) {
+                const ColRef& c = sp.col[dk.src];
+                isnull = c.valid && !bit_get(c.valid, c.voff + row[u]);
+                key = isnull ? 0ull : ld_stream_int(c.ptr, c.width, c.sgn, row[u], pol_stream);
+              } else {
+                const ExtDef e = sp.ext[dk.src - sp.n_cols];
+                uint64_t wd = 0;
+#pragma unroll
+                for (int s = 0; s < kMaxStages; ++s) if (s == e.stage) wd = ext[s];
+                key = ext_field(wd, e.shift, e.width, e.type);
+              }
+              const uint64_t idx = isnull ? dk.nvals : key - dk.kmin;   // modular: one unsigned compare checks both bounds
+              if (idx > dk.nvals || (!isnull && idx == dk.nvals)) { inside = false; break; }
+              sl += idx * dk.stride;
+            }
+            if (inside) slot = (int)sl;
+            else fail |= 2;                                            // a key outside its declared range
+          }
+          const unsigned peers = __match_any_sync(0xffffffffu, slot);
+          const bool lead = slot >= 0 && lane == __ffs(peers) - 1;
+          unsigned long long* const sw = sacc + ((size_t)(dp.per_warp ? wib * dp.n_slots : 0) + (slot < 0 ? 0 : slot)) * dp.n_words;
+          if (lead) {   // word 0: the group's rows (COUNT(*))
+            if (dp.per_warp) sw[0] += (unsigned long long)__popc(peers);
+            else atomicAdd(sw, (unsigned long long)__popc(peers));
+          }
+#pragma unroll 1
+          for (int a = 0; a < dp.n_aggs; ++a) {
+            const DenseAgg& ag = dp.agg[a];
+            if (ag.func == DFGPU_AGG_COUNT_STAR) continue;
+            unsigned long long lo = 0, hi = 0;
+            unsigned ok = 0;
+            if (slot >= 0) {
+              if (ag.small == 2) { lo = eval_int_fast(sp.pool + ag.start, ag.n, row[u], ext); ok = 1; }
+              else if (DEC && ag.small == 3) { lo = pipe_eval_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, &hi); ok = err_ok[1] ? 1 : 0; }
+              else { lo = pipe_eval<DEC>(sp.pool + ag.start, ag.n, ag.small, row[u], ext, err_ok); ok = err_ok[1] ? 1 : 0; }
+              // f64 MIN / MAX skip NaN as the join-keyed sink does (red_f64_min): it stays counted, the value becomes the identity
+              if (ok && (ag.op == DO_MIN_F64 || ag.op == DO_MAX_F64) && isnan(__longlong_as_double((long long)lo))) lo = dp.ident[ag.word];
+            }
+            if (!ok && ag.word >= 0) { lo = dp.ident[ag.word]; hi = ag.op == DO_MIN_128 || ag.op == DO_MAX_128 ? dp.ident[ag.word + 1] : 0ull; }
+            dense_reduce_peers(peers, ag.op, lo, hi, ok);
+            if (lead && ok) {
+              if (dp.per_warp) {
+                if (ag.nn_word >= 0) sw[ag.nn_word] += (unsigned long long)ok;
+                if (ag.op != DO_NONE) dense_apply(ag.op, sw + ag.word, lo, hi);
+              } else {
+                if (ag.nn_word >= 0) atomicAdd(sw + ag.nn_word, (unsigned long long)ok);
+                dense_update(ag.op, sw + ag.word, lo, hi);
+              }
+            }
+          }
+          __syncwarp();   // per-warp copies: this round's stores are seen by the next round's leaders
+        }
+      }
 #pragma unroll
       for (int u = 0; u < PB; ++u) {
-        if (SINK == SINK_OUTPUT_ANY || sunk) break;
+        if (SINK == SINK_OUTPUT_ANY || SINK == SINK_DENSE || sunk) break;
         uint64_t ext[kMaxStages];
 #pragma unroll
         for (int s = 0; s < kMaxStages; ++s) ext[s] = pay[s][u];
@@ -793,6 +1029,44 @@ __global__ void __launch_bounds__(kPipeThreads, ((VAR & 64) && SINK == SINK_PACK
       }
       qn = qbase;
       __syncwarp();
+    }
+  }
+  if constexpr (SINK == SINK_DENSE) {   // flush: this block's slots into the pipeline's accumulators, one thread per slot
+    __syncthreads();
+    const DenseParams& dp = *(const DenseParams*)dyn_smem;
+    unsigned long long* sacc = (unsigned long long*)(dyn_smem + kDenseAccOff);
+    for (int s = threadIdx.x; s < dp.n_slots; s += kPipeThreads) {
+      unsigned long long* w = sacc + (size_t)s * dp.n_words;
+#pragma unroll 1
+      for (int c = 1; dp.per_warp && c < kPipeWarps; ++c) {   // fold the other warps' copies of this slot into warp 0's
+        const unsigned long long* o = w + (size_t)c * dp.n_slots * dp.n_words;
+        if (o[0] == 0ull) continue;
+        w[0] += o[0];
+#pragma unroll 1
+        for (int a = 0; a < dp.n_aggs; ++a) {
+          const DenseAgg& ag = dp.agg[a];
+          if (ag.nn_word >= 0) {
+            if (o[ag.nn_word] == 0ull) continue;
+            w[ag.nn_word] += o[ag.nn_word];
+          }
+          const bool wide = ag.op == DO_ADD_128 || ag.op == DO_MIN_128 || ag.op == DO_MAX_128;
+          if (ag.op != DO_NONE) dense_apply(ag.op, w + ag.word, o[ag.word], wide ? o[ag.word + 1] : 0ull);
+        }
+      }
+      if (w[0] == 0ull) continue;
+      unsigned long long* g = dp.acc + (size_t)s * dp.n_words;
+      atomicAdd(g, w[0]);
+#pragma unroll 1
+      for (int a = 0; a < dp.n_aggs; ++a) {
+        const DenseAgg& ag = dp.agg[a];
+        if (ag.nn_word >= 0) {
+          if (w[ag.nn_word] == 0ull) continue;   // no value: the slot's word still holds the identity
+          atomicAdd(g + ag.nn_word, w[ag.nn_word]);
+        }
+        if (ag.op == DO_NONE) continue;
+        const bool wide = ag.op == DO_ADD_128 || ag.op == DO_MIN_128 || ag.op == DO_MAX_128;
+        dense_update(ag.op, g + ag.word, w[ag.word], wide ? w[ag.word + 1] : 0ull);
+      }
     }
   }
   // block-level counter reduction: one atomic per block and counter
@@ -995,8 +1269,14 @@ __global__ void __launch_bounds__(256) lookup_groups_kernel(LookupDev t, int row
     if (lane == 0) words[w] = b;
   }
 }
-struct EmitCol { int kind /* 0 key, 1 payload field, 2 accumulator word, 3 AVG value, 4 count as u64, 5 Decimal128 sum (two words) */, width, shift, word, nn_word, cnt_word, f64; void* dst; uint32_t* valid; };
-struct EmitCols { int n; EmitCol c[kMaxPipeCols]; };
+struct EmitCol {
+  int kind /* 0 key, 1 payload field, 2 accumulator word, 3 AVG value, 4 count as u64, 5 Decimal128 sum / min / max (two words),
+              6 dense group key decoded from the slot number, 7 Decimal128 AVG value */, width, shift, word, nn_word, cnt_word, f64;
+  void* dst; uint32_t* valid;
+  long long kmin; int kstride, kradix;   // kind 6: key = kmin + (slot / kstride) % kradix, NULL when that index is kradix - 1
+  int avg_mul, avg_prec;                  // kind 7: sum * 10^avg_mul / count must fit Decimal128(avg_prec, _)
+};
+struct EmitCols { int n; EmitCol c[kMaxPipeCols]; unsigned long long* err /* kind 7: set to 1 on overflow */; };
 __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uint32_t* __restrict__ slots, int64_t n, int rows_word, EmitCols ec) {
   const int lane = threadIdx.x & 31;
   const int64_t nw = (n + 31) / 32;
@@ -1019,6 +1299,27 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
             ((unsigned long long*)e.dst)[2 * i] = ok ? r[e.word] : 0ull;
             ((unsigned long long*)e.dst)[2 * i + 1] = ok ? r[e.word + 1] : 0ull;
             break;
+          case 6: {
+            const uint64_t q = ((uint64_t)slots[i] / (uint64_t)e.kstride) % (uint64_t)e.kradix;
+            ok = q + 1 != (uint64_t)e.kradix;
+            v = (uint64_t)e.kmin + q;
+            break;
+          }
+          case 7: {   // DecimalAverager::avg: sum.mul_checked(10^(ts - s)) / count (truncated), validated against the target precision
+            const unsigned long long cnt = r[e.cnt_word];
+            ok = cnt != 0ull;
+            i128 q = 0;
+            if (ok) {
+              const i128 sum = (i128)(((u128)r[e.word + 1] << 64) | (u128)r[e.word]);
+              i128 m;
+              const bool bad = mul_ovf128(sum, pow10_i128(e.avg_mul), &m);
+              if (!bad) q = m / (i128)cnt;
+              if (bad || !dec_fits(q, e.avg_prec)) { atomicOr(ec.err, 1ull); q = 0; }
+            }
+            ((unsigned long long*)e.dst)[2 * i] = (unsigned long long)(u128)q;
+            ((unsigned long long*)e.dst)[2 * i + 1] = (unsigned long long)((u128)q >> 64);
+            break;
+          }
           default: {   // AVG = sum / count over Float64 (functions-aggregate/src/average.rs)
             const unsigned long long cnt = r[e.cnt_word];
             ok = cnt != 0ull;
@@ -1027,7 +1328,7 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
           }
         }
         if (!ok) v = 0;
-        if (e.kind != 5) switch (e.width) {
+        if (e.kind != 5 && e.kind != 7) switch (e.width) {
           case 1: ((uint8_t*)e.dst)[i] = (uint8_t)v; break;
           case 2: ((uint16_t*)e.dst)[i] = (uint16_t)v; break;
           case 4: ((uint32_t*)e.dst)[i] = (uint32_t)v; break;
@@ -1131,6 +1432,9 @@ struct dfgpu_pipeline {
   dfgpu_lookup* target = nullptr; int bkey_col = -1; std::vector<int> bpay_cols;
   // aggregate sink
   std::vector<int> group_cols; std::vector<PipeAgg> aggs; int agg_mode = DFGPU_AGG_SINGLE, agg_stage = -1, rows_word = -1; bool acc_ready = false;
+  // dense-group aggregate sink (group_cols, aggs and agg_mode as above; the aggregates' words address a slot of dense_acc)
+  std::vector<DenseKey> dense_keys; std::vector<int> dense_radix; std::vector<unsigned long long> dense_ident;
+  int dense_slots = 0, dense_words = 0; DevBuf dense_acc;
   // output sink
   std::vector<int> out_cols; bool out_ordered = true;
   std::vector<std::vector<DCol>> out_parts; int64_t out_rows_pending = 0;
@@ -1287,6 +1591,27 @@ static void fill_ring(PipeParams* pp, int ring_bytes_budget) {
   for (size_t k = 0; k < ring.size(); ++k) pp->ring_col[k] = ring[k];
 }
 
+// the predicate as a conjunction of at most max_terms `column <cmp> literal` terms over integer-class columns: {col, op, uns, lit} each
+static bool conjunction_terms(const dfgpu_pipeline* p, int max_terms, std::vector<std::array<long long, 4>>* terms) {
+  const auto& nd = p->pred.nodes;
+  terms->clear();
+  bool fast = true;
+  size_t i = 0;
+  int depth = 0;
+  while (i < nd.size() && fast) {
+    if (i + 2 < nd.size() && nd[i].kind == DFGPU_EXPR_COLUMN && nd[i + 1].kind == DFGPU_EXPR_LITERAL && nd[i + 2].kind == DFGPU_EXPR_BINARY &&
+        nd[i + 2].a >= DFGPU_OP_EQ && nd[i + 2].a <= DFGPU_OP_GTEQ && !nd[i + 1].is_null) {
+      const int ct = p->in_types[nd[i].a];
+      const int cls = cls_of(ct);
+      if ((cls != C_I64 && cls != C_U64) || p->pred.has_decimal || (int)terms->size() >= max_terms) { fast = false; break; }
+      terms->push_back({(long long)nd[i].a, (long long)nd[i + 2].a, (long long)(cls == C_U64), (long long)literal_bits(nd[i + 1])});
+      depth++; i += 3;
+    } else if (nd[i].kind == DFGPU_EXPR_BINARY && nd[i].a == DFGPU_OP_AND && depth >= 2) { depth--; i++; }
+    else fast = false;
+  }
+  return fast && depth == 1 && !terms->empty();
+}
+
 static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipeParams* pp) {
   memset(pp, 0, sizeof(*pp));
   pp->n_cols = (int)cols.size();
@@ -1297,23 +1622,8 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
   pp->pred_mode = 0;
   if (p->has_pred) {
     // fast path: conjunction of `column <cmp> literal` terms over integer-class columns
-    const auto& nd = p->pred.nodes;
     std::vector<std::array<long long, 4>> terms;  // col, op, uns, lit
-    bool fast = true;
-    size_t i = 0;
-    int depth = 0;
-    while (i < nd.size() && fast) {
-      if (i + 2 < nd.size() && nd[i].kind == DFGPU_EXPR_COLUMN && nd[i + 1].kind == DFGPU_EXPR_LITERAL && nd[i + 2].kind == DFGPU_EXPR_BINARY &&
-          nd[i + 2].a >= DFGPU_OP_EQ && nd[i + 2].a <= DFGPU_OP_GTEQ && !nd[i + 1].is_null) {
-        const int ct = p->in_types[nd[i].a];
-        const int cls = cls_of(ct);
-        if ((cls != C_I64 && cls != C_U64) || p->pred.has_decimal || (int)terms.size() >= kMaxTerms) { fast = false; break; }
-        terms.push_back({(long long)nd[i].a, (long long)nd[i + 2].a, (long long)(cls == C_U64), (long long)literal_bits(nd[i + 1])});
-        depth++; i += 3;
-      } else if (nd[i].kind == DFGPU_EXPR_BINARY && nd[i].a == DFGPU_OP_AND && depth >= 2) { depth--; i++; }
-      else fast = false;
-    }
-    if (fast && depth == 1 && !terms.empty()) {
+    if (conjunction_terms(p, kMaxTerms, &terms)) {
       pp->pred_mode = 1; pp->n_terms = (int)terms.size();
       for (size_t t = 0; t < terms.size(); ++t) { pp->term_col[t] = (int)terms[t][0]; pp->term_op[t] = (int)terms[t][1]; pp->term_uns[t] = (int)terms[t][2]; pp->term_lit[t] = terms[t][3]; }
     } else {
@@ -1453,6 +1763,90 @@ static void prepare_acc(dfgpu_pipeline* p) {
   p->acc_ready = true;
 }
 
+// ---- dense-group aggregate sink ----
+static int dense_op(const PipeAgg& ag) {
+  const bool wide = ag.cls == C_DEC, f = ag.cls == C_F64, u = ag.cls == C_U64;
+  switch (ag.func) {
+    case DFGPU_AGG_SUM: case DFGPU_AGG_AVG: return wide ? DO_ADD_128 : (f ? DO_ADD_F64 : DO_ADD_U64);
+    case DFGPU_AGG_MIN: return wide ? DO_MIN_128 : (f ? DO_MIN_F64 : (u ? DO_MIN_U64 : DO_MIN_S64));
+    case DFGPU_AGG_MAX: return wide ? DO_MAX_128 : (f ? DO_MAX_F64 : (u ? DO_MAX_U64 : DO_MAX_S64));
+    default: return DO_NONE;
+  }
+}
+
+// small domains keep one copy of the slots per warp: no atomics in the row loop, the warps of a block are folded at the flush
+static bool dense_per_warp(const dfgpu_pipeline* p) { return (size_t)kPipeWarps * p->dense_slots * p->dense_words * 8 <= (size_t)kDenseWarpBytes; }
+
+static void prepare_dense(dfgpu_pipeline* p) {
+  if (p->dense_acc.ptr) return;
+  const size_t words = (size_t)p->dense_slots * p->dense_words;
+  std::vector<unsigned long long> init(words);
+  for (size_t i = 0; i < words; ++i) init[i] = p->dense_ident[i % p->dense_words];
+  p->dense_acc.alloc(p->ctx, words * 8);
+  DF_CUDA(cudaMemcpyAsync(p->dense_acc.ptr, init.data(), words * 8, cudaMemcpyHostToDevice, p->ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(p->ctx->stream));   // `init` lives on this stack frame
+}
+
+// the dense sink's parameters for one batch: its aggregate programs are bound behind the predicate in pp's pool
+static void fill_dense(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipeParams* pp, DenseParams* dp) {
+  memset(dp, 0, sizeof(*dp));
+  std::vector<std::array<long long, 4>> terms;
+  if (pp->pred_mode == 2 && conjunction_terms(p, kMaxTerms + kDenseMaxXTerms, &terms)) {   // a longer conjunction: the rest in DenseParams
+    pp->pred_mode = 1; pp->n_terms = kMaxTerms; pp->pred_start = 0; pp->pred_n = 0;
+    for (size_t t = 0; t < terms.size(); ++t) {
+      const int k = (int)t - kMaxTerms;
+      if (k < 0) { pp->term_col[t] = (int)terms[t][0]; pp->term_op[t] = (int)terms[t][1]; pp->term_uns[t] = (int)terms[t][2]; pp->term_lit[t] = terms[t][3]; }
+      else { dp->xterm_col[k] = (int)terms[t][0]; dp->xterm_op[k] = (int)terms[t][1]; dp->xterm_uns[k] = (int)terms[t][2]; dp->xterm_lit[k] = terms[t][3]; }
+    }
+    dp->n_xterms = (int)terms.size() - kMaxTerms;
+  }
+  dp->per_warp = dense_per_warp(p) ? 1 : 0;
+  int pool_used = pp->pred_mode == 2 ? pp->pred_start + pp->pred_n : 0;
+  dp->n_keys = (int)p->dense_keys.size(); dp->n_aggs = (int)p->aggs.size(); dp->n_slots = p->dense_slots; dp->n_words = p->dense_words;
+  for (size_t k = 0; k < p->dense_keys.size(); ++k) dp->key[k] = p->dense_keys[k];
+  for (int w = 0; w < p->dense_words; ++w) dp->ident[w] = p->dense_ident[w];
+  dp->acc = p->dense_acc.as<unsigned long long>();
+  for (size_t a = 0; a < p->aggs.size(); ++a) {
+    const PipeAgg& ag = p->aggs[a];
+    DenseAgg& d = dp->agg[a];
+    d.func = ag.func; d.op = dense_op(ag);
+    d.word = ag.func == DFGPU_AGG_COUNT ? -1 : ag.word;   // COUNT(x) is its non-null counter
+    d.nn_word = ag.func == DFGPU_AGG_COUNT ? ag.word : ag.nn_word;
+    if (ag.has_expr) {
+      d.start = bind_pool(p, ag.plan, cols, pp, &pool_used); d.n = (int)ag.plan.nodes.size();
+      d.small = plan_depth(ag.plan) <= 4 ? 1 : 0;
+      if (d.small && plan_is_int_arith(p, ag.plan, cols)) d.small = 2;
+      if (ag.plan.has_decimal) d.small = 3;
+    }
+  }
+}
+
+static bool pipeline_has_decimal(const dfgpu_pipeline* p) {
+  bool dec = p->has_pred && p->pred.has_decimal;
+  for (const auto& ag : p->aggs) dec = dec || (ag.has_expr && ag.plan.has_decimal);
+  return dec;
+}
+
+static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DenseParams& dp, int64_t n) {
+  dfgpu_ctx* ctx = p->ctx;
+  if (!p->params_dev.ptr) p->params_dev.alloc(ctx, kDenseParamsOff + sizeof(DenseParams));
+  DF_CUDA(cudaMemcpyAsync(p->params_dev.ptr, &pp, sizeof(PipeParams), cudaMemcpyHostToDevice, ctx->stream));
+  DF_CUDA(cudaMemcpyAsync((char*)p->params_dev.ptr + kDenseParamsOff, &dp, sizeof(DenseParams), cudaMemcpyHostToDevice, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));   // `pp` and `dp` live on the caller's stack frame
+  // programs that touch Decimal128 values run the instantiation with the 128-bit interpreter
+  void (*kern)(const PipeParams*, int64_t, unsigned long long*) = pipeline_has_decimal(p) ? pipe_kernel<SINK_DENSE, true> : pipe_kernel<SINK_DENSE, false>;
+  const int smem = kDenseAccOff + (dp.per_warp ? kPipeWarps : 1) * p->dense_slots * p->dense_words * 8;
+  DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));   // per device: set on every launch
+  int blocks_per_sm = 0;
+  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, smem));
+  const int64_t ntiles = (n + kPipeTile - 1) / kPipeTile;
+  const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
+  const std::string tname = p->name.empty() ? std::string("pipeline_dense") : "pipe:" + p->name;
+  KernelTimer kt(ctx, tname.c_str());
+  kern<<<grid, kPipeThreads, smem, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, p->counters.as<unsigned long long>());
+  DF_LAUNCH_CHECK(ctx);
+}
+
 static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   DF_CHECK(!p->finished, DFGPU_ERR_STATE, "push after finish");
   DF_CHECK(p->sink != SINK_NONE, DFGPU_ERR_STATE, "pipeline: choose a sink before the first push");
@@ -1519,6 +1913,17 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     launch_pipe<SINK_AGG>(p, pp, n, "pipeline_agg");
     read_counters(p, h);
     check_errors(h[3]);
+    p->m_sink_rows += (int64_t)h[0];
+  } else if (p->sink == SINK_DENSE) {
+    prepare_dense(p);
+    fill_params(p, cols, &pp);
+    DenseParams dp;
+    fill_dense(p, cols, &pp, &dp);
+    p->counters.zero();
+    launch_dense(p, pp, dp, n);
+    read_counters(p, h);
+    check_errors(h[3]);
+    if (h[2] & 2) throw Error(DFGPU_ERR_INVALID, "pipeline dense aggregate: a group key lies outside its declared range");
     p->m_sink_rows += (int64_t)h[0];
   } else if (!p->out_ordered) {   // SINK_OUTPUT, row order unspecified: the two-phase kernel, one global reservation per 128 survivors
     DF_CHECK(n < 0xFFFFFFFFll, DFGPU_ERR_UNSUPPORTED, "pipeline: a batch must have < 2^32-1 rows");
@@ -1600,6 +2005,41 @@ static void emit_sliced(dfgpu_pipeline* p, std::vector<DCol>& merged, int64_t ro
   }
 }
 
+// one column (Single) or the state columns (Partial) per aggregate, read from the accumulator words the aggregate addresses
+template <class Add>
+static void add_agg_columns(const std::vector<PipeAgg>& aggs, int rows_word, bool partial, Add& add) {
+  for (const PipeAgg& ag : aggs) {
+    EmitCol e; memset(&e, 0, sizeof(e));
+    e.nn_word = -1;
+    const int sum_type = ag.cls == C_F64 ? DFGPU_FLOAT64 : (ag.cls == C_U64 ? DFGPU_UINT64 : DFGPU_INT64);   // sum.rs:232-261
+    switch (ag.func) {
+      case DFGPU_AGG_COUNT_STAR: e.kind = 4; e.word = rows_word; add(DFGPU_INT64, false, e); break;
+      case DFGPU_AGG_COUNT: e.kind = 4; e.word = ag.word; add(DFGPU_INT64, false, e); break;
+      case DFGPU_AGG_SUM:
+        if (ag.cls == C_DEC) {   // Sum::return_type: Decimal128(min(38, p + 10), s) (sum.rs:247-249); the Partial state has the same type
+          e.kind = 5; e.word = ag.word; e.nn_word = ag.nn_word;
+          add(dec_type(std::min(38, dec_precision(ag.arg_type) + 10), dec_scale(ag.arg_type)), ag.nn_word >= 0, e);
+        } else { e.kind = 2; e.word = ag.word; e.nn_word = ag.nn_word; add(sum_type, ag.nn_word >= 0, e); }
+        break;
+      case DFGPU_AGG_MIN: case DFGPU_AGG_MAX:   // the argument's type; Decimal128 takes two words
+        e.kind = ag.cls == C_DEC ? 5 : 2; e.word = ag.word; e.nn_word = ag.nn_word; add(ag.arg_type, ag.nn_word >= 0, e);
+        break;
+      case DFGPU_AGG_AVG:
+        if (ag.cls == C_DEC) {   // Avg::return_type: Decimal128(min(38, p + 4), min(38, s + 4)) (average.rs); Single modes only
+          const int tp = std::min(38, dec_precision(ag.arg_type) + 4), ts = std::min(38, dec_scale(ag.arg_type) + 4);
+          e.kind = 7; e.word = ag.word; e.cnt_word = ag.cnt_word; e.avg_mul = ts - dec_scale(ag.arg_type); e.avg_prec = tp;
+          add(dec_type(tp, ts), true, e);
+        } else if (partial) {   // state = [count: UInt64, sum: Float64] (aggregates/mod.rs:3591-3700)
+          EmitCol c1 = e; c1.kind = 4; c1.word = ag.cnt_word; add(DFGPU_UINT64, false, c1);
+          EmitCol c2 = e; c2.kind = 2; c2.word = ag.word; c2.nn_word = ag.cnt_word; add(DFGPU_FLOAT64, true, c2);
+        } else { e.kind = 3; e.word = ag.word; e.cnt_word = ag.cnt_word; add(DFGPU_FLOAT64, true, e); }
+        break;
+    }
+  }
+}
+
+static void dense_finish(dfgpu_pipeline* p);
+
 static void pipeline_finish(dfgpu_pipeline* p) {
   DF_CHECK(!p->finished, DFGPU_ERR_STATE, "finish called twice");
   p->finished = true;
@@ -1617,6 +2057,7 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     emit_sliced(p, merged, p->out_rows_pending);
     return;
   }
+  if (p->sink == SINK_DENSE) { dense_finish(p); return; }
   if (p->sink != SINK_AGG) return;
   dfgpu_lookup* l = p->stages[p->agg_stage].lookup;
   if (l->cap == 0) return;
@@ -1647,30 +2088,59 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     if (g == key_col) { e.kind = 0; add(p->in_types[g], false, e); }
     else { const ExtDef& x = p->exts[g - (int)p->in_types.size()]; e.kind = 1; e.shift = x.shift; add(x.type, false, e); }
   }
-  for (const PipeAgg& ag : p->aggs) {
-    EmitCol e; memset(&e, 0, sizeof(e));
-    e.nn_word = -1;
-    const int sum_type = ag.cls == C_F64 ? DFGPU_FLOAT64 : (ag.cls == C_U64 ? DFGPU_UINT64 : DFGPU_INT64);   // sum.rs:232-261
-    switch (ag.func) {
-      case DFGPU_AGG_COUNT_STAR: e.kind = 4; e.word = p->rows_word; add(DFGPU_INT64, false, e); break;
-      case DFGPU_AGG_COUNT: e.kind = 4; e.word = ag.word; add(DFGPU_INT64, false, e); break;
-      case DFGPU_AGG_SUM:
-        if (ag.cls == C_DEC) {   // Sum::return_type: Decimal128(min(38, p + 10), s) (sum.rs:247-249); the Partial state has the same type
-          e.kind = 5; e.word = ag.word; e.nn_word = ag.nn_word;
-          add(dec_type(std::min(38, dec_precision(ag.arg_type) + 10), dec_scale(ag.arg_type)), ag.nn_word >= 0, e);
-        } else { e.kind = 2; e.word = ag.word; e.nn_word = ag.nn_word; add(sum_type, ag.nn_word >= 0, e); }
-        break;
-      case DFGPU_AGG_MIN: case DFGPU_AGG_MAX: e.kind = 2; e.word = ag.word; e.nn_word = ag.nn_word; add(ag.arg_type, ag.nn_word >= 0, e); break;
-      case DFGPU_AGG_AVG:
-        if (partial) {   // state = [count: UInt64, sum: Float64] (aggregates/mod.rs:3591-3700)
-          EmitCol c1 = e; c1.kind = 4; c1.word = ag.cnt_word; add(DFGPU_UINT64, false, c1);
-          EmitCol c2 = e; c2.kind = 2; c2.word = ag.word; c2.nn_word = ag.cnt_word; add(DFGPU_FLOAT64, true, c2);
-        } else { e.kind = 3; e.word = ag.word; e.cnt_word = ag.cnt_word; add(DFGPU_FLOAT64, true, e); }
-        break;
-    }
-  }
+  add_agg_columns(p->aggs, p->rows_word, partial, add);
   lookup_emit_kernel<<<grid_for(groups, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), groups, p->rows_word, ec);
   DF_LAUNCH_CHECK(ctx);
+  emit_sliced(p, out, groups);
+}
+
+// the dense sink's output: one row per slot that received a row (exactly one row without GROUP BY, also for empty input), in slot
+// order = ascending key order with NULL after the values of its column
+static void dense_finish(dfgpu_pipeline* p) {
+  dfgpu_ctx* ctx = p->ctx;
+  prepare_dense(p);
+  LookupDev t;
+  memset(&t, 0, sizeof(t));
+  t.recs = p->dense_acc.as<unsigned long long>(); t.cap = (uint64_t)p->dense_slots; t.stride = p->dense_words;
+  DevBuf idx, err(ctx, 8);
+  err.zero();
+  int64_t groups = 1;
+  if (p->dense_keys.empty()) {   // AggregateStream: the single slot
+    idx.alloc(ctx, 8);
+    idx.zero();
+  } else {
+    const uint64_t nw = (t.cap + 31) / 32;
+    DevBuf words(ctx, (size_t)nw * 4 + 8);
+    lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, 0, words.as<uint32_t>());
+    DF_LAUNCH_CHECK(ctx);
+    groups = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)t.cap, 1, &idx);
+  }
+  p->m_groups = groups;
+  if (groups == 0) return;
+  EmitCols ec;
+  memset(&ec, 0, sizeof(ec));
+  ec.err = err.as<unsigned long long>();
+  std::vector<DCol> out;
+  auto add = [&](int type, bool nullable, EmitCol e) {
+    DF_CHECK(ec.n < kMaxPipeCols, DFGPU_ERR_UNSUPPORTED, "pipeline: too many output columns");
+    DCol d = alloc_col(ctx, type, groups, nullable);
+    e.width = type_width(type); e.dst = d.own_values->ptr; e.valid = nullable ? d.own_validity->as<uint32_t>() : nullptr;
+    d.null_count = nullable ? -1 : 0;
+    ec.c[ec.n++] = e;
+    out.push_back(std::move(d));
+  };
+  for (size_t k = 0; k < p->dense_keys.size(); ++k) {
+    EmitCol e; memset(&e, 0, sizeof(e));
+    e.kind = 6; e.kmin = (long long)p->dense_keys[k].kmin; e.kstride = (int)p->dense_keys[k].stride; e.kradix = p->dense_radix[k];
+    add(p->vtypes[p->group_cols[k]], true, e);
+  }
+  add_agg_columns(p->aggs, 0, p->agg_mode == DFGPU_AGG_PARTIAL, add);
+  lookup_emit_kernel<<<grid_for(groups, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), groups, 0, ec);
+  DF_LAUNCH_CHECK(ctx);
+  unsigned long long h_err = 0;
+  DF_CUDA(cudaMemcpyAsync(&h_err, err.ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (h_err) throw Error(DFGPU_ERR_ARITH, "Arithmetic Overflow in AvgAccumulator");
   emit_sliced(p, out, groups);
 }
 
@@ -1945,6 +2415,90 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   p->aggs = std::move(new_aggs);
   l->acc_claimed = true;
   p->agg_stage = stage; p->agg_mode = mode; p->batch_size = batch_size; p->sink = SINK_AGG;
+  DF_API_END
+}
+
+int dfgpu_pipeline_sink_aggregate_dense(dfgpu_pipeline* p, const int32_t* group_cols, const int64_t* key_min, const int64_t* key_max, int32_t n_group,
+                                        const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size) {
+  DF_API_BEGIN(p ? p->ctx : nullptr)
+  DF_CHECK(p && n_group >= 0 && (n_group == 0 || (group_cols && key_min && key_max)), DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  DF_CHECK(n_group <= kDenseMaxKeys, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: 0..8 group columns");
+  DF_CHECK(n_aggs >= 0 && n_aggs <= kDenseMaxAggs && (n_aggs == 0 || aggs), DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: 0..8 aggregates");
+  DF_CHECK(mode == DFGPU_AGG_SINGLE || mode == DFGPU_AGG_SINGLE_PARTITIONED || mode == DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Single / SinglePartitioned / Partial");
+  for (auto& st : p->stages) DF_CHECK(st.kind != DFGPU_STAGE_MAYBE, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: a MAYBE stage's false positives would be counted");
+  // group keys: slot = sum_g stride_g * idx_g, row-major over radix_g = max - min + 2 (the values, then NULL)
+  std::vector<DenseKey> keys(n_group);
+  std::vector<int> radix(n_group);
+  uint64_t slots = 1;
+  for (int g = 0; g < n_group; ++g) {
+    const int c = group_cols[g];
+    DF_CHECK(c >= 0 && c < (int)p->vtypes.size(), DFGPU_ERR_INVALID, "pipeline dense aggregate: group column out of range");
+    const int t = p->vtypes[c];
+    DF_CHECK(key_type_ok(t), DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: group keys must be integer-like columns of <= 64 bits");
+    const bool uns = type_is_unsigned_int(t);
+    DF_CHECK(uns ? (uint64_t)key_min[g] <= (uint64_t)key_max[g] : key_min[g] <= key_max[g], DFGPU_ERR_INVALID, "pipeline dense aggregate: key_min > key_max");
+    const uint64_t span = (uint64_t)key_max[g] - (uint64_t)key_min[g];
+    DF_CHECK(span < (uint64_t)kDenseMaxSlots, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: more than 256 groups (DFGPU_DENSE_MAX_GROUPS)");
+    radix[g] = (int)span + 2;
+    slots *= (uint64_t)radix[g];
+    DF_CHECK(slots <= (uint64_t)kDenseMaxSlots, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: more than 256 groups (DFGPU_DENSE_MAX_GROUPS)");
+    memset(&keys[g], 0, sizeof(DenseKey));
+    keys[g].src = c; keys[g].kmin = (unsigned long long)key_min[g]; keys[g].nvals = span + 1;
+  }
+  uint64_t stride = 1;
+  for (int g = n_group - 1; g >= 0; --g) { keys[g].stride = stride; stride *= (uint64_t)radix[g]; }
+  // accumulator words of a slot: word 0 counts the rows; every SUM / MIN / MAX / AVG has its own non-null counter
+  std::vector<unsigned long long> ident(1, 0ull);
+  auto take = [&](int nw, unsigned long long lo, unsigned long long hi) {
+    if (nw == 2 && (ident.size() & 1)) ident.push_back(0ull);   // 128-bit fields 16-byte aligned
+    const int w = (int)ident.size();
+    ident.push_back(lo);
+    if (nw == 2) ident.push_back(hi);
+    return w;
+  };
+  std::vector<PipeAgg> new_aggs;
+  for (int a = 0; a < n_aggs; ++a) {
+    PipeAgg ag;
+    ag.func = aggs[a].func;
+    DF_CHECK(ag.func >= DFGPU_AGG_SUM && ag.func <= DFGPU_AGG_COUNT_STAR, DFGPU_ERR_INVALID, "pipeline aggregate: unknown function");
+    if (ag.func != DFGPU_AGG_COUNT_STAR) {
+      DF_CHECK(aggs[a].expr && aggs[a].n_nodes > 0, DFGPU_ERR_INVALID, "pipeline aggregate: missing argument expression");
+      ag.plan = plan_expr(p->vtypes.data(), (int)p->vtypes.size(), aggs[a].expr, aggs[a].n_nodes);
+      ag.has_expr = true;
+      ag.arg_type = ag.plan.root_type;
+      ag.cls = cls_of(ag.arg_type);
+      DF_CHECK(ag.cls != C_BOOL || ag.func == DFGPU_AGG_COUNT, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Boolean arguments only for COUNT");
+      if (ag.func == DFGPU_AGG_AVG) {
+        DF_CHECK(ag.arg_type == DFGPU_FLOAT64 || ag.cls == C_DEC, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: AVG takes a Float64 (the planner casts) or Decimal128 argument");
+        DF_CHECK(ag.cls != C_DEC || mode != DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: AVG over Decimal128 runs in Single modes only");
+      }
+      if (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) DF_CHECK(ag.arg_type != DFGPU_FLOAT32, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: MIN/MAX over Float32 stays on dfgpu_agg");
+      const int nw = ag.cls == C_DEC ? 2 : 1;
+      const bool is_min = ag.func == DFGPU_AGG_MIN;
+      unsigned long long lo = 0, hi = 0;   // MIN / MAX identities
+      if (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) {
+        if (ag.cls == C_DEC) { lo = is_min ? ~0ull : 0ull; hi = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN; }
+        else if (ag.cls == C_F64) { const double d = is_min ? INFINITY : -INFINITY; memcpy(&lo, &d, 8); }
+        else if (ag.cls == C_U64) lo = is_min ? ~0ull : 0ull;
+        else lo = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN;
+      }
+      if (ag.func == DFGPU_AGG_COUNT) ag.word = take(1, 0, 0);
+      else {
+        ag.word = take(nw, lo, hi);
+        ag.nn_word = take(1, 0, 0);
+        if (ag.func == DFGPU_AGG_AVG) ag.cnt_word = ag.nn_word;
+      }
+    }
+    new_aggs.push_back(std::move(ag));
+  }
+  if (ident.size() & 1) ident.push_back(0ull);
+  DF_CHECK((int)ident.size() <= kDenseMaxWords, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: too many accumulator words");
+  p->dense_keys = std::move(keys); p->dense_radix = std::move(radix); p->dense_ident = std::move(ident);
+  p->dense_slots = (int)slots; p->dense_words = (int)p->dense_ident.size();
+  p->group_cols.assign(group_cols, group_cols + n_group);
+  p->aggs = std::move(new_aggs);
+  p->agg_mode = mode; p->batch_size = batch_size; p->sink = SINK_DENSE;
   DF_API_END
 }
 

@@ -531,7 +531,9 @@ class AggregateExpr:
     def value_type(self, t: Optional[pa.DataType]) -> pa.DataType:
         if self.func in ("count", "count_star"):
             return pa.int64()
-        if self.func == "avg":
+        if self.func == "avg":  # Avg::return_type (functions-aggregate average.rs): Decimal128(min(38, p + 4), min(38, s + 4))
+            if pa.types.is_decimal128(t):
+                return pa.decimal128(min(38, t.precision + 4), min(38, t.scale + 4))
             return pa.float64()
         if self.func == "sum":  # Sum::return_type, functions-aggregate/src/sum.rs:232-261
             if pa.types.is_decimal128(t):
@@ -672,8 +674,10 @@ class GpuPipelineExec(ExecutionPlan):
     """One fused pipeline (dfgpu_pipeline): source -> predicate -> probe stages -> {build | aggregate | output}.  Built by fuse_pipelines()."""
 
     def __init__(self, scan: _Scan, sink: str, key: Optional[str] = None, payload: Sequence[str] = (), group_by: Sequence[str] = (),
-                 aggs: Sequence[Tuple[str, Optional[Expr], str]] = (), mode: str = "Single", out_schema: Optional[pa.Schema] = None):
+                 aggs: Sequence[Tuple[str, Optional[Expr], str]] = (), mode: str = "Single", out_schema: Optional[pa.Schema] = None,
+                 key_range: Sequence[Tuple[int, int]] = ()):
         self.scan, self.sink, self.key, self.payload, self.group_by, self.aggs, self.mode = scan, sink, key, list(payload), list(group_by), list(aggs), mode
+        self.key_range = list(key_range)   # dense sink: the declared (min, max) of every group column
         self.schema = out_schema if out_schema is not None else pa.schema([])
         self.n_acc_words = 0
         self._metrics = {}
@@ -722,19 +726,23 @@ class GpuPipelineExec(ExecutionPlan):
         return D.Pipeline(ctx.gpu, [type_id(f.type) for f in ssch], nodes, stages), keep
 
     def execute(self, ctx):
-        assert self.sink == "aggregate", "build pipelines are driven by their consumer"
+        assert self.sink in ("aggregate", "dense"), "build pipelines are driven by their consumer"
         vs = self.scan.virtual_schema()
         pipe, keep = self._make_pipeline(ctx)
         try:
             aggs = []
             for func, expr, _ in self.aggs:
                 if expr is None:
-                    aggs.append((_AGG_FUNCS[func], None))
+                    aggs.append((D.AGG_COUNT_STAR if self.sink == "dense" else _AGG_FUNCS[func], None))
                 else:
                     nodes: list = []
                     expr.rpn(vs, nodes)
                     aggs.append((_AGG_FUNCS[func], nodes))
-            pipe.sink_aggregate([vs.get_field_index(g) for g in self.group_by], aggs, _AGG_MODES[self.mode], 0)
+            gcols = [vs.get_field_index(g) for g in self.group_by]
+            if self.sink == "dense":
+                pipe.sink_aggregate_dense(gcols, self.key_range, aggs, _AGG_MODES[self.mode], 0)
+            else:
+                pipe.sink_aggregate(gcols, aggs, _AGG_MODES[self.mode], 0)
             for rb in self.scan.source.execute(ctx):
                 pipe.push_arrow(rb)
             pipe.finish()
@@ -749,11 +757,90 @@ class GpuPipelineExec(ExecutionPlan):
                 l.close()
 
 
+def _source_bounds(source: ExecutionPlan, name: str) -> Optional[Tuple[int, int]]:
+    """(min, max) of an integer-like source column, when known at planning time.  The twin reads a MemoryExec's batches; DataFusion
+    has them as ColumnStatistics::{min_value, max_value} of partition_statistics.  None when unknown (or no non-NULL value)."""
+    if not isinstance(source, MemoryExec):
+        return None
+    t = source.schema.field(name).type
+    if not (pa.types.is_integer(t) or pa.types.is_date32(t)):
+        return None
+    import pyarrow.compute as pc
+    i = source.schema.get_field_index(name)
+    lo = hi = None
+    for b in source.batches:
+        c = b.column(i)
+        if c.null_count == len(c):
+            continue
+        mm = pc.min_max(c.cast(pa.int64()) if pa.types.is_date32(t) else c)
+        lo = mm["min"].as_py() if lo is None else min(lo, mm["min"].as_py())
+        hi = mm["max"].as_py() if hi is None else max(hi, mm["max"].as_py())
+    if lo is None or hi > (1 << 63) - 1:
+        return None
+    return lo, hi
+
+
+def _fuse_dense(plan: "GpuAggregateExec") -> Optional["GpuPipelineExec"]:
+    """AggregateExec over [ProjectionExec] over FilterExec over a source (no join) whose GROUP BY columns are source columns with known
+    bounds spanning at most DENSE_MAX_GROUPS slots (NULL included) -> a GpuPipelineExec with the dense sink; None otherwise"""
+    below, proj = plan.input, None
+    if isinstance(below, GpuProjectionExec):
+        proj, below = below, below.input
+    if not isinstance(below, GpuFilterExec):
+        return None
+    sc = _as_scan(below)
+    if sc is None or sc.stages:
+        return None
+    src = sc.source.schema
+    exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
+    group, ranges, slots = [], [], 1
+    for g in plan.group_by:
+        e = exprs.get(g)
+        if not isinstance(e, Column) or e.name not in sc.visible or src.get_field_index(e.name) < 0:
+            return None
+        b = _source_bounds(sc.source, e.name)
+        if b is None:
+            return None
+        slots *= b[1] - b[0] + 2
+        if slots > D.DENSE_MAX_GROUPS:
+            return None
+        group.append(e.name)
+        ranges.append(b)
+    if len(plan.aggr_expr) > 8:
+        return None
+    aggs = []
+    for a in plan.aggr_expr:
+        if a.filter is not None:
+            return None
+        e = None if a.arg is None else exprs.get(a.arg)
+        if a.arg is not None and e is None:
+            return None
+        if e is not None:
+            try:
+                e.rpn(src, [])                             # every referenced name must be a source column
+                t = e.data_type(src)
+            except KeyError:
+                return None
+            if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
+                return None                                # AVG(Decimal128) has no pinned Partial state
+            if a.func in ("min", "max") and t == pa.float32():
+                return None
+        aggs.append((a.func, e, a.alias))
+    return GpuPipelineExec(sc, sink="dense", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, key_range=ranges)
+
+
 def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a): AggregateExec(Single / SinglePartitioned / Partial) over [ProjectionExec] over
     HashJoinExec(Inner) whose GROUP BY is the probe key plus build-side columns becomes ONE GpuPipelineExec; its build side (filters, semi
-    joins, column projections) becomes build pipelines.  Anything else is returned unchanged (the unfused Gpu*Exec operators run)."""
-    if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial") or not plan.group_by:
+    joins, column projections) becomes build pipelines.  The same AggregateExec over [ProjectionExec] over FilterExec over a source, with
+    no join, becomes a GpuPipelineExec with the dense sink when its GROUP BY columns have small known bounds (_fuse_dense: TPC-H Q1, Q6).
+    Anything else is returned unchanged (the unfused Gpu*Exec operators run)."""
+    if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial"):
+        return plan
+    dense = _fuse_dense(plan)
+    if dense is not None:
+        return dense
+    if not plan.group_by:
         return plan
     below, proj = plan.input, None
     if isinstance(below, GpuProjectionExec):

@@ -464,6 +464,21 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
 int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload);
 int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, int32_t n_group,
                                   const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size);
+/* dense aggregate: AggregateExec over the surviving rows whose 0..8 group columns (virtual columns: input columns or payload
+ * fields of INNER stages, integer-like, <= 64 bits) take values in small declared domains [key_min[g], key_max[g]] (column
+ * statistics).  The group of a row is arithmetic, slot = sum_g stride_g * idx_g with idx_g = key - key_min[g] for a value and
+ * key_max[g] - key_min[g] + 1 for NULL (a group of its own), row-major strides; no hash table.  The domain may have at most
+ * DFGPU_DENSE_MAX_GROUPS slots, prod_g (key_max[g] - key_min[g] + 2), else DFGPU_ERR_UNSUPPORTED; a key outside its range at run
+ * time is DFGPU_ERR_INVALID.  n_group = 0 is AggregateStream: exactly one output row, also for empty input (COUNT 0; SUM, MIN, MAX,
+ * AVG NULL).  Output: one row per slot that received a row, in slot order (ascending keys, NULL after the values of its column).
+ * Up to 8 aggregates: COUNT(*), COUNT(x); SUM over integers (wrapping), Float64, Decimal128 (-> Decimal128(min(38, p+10), s));
+ * MIN / MAX over integers, Date32, Float64, Decimal128; AVG over Float64 and Decimal128(p, s) -> Decimal128(min(38, p+4),
+ * min(38, s+4)) = sum * 10^(ts - s) / count truncated toward zero, DFGPU_ERR_ARITH when that overflows i128 or the target
+ * precision (DataFusion's DecimalAverager::avg).  mode = DFGPU_AGG_SINGLE* or DFGPU_AGG_PARTIAL (state columns as dfgpu_agg emits
+ * them; Decimal128 AVG: Single modes only).  MAYBE stages are rejected (their false positives would be counted). */
+#define DFGPU_DENSE_MAX_GROUPS 256
+int dfgpu_pipeline_sink_aggregate_dense(dfgpu_pipeline* p, const int32_t* group_cols, const int64_t* key_min, const int64_t* key_max,
+                                        int32_t n_group, const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size);
 int dfgpu_pipeline_sink_output(dfgpu_pipeline* p, const int32_t* out_cols, int32_t n_out, int64_t batch_size);
 /* the same, row order unspecified (what a RepartitionExec consumer sees anyway, repartition/mod.rs:1320-1400): runs on the two-phase
  * kernel and is several times faster than the ordered sink on selective pipelines */
