@@ -1442,7 +1442,7 @@ struct dfgpu_pipeline {
   bool finished = false;
   DevBuf params_dev, counters;
   std::deque<BatchPtr> outq;
-  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0;
+  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0, m_dense_block_launches = 0;
   std::string name;   // optional label: the kernel-timing family becomes "pipe:<name>" (dfgpu_kernel_time)
 };
 
@@ -1845,6 +1845,7 @@ static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DensePar
   KernelTimer kt(ctx, tname.c_str());
   kern<<<grid, kPipeThreads, smem, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, p->counters.as<unsigned long long>());
   DF_LAUNCH_CHECK(ctx);
+  if (!dp.per_warp) p->m_dense_block_launches++;
 }
 
 static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
@@ -2577,6 +2578,7 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name) {
   if (s == "output_rows") return p->m_output_rows;
   if (s == "num_groups") return p->m_groups;
   if (s == "ring_launches") return p->m_ring_launches;   // launches of the ring-fed pipeline kernel
+  if (s == "dense_block_launches") return p->m_dense_block_launches;   // dense sink launches with one accumulator copy per block (shared atomics)
   return -1;
 }
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p) {

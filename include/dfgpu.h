@@ -491,7 +491,7 @@ int dfgpu_pipeline_push_device(dfgpu_pipeline* p, const dfgpu_column* cols, int3
 int dfgpu_pipeline_push_arrow(dfgpu_pipeline* p, const struct ArrowArray* batch, const struct ArrowSchema* schema);
 int dfgpu_pipeline_finish(dfgpu_pipeline* p);
 int dfgpu_pipeline_next(dfgpu_pipeline* p, int host, dfgpu_batch** out);
-int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches" */
+int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches","dense_block_launches" */
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p);
 
 /* ===================================================================================== */

@@ -49,7 +49,7 @@ def run_dense(ctx, cols, types, pred, group_cols, key_range, aggs, mode=D.AGG_SI
         cs = [gpu_col_as_py(D, b, i) for i in range(b.num_columns)]
         otypes = [t for _, t in cs]
         rows += list(zip(*[v for v, _ in cs]))
-    m = {k: p.metric(k) for k in ("num_groups", "input_rows", "sink_rows", "output_rows")}
+    m = {k: p.metric(k) for k in ("num_groups", "input_rows", "sink_rows", "output_rows", "dense_block_launches")}
     m["batches"] = len(outs)
     p.close()
     return rows, otypes, m
