@@ -19,6 +19,7 @@
 // the grow, so every row is accumulated exactly once.
 // Partial/Final use the same table: Final consumes [group cols, state cols] and merges.
 #include "batch.cuh"
+#include "expr_dec.cuh"
 #include "scan.cuh"
 
 namespace dfgpu {
@@ -148,8 +149,8 @@ struct AggDev {
   const void* in0; const uint8_t* in0_valid; int64_t in0_voff;  // BOOL in0: in0_voff doubles as value offset
   const void* in1; const uint8_t* in1_valid; int64_t in1_voff;
   const uint8_t* filt; int64_t filt_off; const uint8_t* filt_valid; int64_t filt_voff;
-  unsigned long long* acc0;  // sum / min / max / count
-  unsigned long long* acc1;  // AVG: count
+  unsigned long long* acc0;  // sum / min / max / count; Decimal128 SUM: low words; Decimal128 MIN / MAX / AVG: one {lo, hi} pair per slot
+  unsigned long long* acc1;  // AVG: count; Decimal128 SUM: high words
   uint8_t* seen;             // NullState::seen_values (nullptr = SeenValues::All)
 };
 struct AggSet { int n; AggDev a[kMaxAggs]; };
@@ -188,6 +189,41 @@ __host__ __device__ __forceinline__ double ordered_to_f64(uint64_t u) {
   return d;
 }
 
+__device__ __forceinline__ Key2 cas128(Key2* addr, Key2 cmp, Key2 val) {
+  Key2 old;
+  asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.global.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
+               : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
+  return old;
+}
+// a slot's Decimal128 {lo, hi} pair in one 128-bit access: never a mix of two CAS results
+__device__ __forceinline__ Key2 ld_pair(const Key2* addr) {
+  Key2 v;
+  asm volatile("{\n\t.reg .b128 t;\n\tld.relaxed.gpu.global.b128 t, [%2];\n\tmov.b128 {%0, %1}, t;\n\t}" : "=l"(v.lo), "=l"(v.hi) : "l"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ bool lt_i128(Key2 a, Key2 b) { return (long long)a.hi < (long long)b.hi || (a.hi == b.hi && a.lo < b.lo); }
+// i128 add_wrapping as two 64-bit atomics: the carry out of the low word is a function of this add alone (old + lo overflowed), so the
+// high words sum to the right value in any interleaving
+__device__ __forceinline__ void add_i128(unsigned long long* lo_word, unsigned long long* hi_word, unsigned long long lo, unsigned long long hi) {
+  const unsigned long long old = atomicAdd(lo_word, lo);
+  const unsigned long long carry = (old + lo) < old ? 1ull : 0ull;
+  if (hi + carry) atomicAdd(hi_word, hi + carry);
+}
+// Decimal128 MIN / MAX of the value at p into the slot w, signed i128 order.  Once a group has a few rows most values are not better than
+// the slot: one load, no atomic.  The load is one 128-bit access and the slot only ever improves, so "not better" than it is final.
+__device__ __forceinline__ void minmax_i128(Key2* w, const unsigned long long* p, bool is_min) {
+  const Key2 v{p[0], p[1]};
+  Key2 cur = ld_pair(w);
+  while (is_min ? lt_i128(v, cur) : lt_i128(cur, v)) {
+    const Key2 prev = cas128(w, cur, v);
+    if (prev.lo == cur.lo && prev.hi == cur.hi) break;
+    cur = prev;
+  }
+}
+
+// PAIR: the aggregate set has a Decimal128 MIN / MAX / AVG ({lo, hi} pair accumulators).  Only those update kernels compile their
+// updates: in the others the CAS loop would cost registers on every path (the 128-bit-key kernel would spill)
+template <bool PAIR>
 __device__ __forceinline__ void apply_agg(const AggDev& a, int64_t row, uint64_t slot) {
   // opt_filter: only rows whose filter is Some(true) contribute (accumulate.rs:373-470)
   if (a.filt) {
@@ -205,14 +241,9 @@ __device__ __forceinline__ void apply_agg(const AggDev& a, int64_t row, uint64_t
       atomicAdd(&a.acc0[slot], a.merge ? (unsigned long long)((const int64_t*)a.in0)[row] : 1ull);
       break;
     case DFGPU_AGG_SUM:
-      if (a.cls == 3) {
-        // Decimal128: i128 add_wrapping (sum.rs:316 on Decimal128Type) as two 64-bit atomics — the carry out of the low word is a
-        // function of this add alone (old + lo overflowed), so the high words sum to the right value in any interleaving
+      if (a.cls == 3) {   // Decimal128: i128 add_wrapping (sum.rs:316 on Decimal128Type)
         const unsigned long long* p = (const unsigned long long*)a.in0 + 2 * row;
-        const unsigned long long lo = p[0], hi = p[1];
-        const unsigned long long old = atomicAdd(&a.acc0[slot], lo);
-        const unsigned long long carry = (old + lo) < old ? 1ull : 0ull;
-        if (hi + carry) atomicAdd(&a.acc1[slot], hi + carry);
+        add_i128(&a.acc0[slot], &a.acc1[slot], p[0], p[1]);
       } else if (a.cls == 2) atomicAdd((double*)&a.acc0[slot], load_as_f64(a.in0, a.in0_type, row));
       else if (a.in0_type == DFGPU_UINT64) atomicAdd(&a.acc0[slot], (unsigned long long)((const uint64_t*)a.in0)[row]);
       else atomicAdd(&a.acc0[slot], (unsigned long long)load_as_i64(a.in0, a.in0_type, row));  // add_wrapping (sum.rs:316)
@@ -221,7 +252,8 @@ __device__ __forceinline__ void apply_agg(const AggDev& a, int64_t row, uint64_t
     case DFGPU_AGG_MIN:
     case DFGPU_AGG_MAX: {
       const bool is_min = a.func == DFGPU_AGG_MIN;
-      if (a.cls == 0) {
+      if (PAIR && a.cls == 3) minmax_i128((Key2*)a.acc0 + slot, (const unsigned long long*)a.in0 + 2 * row, is_min);
+      else if (a.cls == 0) {
         long long v = load_as_i64(a.in0, a.in0_type, row);
         if (is_min) atomicMin((long long*)&a.acc0[slot], v); else atomicMax((long long*)&a.acc0[slot], v);
       } else {
@@ -233,7 +265,15 @@ __device__ __forceinline__ void apply_agg(const AggDev& a, int64_t row, uint64_t
       break;
     }
     case DFGPU_AGG_AVG:
-      if (a.merge) {
+      if (PAIR && a.cls == 3) {
+        // Decimal128: i128 add_wrapping of the sum into the slot's {lo, hi} pair + a count (DecimalAverager's inputs).  The merge reads the
+        // no-GROUP-BY composite's internal state [count: UInt64, sum: Decimal128]
+        if (!(a.merge && a.in1_valid && !bit_get(a.in1_valid, a.in1_voff + row))) {
+          const unsigned long long* p = (const unsigned long long*)(a.merge ? a.in1 : a.in0) + 2 * row;
+          add_i128(&a.acc0[2 * slot], &a.acc0[2 * slot + 1], p[0], p[1]);
+        }
+        atomicAdd(&a.acc1[slot], a.merge ? (unsigned long long)((const uint64_t*)a.in0)[row] : 1ull);
+      } else if (a.merge) {
         // state = [count: UInt64, sum: Float64]
         unsigned long long c = ((const uint64_t*)a.in0)[row];
         atomicAdd(&a.acc1[slot], c);
@@ -254,13 +294,6 @@ struct TableDev {
   uint32_t* special_used;       // [0]: slot cap (key == all-ones), [1]: slot cap+1 (NULL group)
   int bucketed;                 // probe sequences start on a 32-byte boundary (4 x 8-byte tags): one sector holds the first 4 candidates
 };
-
-__device__ __forceinline__ Key2 cas128(Key2* addr, Key2 cmp, Key2 val) {
-  Key2 old;
-  asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.global.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
-               : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
-  return old;
-}
 
 // find-or-claim; returns slot or ~0ull when the row must be deferred (table budget exhausted)
 template <int KW>
@@ -309,7 +342,7 @@ __device__ __forceinline__ uint64_t find_or_claim(const TableDev& t, Key2 k, boo
 // the hot kernel: intern + accumulate.  Each thread owns R independent rows per iteration: their keys, then
 // their first-probe tags, are loaded back to back BEFORE any is consumed — the loop is latency-bound
 // (DRAM stream -> L2 tag -> RED), so memory-level parallelism per thread is what sets the rate.
-template <int KW, int R>
+template <int KW, int R, bool PAIR>
 __global__ void __launch_bounds__(256) agg_update_kernel(GroupCols g, AggSet aggs, TableDev t, int64_t row0, int64_t n,
                                                       const uint32_t* __restrict__ row_list, uint32_t* __restrict__ overflow,
                                                       unsigned long long* __restrict__ overflow_count) {
@@ -360,7 +393,7 @@ __global__ void __launch_bounds__(256) agg_update_kernel(GroupCols g, AggSet agg
       }
       if (KW == 1 && claimed && g.wide) store_group_key(g, row[r], slot);   // read back only by later kernels (verify, rehash, emit)
 #pragma unroll 1
-      for (int a = 0; a < aggs.n; ++a) apply_agg(aggs.a[a], row[r], slot);
+      for (int a = 0; a < aggs.n; ++a) apply_agg<PAIR>(aggs.a[a], row[r], slot);
     }
   }
 }
@@ -563,6 +596,8 @@ __global__ void __launch_bounds__(256) agg_fold_pairs_kernel(ulonglong2* __restr
   }
 }
 
+// per aggregate at most acc0, acc1 and seen (a Decimal128 MIN / MAX has acc0 + seen, a Decimal128 AVG acc0 + acc1); wide keys add two
+// stored words per group column and the NULL masks
 struct AccArrays { int n; void* ptr[kMaxAggs * 3 + kMaxGroupCols * 2 + 1]; void* new_ptr[kMaxAggs * 3 + kMaxGroupCols * 2 + 1]; int elem[kMaxAggs * 3 + kMaxGroupCols * 2 + 1]; };
 
 // grow: re-insert every occupied slot of the old table into the new one and move its accumulators
@@ -584,6 +619,7 @@ __global__ void __launch_bounds__(256) agg_rehash_kernel(TableDev old_t, TableDe
     }
     for (int a = 0; a < acc.n; ++a) {
       if (acc.elem[a] == 8) ((uint64_t*)acc.new_ptr[a])[ns] = ((const uint64_t*)acc.ptr[a])[s];
+      else if (acc.elem[a] == 16) ((ulonglong2*)acc.new_ptr[a])[ns] = ((const ulonglong2*)acc.ptr[a])[s];
       else ((uint8_t*)acc.new_ptr[a])[ns] = ((const uint8_t*)acc.ptr[a])[s];
     }
   }
@@ -622,7 +658,7 @@ __global__ void agg_init_seen_kernel(TableDev t, uint8_t* __restrict__ seen) {
 }
 
 // ---- emit kernels: one per output column, 32 consecutive outputs per warp ----
-enum EmitKind : int { EK_KEY = 0, EK_COPY64 = 1, EK_AVG = 2, EK_MINMAX = 3, EK_DEC128 = 4, EK_WIDEKEY = 5 };
+enum EmitKind : int { EK_KEY = 0, EK_COPY64 = 1, EK_AVG = 2, EK_MINMAX = 3, EK_DEC128 = 4, EK_WIDEKEY = 5, EK_PAIR128 = 6, EK_AVG_DEC = 7 };
 struct EmitDesc {
   int kind;
   int out_type;        // output column type
@@ -634,6 +670,8 @@ struct EmitDesc {
   const unsigned long long* acc1;
   const uint8_t* seen;
   int cls;             // EK_MINMAX: 0 signed, 1 unsigned, 2 float
+  int avg_mul, avg_prec;           // EK_AVG_DEC: sum * 10^avg_mul / count must fit Decimal128(avg_prec, _)
+  unsigned long long* err;         // EK_AVG_DEC: set to 1 on overflow
 };
 
 __device__ __forceinline__ void store_typed(void* out, int type, int64_t i, uint64_t bits) {
@@ -689,6 +727,20 @@ __global__ void __launch_bounds__(256) agg_emit_kernel(EmitDesc d, const uint32_
           ((unsigned long long*)out)[2 * i] = ok ? d.acc0[s] : 0ull;
           ((unsigned long long*)out)[2 * i + 1] = ok ? d.acc1[s] : 0ull;
           break;
+        case EK_PAIR128:   // the slot's {lo, hi} pair: Decimal128 MIN / MAX, the AVG sum state
+          if (d.seen) ok = d.seen[s] != 0;
+          ((unsigned long long*)out)[2 * i] = ok ? d.acc0[2 * s] : 0ull;
+          ((unsigned long long*)out)[2 * i + 1] = ok ? d.acc0[2 * s + 1] : 0ull;
+          break;
+        case EK_AVG_DEC: {   // DecimalAverager::avg (expr_dec.cuh dec_avg); no value -> NULL
+          const unsigned long long c = d.acc1[s];
+          ok = c != 0ull;
+          i128 q = 0;
+          if (ok && !dec_avg((i128)(((u128)d.acc0[2 * s + 1] << 64) | (u128)d.acc0[2 * s]), c, d.avg_mul, d.avg_prec, &q)) atomicOr(d.err, 1ull);
+          ((unsigned long long*)out)[2 * i] = (unsigned long long)(u128)q;
+          ((unsigned long long*)out)[2 * i + 1] = (unsigned long long)((u128)q >> 64);
+          break;
+        }
         case EK_AVG: {
           unsigned long long c = d.acc1[s];
           if (c == 0) { ok = false; break; }
@@ -751,6 +803,11 @@ __global__ void __launch_bounds__(256) agg_convert_state_kernel(AggSet aggs, Sta
             else ((uint64_t*)o.v0)[row] = !ok ? 0ull : (a.in0_type == DFGPU_UINT64 ? ((const uint64_t*)a.in0)[row] : (uint64_t)load_as_i64(a.in0, a.in0_type, row));
             break;
           case DFGPU_AGG_MIN: case DFGPU_AGG_MAX: {
+            if (type_width(o.t0) == 16) {   // Decimal128
+              const unsigned long long* p = (const unsigned long long*)a.in0 + 2 * row;
+              ((unsigned long long*)o.v0)[2 * row] = ok ? p[0] : 0ull; ((unsigned long long*)o.v0)[2 * row + 1] = ok ? p[1] : 0ull;
+              break;
+            }
             uint64_t v = 0;
             if (ok) {
               if (a.in0_type == DFGPU_FLOAT64) { double d = ((const double*)a.in0)[row]; memcpy(&v, &d, 8); }
@@ -787,6 +844,9 @@ __global__ void __launch_bounds__(256) salt_kernel(uint16_t* __restrict__ out, i
 __global__ void fill_u64_kernel(unsigned long long* p, uint64_t n, unsigned long long v) {
   for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) p[i] = v;
 }
+__global__ void fill_pair_kernel(ulonglong2* p, uint64_t n, ulonglong2 v) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) p[i] = v;
+}
 
 }  // namespace dfgpu
 
@@ -803,7 +863,9 @@ struct AggState {
   int first_state_col;  // state modes: index of this aggregate's first state column in the input
   DevBuf acc0, acc1, seen;
   bool track_seen = false;
-  unsigned long long init0 = 0;
+  unsigned long long init0 = 0, init1 = 0;   // init1: high word of a {lo, hi} pair accumulator
+  // Decimal128 MIN / MAX / AVG keep one 16-byte {lo, hi} pair per slot in acc0 (atom.cas.b128 swaps both words at once)
+  bool pair_acc() const { return cls == 3 && func != DFGPU_AGG_SUM; }
 };
 
 struct dfgpu_agg {
@@ -882,9 +944,16 @@ static void alloc_table(dfgpu_agg* a, uint64_t cap, DevBuf* tags, std::vector<De
   }
   acc0->resize(a->aggs.size()); acc1->resize(a->aggs.size()); seen->resize(a->aggs.size());
   for (size_t i = 0; i < a->aggs.size(); ++i) {
-    (*acc0)[i].alloc(ctx, (size_t)(cap + 2) * 8);
-    fill_u64(ctx, (*acc0)[i].ptr, cap + 2, a->aggs[i].init0);
-    if (a->aggs[i].func == DFGPU_AGG_AVG || a->aggs[i].cls == 3) { (*acc1)[i].alloc(ctx, (size_t)(cap + 2) * 8); (*acc1)[i].zero(); }   // AVG: count; Decimal128 SUM: high word
+    const AggState& st = a->aggs[i];
+    if (st.pair_acc()) {
+      (*acc0)[i].alloc(ctx, (size_t)(cap + 2) * 16);
+      fill_pair_kernel<<<grid_for((int64_t)cap + 2, 256, kNumSMs * 8), 256, 0, ctx->stream>>>((*acc0)[i].as<ulonglong2>(), cap + 2, make_ulonglong2(st.init0, st.init1));
+      DF_LAUNCH_CHECK(ctx);
+    } else {
+      (*acc0)[i].alloc(ctx, (size_t)(cap + 2) * 8);
+      fill_u64(ctx, (*acc0)[i].ptr, cap + 2, st.init0);
+    }
+    if (st.func == DFGPU_AGG_AVG || (st.cls == 3 && st.func == DFGPU_AGG_SUM)) { (*acc1)[i].alloc(ctx, (size_t)(cap + 2) * 8); (*acc1)[i].zero(); }   // AVG: count; Decimal128 SUM: high word
     if (a->aggs[i].track_seen) { (*seen)[i].alloc(ctx, (size_t)(cap + 2)); (*seen)[i].zero(); }
   }
 }
@@ -915,7 +984,7 @@ static void grow_table(dfgpu_agg* a, uint64_t new_cap) {
   AccArrays arr;
   arr.n = 0;
   for (size_t i = 0; i < a->aggs.size(); ++i) {
-    arr.ptr[arr.n] = a->aggs[i].acc0.ptr; arr.new_ptr[arr.n] = nacc0[i].ptr; arr.elem[arr.n++] = 8;
+    arr.ptr[arr.n] = a->aggs[i].acc0.ptr; arr.new_ptr[arr.n] = nacc0[i].ptr; arr.elem[arr.n++] = a->aggs[i].pair_acc() ? 16 : 8;
     if (a->aggs[i].acc1.ptr) { arr.ptr[arr.n] = a->aggs[i].acc1.ptr; arr.new_ptr[arr.n] = nacc1[i].ptr; arr.elem[arr.n++] = 8; }
     if (a->aggs[i].seen.ptr) { arr.ptr[arr.n] = a->aggs[i].seen.ptr; arr.new_ptr[arr.n] = nseen[i].ptr; arr.elem[arr.n++] = 1; }
   }
@@ -1065,6 +1134,8 @@ static void agg_push(dfgpu_agg* a, const std::vector<DCol>& cols) {
     if ((in0 && in0->validity) || filt) ensure_seen(a, s);
   }
   if (a->skipping) { agg_convert_batch_to_state(a, cols, set, n); return; }
+  bool pair = false;
+  for (const AggState& s : a->aggs) pair |= s.pair_acc();
   // fast-path eligibility (decided per batch: it depends on the validity of THIS batch's columns)
   static const int fast_enabled = getenv("DFGPU_AGG_FAST") ? atoi(getenv("DFGPU_AGG_FAST")) : 1;
   bool fast = fast_enabled && a->kw == 1 && g.n == 1 && g.width[0] == 8 && !g.valid[0] && !g.is_float[0] && set.n >= 1 && set.n <= kMaxFastAggs;
@@ -1151,10 +1222,17 @@ static void agg_push(dfgpu_agg* a, const std::vector<DCol>& cols) {
               default: agg_update_fast_kernel<4, 4, 0><<<grid, 256, 0, ctx->stream>>>(kp, fa, t, done, work, list, ov, oc); break;
             }
           }
-        } else if (a->kw == 1)
-          agg_update_kernel<1, 4><<<grid, 256, 0, ctx->stream>>>(g, set, t, done, work, list, overflow.as<uint32_t>(), a->counters.as<unsigned long long>() + 1);
-        else
-          agg_update_kernel<2, 4><<<grid, 256, 0, ctx->stream>>>(g, set, t, done, work, list, overflow.as<uint32_t>(), a->counters.as<unsigned long long>() + 1);
+        } else {
+          uint32_t* ov = overflow.as<uint32_t>();
+          unsigned long long* oc = a->counters.as<unsigned long long>() + 1;
+          if (a->kw == 1) {
+            if (pair) agg_update_kernel<1, 4, true><<<grid, 256, 0, ctx->stream>>>(g, set, t, done, work, list, ov, oc);
+            else agg_update_kernel<1, 4, false><<<grid, 256, 0, ctx->stream>>>(g, set, t, done, work, list, ov, oc);
+          } else {
+            if (pair) agg_update_kernel<2, 4, true><<<grid, 256, 0, ctx->stream>>>(g, set, t, done, work, list, ov, oc);
+            else agg_update_kernel<2, 4, false><<<grid, 256, 0, ctx->stream>>>(g, set, t, done, work, list, ov, oc);
+          }
+        }
         DF_LAUNCH_CHECK(ctx);
       }
       unsigned long long hc[2];
@@ -1275,7 +1353,8 @@ static void agg_emit_table(dfgpu_agg* a) {
   // a global aggregate (no GROUP BY) over empty input still yields one row in Final/Single modes; grouped: zero rows.
   BatchPtr out(new dfgpu_batch());
   out->ctx = ctx; out->rows = ng; out->host = false;
-  auto run_emit = [&](EmitDesc& d, int out_type, bool with_valid) -> DCol {
+  DevBuf avg_err;   // Decimal128 AVG overflow flag
+  auto run_emit =[&](EmitDesc& d, int out_type, bool with_valid) -> DCol {
     DCol col = alloc_col(ctx, out_type, ng, with_valid);
     if (ng > 0) {
       d.out_type = out_type; d.kw = a->kw; d.tags = a->tags.ptr; d.cap = a->cap;
@@ -1318,11 +1397,21 @@ static void agg_emit_table(dfgpu_agg* a) {
         out->cols.push_back(run_emit(d, DFGPU_INT64, false));  // COUNT is never NULL (count.rs:700-708)
         break;
       case DFGPU_AGG_MIN: case DFGPU_AGG_MAX:
-        d.kind = EK_MINMAX;
+        d.kind = s.pair_acc() ? EK_PAIR128 : EK_MINMAX;
         out->cols.push_back(run_emit(d, s.out_type, s.track_seen));
         break;
       case DFGPU_AGG_AVG:
-        if (a->state_output) {
+        if (s.cls == 3 && a->state_output) {   // the no-GROUP-BY composite's internal state [count: UInt64, sum: the argument's type]
+          EmitDesc dc = d; dc.kind = EK_COPY64; dc.acc0 = s.acc1.as<unsigned long long>(); dc.seen = nullptr;
+          out->cols.push_back(run_emit(dc, DFGPU_UINT64, false));
+          EmitDesc ds = d; ds.kind = EK_PAIR128; ds.seen = nullptr;
+          out->cols.push_back(run_emit(ds, s.in_type, false));
+        } else if (s.cls == 3) {
+          if (!avg_err.ptr) { avg_err.alloc(ctx, 8); avg_err.zero(); }
+          d.kind = EK_AVG_DEC; d.avg_mul = dec_scale(s.out_type) - dec_scale(s.in_type); d.avg_prec = dec_precision(s.out_type);
+          d.err = avg_err.as<unsigned long long>();
+          out->cols.push_back(run_emit(d, s.out_type, true));
+        } else if (a->state_output) {
           EmitDesc dc = d; dc.kind = EK_COPY64; dc.acc0 = s.acc1.as<unsigned long long>(); dc.seen = nullptr;
           out->cols.push_back(run_emit(dc, DFGPU_UINT64, false));
           EmitDesc ds = d; ds.kind = EK_COPY64; ds.seen = nullptr;
@@ -1334,18 +1423,17 @@ static void agg_emit_table(dfgpu_agg* a) {
         break;
     }
   }
+  if (avg_err.ptr && read_scalar<unsigned long long>(ctx, avg_err.as<unsigned long long>()))
+    throw Error(DFGPU_ERR_ARITH, "Arithmetic Overflow in AvgAccumulator");
   a->m_output_rows += ng;
   if (ng > 0 || a->group_cols.empty()) a->outq.push_back(std::move(out));
 }
 
-}  // namespace dfgpu
-
-extern "C" {
-
-int dfgpu_agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols, const int32_t* group_cols, int32_t n_group,
-                     const dfgpu_agg_desc* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size, int64_t capacity_hint, dfgpu_agg** out) {
-  DF_API_BEGIN(ctx)
-  DF_CHECK(ctx && out, DFGPU_ERR_INVALID, "null argument");
+// dec_avg_state: AVG over Decimal128 may take or emit the state [count: UInt64, sum: Decimal128(p, s)], where the sum is the i128
+// add_wrapping sum labelled with the argument's type.  Only the no-GROUP-BY composite sets it, between its two inner handles: DataFusion
+// pins no public Partial state for this AVG, so dfgpu_agg_create rejects it in the state modes.
+static dfgpu_agg* agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols, const int32_t* group_cols, int32_t n_group,
+                             const dfgpu_agg_desc* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size, int64_t capacity_hint, bool dec_avg_state) {
   DF_CHECK(n_group >= 0 && n_group <= kMaxGroupCols, DFGPU_ERR_UNSUPPORTED, "aggregate: at most 8 group columns");
   if (n_group == 0) {
     // ---- AggregateStream (no GROUP BY, aggregates/aggregate_stream.rs): exactly one output row, also for empty input ----
@@ -1360,25 +1448,25 @@ int dfgpu_agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols,
     std::vector<dfgpu_agg_desc> d1(aggs, aggs + n_aggs);
     if (!state_in) for (auto& d : d1) { if (d.func != DFGPU_AGG_COUNT_STAR) d.arg_col += 1; if (d.filter_col >= 0) d.filter_col += 1; }
     const int32_t g0 = 0;
-    int rc = dfgpu_agg_create(ctx, t1.data(), (int)t1.size(), &g0, 1, d1.data(), n_aggs, state_in ? DFGPU_AGG_PARTIAL_REDUCE : DFGPU_AGG_PARTIAL, batch_size, 1024, &a->inner1);
-    if (rc != DFGPU_OK) throw Error(rc, ctx->last_error);
+    const bool single = !state_in && !state_out;   // the inner state of a Decimal128 AVG never leaves the composite
+    a->inner1 = agg_create(ctx, t1.data(), (int)t1.size(), &g0, 1, d1.data(), n_aggs, state_in ? DFGPU_AGG_PARTIAL_REDUCE : DFGPU_AGG_PARTIAL, batch_size, 1024, single);
     // state schema emitted by inner1: [salt, state columns...]
     std::vector<int32_t> t2{DFGPU_UINT16};
     for (auto& st : a->inner1->aggs) {
       switch (st.func) {
-        case DFGPU_AGG_SUM: t2.push_back(st.cls == 2 ? DFGPU_FLOAT64 : (st.cls == 1 ? DFGPU_UINT64 : DFGPU_INT64)); break;
+        case DFGPU_AGG_SUM: t2.push_back(st.cls == 3 ? st.out_type : (st.cls == 2 ? DFGPU_FLOAT64 : (st.cls == 1 ? DFGPU_UINT64 : DFGPU_INT64))); break;
         case DFGPU_AGG_COUNT: case DFGPU_AGG_COUNT_STAR: t2.push_back(DFGPU_INT64); break;
         case DFGPU_AGG_MIN: case DFGPU_AGG_MAX: t2.push_back(st.out_type); break;
-        case DFGPU_AGG_AVG: t2.push_back(DFGPU_UINT64); t2.push_back(DFGPU_FLOAT64); break;
+        case DFGPU_AGG_AVG: t2.push_back(DFGPU_UINT64); t2.push_back(st.cls == 3 ? st.in_type : DFGPU_FLOAT64); break;
       }
     }
     a->scalar_state_types.assign(t2.begin() + 1, t2.end());
     std::vector<dfgpu_agg_desc> d2(aggs, aggs + n_aggs);
     for (auto& d : d2) { d.arg_col = -1; d.filter_col = -1; }
-    rc = dfgpu_agg_create(ctx, t2.data(), (int)t2.size(), &g0, 1, d2.data(), n_aggs, state_out ? DFGPU_AGG_PARTIAL_REDUCE : DFGPU_AGG_FINAL, batch_size, 16, &a->inner2);
-    if (rc != DFGPU_OK) { dfgpu_agg_destroy(a->inner1); a->inner1 = nullptr; throw Error(rc, ctx->last_error); }
-    *out = a.release();
-    return DFGPU_OK;
+    try {
+      a->inner2 = agg_create(ctx, t2.data(), (int)t2.size(), &g0, 1, d2.data(), n_aggs, state_out ? DFGPU_AGG_PARTIAL_REDUCE : DFGPU_AGG_FINAL, batch_size, 16, single);
+    } catch (...) { dfgpu_agg_destroy(a->inner1); a->inner1 = nullptr; throw; }
+    return a.release();
   }
   DF_CHECK(n_aggs >= 0 && n_aggs <= kMaxAggs, DFGPU_ERR_UNSUPPORTED, "aggregate: at most 8 aggregate expressions");
   set_device(ctx);
@@ -1457,14 +1545,32 @@ int dfgpu_agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols,
         s.init0 = 0; break;
       case DFGPU_AGG_COUNT: case DFGPU_AGG_COUNT_STAR: s.init0 = 0; break;
       case DFGPU_AGG_AVG:
-        DF_CHECK(type_is_int(vt) || type_is_float(vt), DFGPU_ERR_UNSUPPORTED, "AVG: numeric argument required");
-        s.cls = 2; s.init0 = 0; break;
+        if (type_is_decimal(vt)) {
+          // Avg::return_type (average.rs): Decimal128(min(38, p + 4), min(38, s + 4)), the value by DecimalAverager::avg at emission
+          DF_CHECK(dec_precision(vt) >= 1, DFGPU_ERR_UNSUPPORTED, "AVG: Decimal128 argument needs its precision and scale (DFGPU_DECIMAL128_TYPE)");
+          DF_CHECK(dec_avg_state || !(a->state_input || a->state_output), DFGPU_ERR_UNSUPPORTED,
+                   "AVG over Decimal128 runs in Single modes only: its Partial state is not defined");
+          s.cls = 3;
+          s.out_type = dec_type(std::min(38, dec_precision(vt) + 4), std::min(38, dec_scale(vt) + 4));
+        } else {
+          DF_CHECK(type_is_int(vt) || type_is_float(vt), DFGPU_ERR_UNSUPPORTED, "AVG: numeric argument required");
+          s.cls = 2;
+        }
+        s.init0 = 0; break;
       case DFGPU_AGG_MIN:
-        DF_CHECK(type_is_int(vt) || type_is_float(vt), DFGPU_ERR_UNSUPPORTED, "MIN: numeric argument required");
-        s.init0 = s.cls == 0 ? (unsigned long long)LLONG_MAX : ~0ull; break;
-      case DFGPU_AGG_MAX:
-        DF_CHECK(type_is_int(vt) || type_is_float(vt), DFGPU_ERR_UNSUPPORTED, "MAX: numeric argument required");
-        s.init0 = s.cls == 0 ? (unsigned long long)LLONG_MIN : 0ull; break;
+      case DFGPU_AGG_MAX: {
+        const bool is_min = s.func == DFGPU_AGG_MIN;
+        if (type_is_decimal(vt)) {   // signed i128 order; identity i128::MAX / i128::MIN as {lo, hi}
+          s.cls = 3;
+          s.init0 = is_min ? ~0ull : 0ull;
+          s.init1 = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN;
+          break;
+        }
+        DF_CHECK(type_is_int(vt) || type_is_float(vt), DFGPU_ERR_UNSUPPORTED, is_min ? "MIN: numeric argument required" : "MAX: numeric argument required");
+        if (is_min) s.init0 = s.cls == 0 ? (unsigned long long)LLONG_MAX : ~0ull;
+        else s.init0 = s.cls == 0 ? (unsigned long long)LLONG_MIN : 0ull;
+        break;
+      }
       default: throw Error(DFGPU_ERR_INVALID, "unknown aggregate function");
     }
     a->aggs.push_back(std::move(s));
@@ -1489,7 +1595,18 @@ int dfgpu_agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols,
     alloc_table(a.get(), cap, &a->tags, &acc0, &acc1, &seen, &a->kstore, &a->knull);
     for (size_t i = 0; i < a->aggs.size(); ++i) { a->aggs[i].acc0 = std::move(acc0[i]); a->aggs[i].acc1 = std::move(acc1[i]); a->aggs[i].seen = std::move(seen[i]); }
   }
-  *out = a.release();
+  return a.release();
+}
+
+}  // namespace dfgpu
+
+extern "C" {
+
+int dfgpu_agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols, const int32_t* group_cols, int32_t n_group,
+                     const dfgpu_agg_desc* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size, int64_t capacity_hint, dfgpu_agg** out) {
+  DF_API_BEGIN(ctx)
+  DF_CHECK(ctx && out, DFGPU_ERR_INVALID, "null argument");
+  *out = agg_create(ctx, input_types, n_cols, group_cols, n_group, aggs, n_aggs, mode, batch_size, capacity_hint, false);
   DF_API_END
 }
 

@@ -66,6 +66,18 @@ __device__ __forceinline__ bool dec_fits(i128 v, int precision) {
   return v < lim && v > -lim;
 }
 
+// AVG over Decimal128(p, s) into Decimal128(tp, ts) (DecimalAverager::avg): sum.mul_checked(10^mul) / count, mul = ts - s, truncated
+// toward zero and validated against tp.  count > 0.  Returns false on either overflow ("Arithmetic Overflow in AvgAccumulator").
+__device__ __forceinline__ bool dec_avg(i128 sum, unsigned long long count, int mul, int tp, i128* q) {
+  i128 m;
+  *q = 0;
+  if (mul_ovf128(sum, pow10_i128(mul), &m)) return false;
+  const i128 r = m / (i128)count;
+  if (!dec_fits(r, tp)) return false;
+  *q = r;
+  return true;
+}
+
 // i128 -> f64 (`as f64`, round to nearest even)
 __device__ __forceinline__ double i128_to_f64(i128 v) {
   const bool neg = v < 0;

@@ -1305,17 +1305,11 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
             v = (uint64_t)e.kmin + q;
             break;
           }
-          case 7: {   // DecimalAverager::avg: sum.mul_checked(10^(ts - s)) / count (truncated), validated against the target precision
+          case 7: {   // DecimalAverager::avg (expr_dec.cuh dec_avg)
             const unsigned long long cnt = r[e.cnt_word];
             ok = cnt != 0ull;
             i128 q = 0;
-            if (ok) {
-              const i128 sum = (i128)(((u128)r[e.word + 1] << 64) | (u128)r[e.word]);
-              i128 m;
-              const bool bad = mul_ovf128(sum, pow10_i128(e.avg_mul), &m);
-              if (!bad) q = m / (i128)cnt;
-              if (bad || !dec_fits(q, e.avg_prec)) { atomicOr(ec.err, 1ull); q = 0; }
-            }
+            if (ok && !dec_avg((i128)(((u128)r[e.word + 1] << 64) | (u128)r[e.word]), cnt, e.avg_mul, e.avg_prec, &q)) atomicOr(ec.err, 1ull);
             ((unsigned long long*)e.dst)[2 * i] = (unsigned long long)(u128)q;
             ((unsigned long long*)e.dst)[2 * i + 1] = (unsigned long long)((u128)q >> 64);
             break;

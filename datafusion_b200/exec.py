@@ -542,6 +542,8 @@ class AggregateExpr:
         return t
 
     def state_fields(self, t: Optional[pa.DataType]) -> List[pa.Field]:
+        if self.func == "avg" and pa.types.is_decimal128(t):
+            raise NotImplementedError(f"{self.alias}: AVG over {t} runs in Single modes only; its Partial state is not defined")
         if self.func == "avg":  # [count, sum] (aggregates/mod.rs:3591-3700 snapshots)
             return [pa.field(f"{self.alias}[count]", pa.uint64()), pa.field(f"{self.alias}[sum]", pa.float64())]
         return [pa.field(f"{self.alias}[{self.func}]", self.value_type(t))]
@@ -559,18 +561,30 @@ class GpuAggregateExec(ExecutionPlan):
         self.state_output = mode in ("Partial", "PartialReduce")
         gfields = [input.schema.field(g) for g in self.group_by]
         afields: List[pa.Field] = []
+        self._plan_error: Optional[NotImplementedError] = None
         for a in self.aggr_expr:
             t = self.input_schema.field(a.arg).type if a.arg is not None else None
             if self.state_output:
-                afields += a.state_fields(t)
+                try:
+                    afields += a.state_fields(t)
+                except NotImplementedError as e:   # the node stays inspectable by the optimizer rules; its schema and execution raise
+                    self._plan_error = e
             else:
                 afields.append(pa.field(a.alias, a.value_type(t)))
-        self.schema = pa.schema([pa.field(f.name, f.type, True) for f in gfields] + afields)
+        self._schema = pa.schema([pa.field(f.name, f.type, True) for f in gfields] + afields)
         self._metrics = {}
+
+    @property
+    def schema(self) -> pa.Schema:
+        if self._plan_error is not None:
+            raise self._plan_error
+        return self._schema
 
     def children(self): return [self.input]
 
     def execute(self, ctx):
+        if self._plan_error is not None:
+            raise self._plan_error
         isch = self.input.schema
         types = [type_id(f.type) for f in isch]
         gcols = [isch.get_field_index(g) for g in self.group_by]

@@ -347,7 +347,7 @@ enum dfgpu_agg_func {
   DFGPU_AGG_COUNT = 2,  /* functions-aggregate/src/count.rs:631-780                   */
   DFGPU_AGG_MIN = 3,
   DFGPU_AGG_MAX = 4,
-  DFGPU_AGG_AVG = 5,    /* state = [count:u64, sum] (aggregates/mod.rs:3591-3700)     */
+  DFGPU_AGG_AVG = 5,    /* state = [count:u64, sum] (aggregates/mod.rs:3591-3700); over Decimal128(p, s): Single modes only, see below */
   DFGPU_AGG_COUNT_STAR = 6
 };
 typedef struct dfgpu_agg_desc {
@@ -358,7 +358,13 @@ typedef struct dfgpu_agg_desc {
 } dfgpu_agg_desc;
 
 /* input schema: raw modes = the child's columns; state modes = [group cols..., state cols...] as emitted
- * by a Partial aggregate (sum: [sum]; count: [count]; avg: [count,sum]; min/max: [value]). */
+ * by a Partial aggregate (sum: [sum]; count: [count]; avg: [count,sum]; min/max: [value]).
+ * Arguments: SUM over integers (wrapping), floats and Decimal128(p, s) (-> Decimal128(min(38, p+10), s)); MIN / MAX over integers,
+ * floats and Decimal128 (the argument's type, signed i128 order; state = [value], every mode); AVG over integers and floats (-> Float64)
+ * and over Decimal128(p, s) -> Decimal128(min(38, p+4), min(38, s+4)) = sum * 10^(ts - s) / count truncated toward zero (DataFusion's
+ * DecimalAverager::avg).  DFGPU_ERR_ARITH ("Arithmetic Overflow in AvgAccumulator") from dfgpu_agg_finish when that multiply overflows
+ * i128 or the value exceeds the target precision.  AVG over Decimal128 has no defined Partial state: DFGPU_AGG_PARTIAL,
+ * DFGPU_AGG_PARTIAL_REDUCE and the Final modes reject it with DFGPU_ERR_UNSUPPORTED; without GROUP BY it runs in the Single modes. */
 int dfgpu_agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols,
                      const int32_t* group_cols, int32_t n_group,
                      const dfgpu_agg_desc* aggs, int32_t n_aggs,

@@ -9,8 +9,8 @@ lineitem-shaped columns are generated in HBM with dfgpu_generate_i64 (seeded): l
 values), l_shipdate Date32, and the money columns l_quantity, l_extendedprice, l_discount, l_tax in hundredths, as Int64 or as
 Decimal128(15,2) (the same unscaled integers).  The fused results are checked exactly against a host evaluation of the same columns
 at the timed size, in chunks (Float64 AVG within 1e-9 relative); kernels are timed with dfgpu_kernel_time over warmed steps.  The
-unfused chain (dfgpu_filter -> dfgpu_expr_evaluate_device -> dfgpu_agg) runs where it can: Q6 in both money types, Q1 with Int64
-money (AVG over Decimal128 is not on dfgpu_agg).  It streams the table in slices, as the operators would see batches.
+unfused chain (dfgpu_filter -> dfgpu_expr_evaluate_device -> dfgpu_agg) runs Q1 and Q6 in both money types, checked exactly the same
+way.  It streams the table in slices, as the operators would see batches.
 
 usage: python scripts/q1_q6_fused_timing.py [SF=100] [steps=5]"""
 import datetime
@@ -88,7 +88,8 @@ def as_decimal(ctx, cols, n, keep):
     return out
 
 
-def q1_program(dec):
+def q1_exprs(dec):
+    """Q1's two computed money expressions and its AVG argument programs"""
     if dec:
         one = [(D.EXPR_LITERAL, 0, D.decimal128(20, 0), 0, 1, 0.0)]
         dp = B(D.OP_MULTIPLY, C(4), B(D.OP_MINUS, one, C(5)))
@@ -98,6 +99,11 @@ def q1_program(dec):
         dp = B(D.OP_MULTIPLY, C(4), B(D.OP_MINUS, L(100), C(5)))
         ch = B(D.OP_MULTIPLY, dp, B(D.OP_PLUS, L(100), C(6)))
         avg = lambda i: CAST(C(i), D.FLOAT64)
+    return dp, ch, avg
+
+
+def q1_program(dec):
+    dp, ch, avg = q1_exprs(dec)
     pred = B(D.OP_LTEQ, C(2), L(Q1_CUT, D.DATE32))
     aggs = [(D.AGG_SUM, C(3)), (D.AGG_SUM, C(4)), (D.AGG_SUM, dp), (D.AGG_SUM, ch), (D.AGG_AVG, avg(3)), (D.AGG_AVG, avg(4)), (D.AGG_AVG, avg(5)),
             (D.AGG_COUNT_STAR, None)]
@@ -261,21 +267,20 @@ def main():
         rows, t = timed(ctx, lambda: run_fused(ctx, dcols, types, n, pred6, aggs6, [], [], "q6"), steps, fam)
         assert rows == [(ref_q6[0] if dec else wrap64(ref_q6[0]), ref_q6[1])], (rows, ref_q6)
         res[f"q6_{money}_fused"] = t
-        # the unfused chain: Q6 in both money types, Q1 with Int64 money
+        # the unfused chain; Q6 is SUM alone: dfgpu_agg without GROUP BY
         ex6 = [B(D.OP_MULTIPLY, C(4), C(5))]
-        try:   # SUM alone: dfgpu_agg without GROUP BY
-            rows, t = timed(ctx, lambda: run_unfused(ctx, dcols, types, n, pred6, ex6, [], [(D.AGG_SUM, 7)]), 1, fam)
-            assert rows == [(ref_q6[0] if dec else wrap64(ref_q6[0]),)], (rows, ref_q6)
-        except D.DfgpuError as e:
-            t = {"error": str(e)}
+        rows, t = timed(ctx, lambda: run_unfused(ctx, dcols, types, n, pred6, ex6, [], [(D.AGG_SUM, 7)]), 1, fam)
+        assert rows == [(ref_q6[0] if dec else wrap64(ref_q6[0]),)], (rows, ref_q6)
         res[f"q6_{money}_unfused"] = t
-        if not dec:
-            dp = B(D.OP_MULTIPLY, C(4), B(D.OP_MINUS, L(100), C(5)))
-            ex1 = [dp, B(D.OP_MULTIPLY, dp, B(D.OP_PLUS, L(100), C(6))), CAST(C(3), D.FLOAT64), CAST(C(4), D.FLOAT64), CAST(C(5), D.FLOAT64)]
-            a1 = [(D.AGG_SUM, 3), (D.AGG_SUM, 4), (D.AGG_SUM, 7), (D.AGG_SUM, 8), (D.AGG_AVG, 9), (D.AGG_AVG, 10), (D.AGG_AVG, 11), (D.AGG_COUNT_STAR, -1)]
-            rows, t = timed(ctx, lambda: run_unfused(ctx, dcols, types, n, pred, ex1, [0, 1], a1), 1, fam)
-            check_q1(sorted(rows, key=lambda r: (r[0], r[1])), ref_q1, False)
-            res[f"q1_{money}_unfused"] = t
+        dp, ch, avg = q1_exprs(dec)
+        if dec:   # AVG over the Decimal128 columns themselves
+            ex1, avg_cols = [dp, ch], (3, 4, 5)
+        else:
+            ex1, avg_cols = [dp, ch] + [avg(i) for i in (3, 4, 5)], (9, 10, 11)
+        a1 = [(D.AGG_SUM, 3), (D.AGG_SUM, 4), (D.AGG_SUM, 7), (D.AGG_SUM, 8)] + [(D.AGG_AVG, i) for i in avg_cols] + [(D.AGG_COUNT_STAR, -1)]
+        rows, t = timed(ctx, lambda: run_unfused(ctx, dcols, types, n, pred, ex1, [0, 1], a1), 1, fam)
+        check_q1(sorted(rows, key=lambda r: (r[0], r[1])), ref_q1, dec)
+        res[f"q1_{money}_unfused"] = t
     # DRAM floors from the shapes (not measured): every streamed byte once; Q6 touches l_extendedprice only for its survivors
     q6_sel = ref_q6[1] / n
     floors = {"q1_int64": 44 * n, "q1_decimal128": 76 * n, "q6_int64": (4 + 8 + 8 + 8 * q6_sel) * n, "q6_decimal128": (4 + 16 + 16 + 16 * q6_sel) * n}
