@@ -471,6 +471,8 @@ __global__ void __launch_bounds__(kFusedThreads) join_probe_fused_kernel(KeyCols
 //   Any duplicate key or the all-ones key aborts the attempt (flag) and the generic table is built instead.
 // ------------------------------------------------------------------------------------------
 constexpr int kMaxPayloadCols = 8;
+constexpr int kInlineSlotsPer100Rows = 250;   // hashed inline table: 250 slots per 100 build rows
+constexpr int kRadixSubTableMB = 16;          // radix-partitioned probe: table bytes per partition, a third of the 50 MB L2
 struct PayloadCols { int n; const void* ptr[kMaxPayloadCols]; int width[kMaxPayloadCols]; int shift[kMaxPayloadCols]; };
 struct InlineRef { void* slots; uint64_t cap; int dense; uint64_t amin; int bucket; /* probe sequences start on a 4-slot boundary (one 64 B line for 16 B slots) */
                    const unsigned long long* bloom; uint64_t bloom_blocks; /* optional membership filter over the build keys (dfgpu_hashjoin_options.membership_filter) */ };
@@ -540,7 +542,7 @@ __global__ void __launch_bounds__(256) join_build_inline_kernel(KeyCols kc, Payl
 }
 
 template <int W, bool BLOOM>
-__global__ void __launch_bounds__(kFusedThreads) join_probe_inline_v0_kernel(KeyCols kc, int64_t n, InlineRef t, InlineOut oc,
+__global__ void __launch_bounds__(kFusedThreads) join_probe_inline_kernel(KeyCols kc, int64_t n, InlineRef t, InlineOut oc,
                                                                        unsigned long long* __restrict__ tile_desc, unsigned int* __restrict__ tile_counter,
                                                                        unsigned long long* __restrict__ totals) {
   __shared__ unsigned long long s_pay[W == 2 ? kFusedTile : 1];
@@ -638,191 +640,6 @@ __global__ void __launch_bounds__(kFusedThreads) join_probe_inline_v0_kernel(Key
   }
 }
 
-// ------------------------------------------------------------------------------------------
-// L2-sliced probe of the inline table (table much larger than the 50 MB L2).
-//
-// A random 16 B lookup that misses L2 costs one DRAM access whatever the fetch size (scripts/microbench_gran.cu measures
-// it); the same lookup served by L2 is several times faster.  So the table is cut into S slices of
-// contiguous slots that fit L2 (slice of a key = fastrange(hash, S), monotone in the slot), and the probe runs slice
-// by slice: pass s streams ALL probe keys (coalesced, 8 B/row) but looks up only the rows of slice s, so every
-// lookup of the pass hits the same L2-resident slice (DFGPU_JOIN_SLICE_MB).  A pass leaves, per 1024-row tile, the payloads of its rows as
-// one dense run (tile-major scratch: [tile][slice 0 rows | slice 1 rows | ...], 8 B + 1 hit byte per row).  The emit
-// kernel then walks the tiles in order, recomputes every row's (slice, rank inside the slice run) from packed
-// counters, picks up payload + hit flag, and finishes exactly like the single-pass kernel (compaction, decoupled
-// look-back, coalesced column writes) — same output, same order.
-// ------------------------------------------------------------------------------------------
-constexpr int kMaxSlices = 8;
-
-template <int W>
-__global__ void __launch_bounds__(kFusedThreads) join_probe_slice_pass_kernel(KeyCols kc, int64_t n, InlineRef t, int slice, int n_slices,
-                                                                             unsigned long long* __restrict__ inter, uint8_t* __restrict__ hit8) {
-  __shared__ unsigned long long s_pay[W == 2 ? kFusedTile : 1];
-  __shared__ uint8_t s_hit[kFusedTile];
-  const int64_t tile = blockIdx.x;
-  const int64_t row0 = tile * kFusedTile + (int64_t)threadIdx.x * kFusedItems;
-  uint64_t tags[kFusedItems], slot[kFusedItems];
-  bool mine[kFusedItems];
-  uint32_t below = 0, m = 0;
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    const int64_t i = row0 + k;
-    uint64_t tag;
-    mine[k] = false; tags[k] = 0; slot[k] = 0;
-    if (i < n && load_tag(kc, i, &tag) && tag != kEmpty64) {
-      const uint64_t h = hash_u64(tag, kSeedJoin);
-      const int sl = (int)__umul64hi(h, (uint64_t)n_slices);
-      if (sl < slice) below++;
-      else if (sl == slice) { mine[k] = true; m++; tags[k] = tag; slot[k] = __umul64hi(h, t.cap); }
-    }
-  }
-  uint64_t cur[kFusedItems], curp[kFusedItems];
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    cur[k] = kEmpty64; curp[k] = 0;
-    if (mine[k]) {
-      if (W == 2) { const uint4 v = __ldcg((const uint4*)t.slots + slot[k]); cur[k] = (uint64_t)v.x | ((uint64_t)v.y << 32); curp[k] = (uint64_t)v.z | ((uint64_t)v.w << 32); }
-      else cur[k] = __ldcg((const unsigned long long*)t.slots + slot[k]);
-    }
-  }
-  bool hit[kFusedItems];
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    hit[k] = false;
-    if (!mine[k]) continue;
-    while (true) {
-      if (cur[k] == tags[k]) { hit[k] = true; break; }
-      if (cur[k] == kEmpty64) break;
-      if (++slot[k] == t.cap) slot[k] = 0;
-      if (W == 2) { const uint4 v = __ldcg((const uint4*)t.slots + slot[k]); cur[k] = (uint64_t)v.x | ((uint64_t)v.y << 32); curp[k] = (uint64_t)v.z | ((uint64_t)v.w << 32); }
-      else cur[k] = __ldcg((const unsigned long long*)t.slots + slot[k]);
-    }
-  }
-  uint32_t tot;
-  uint32_t ex = block_exclusive_scan<kFusedThreads, uint32_t>(m | (below << 16), &tot);   // both fit 16 bits (tile = 1024 rows)
-  ex &= 0xFFFFu;
-  const uint32_t mine_tot = tot & 0xFFFFu, off = tot >> 16;   // this slice's run starts after the rows of the lower slices
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k)
-    if (mine[k]) { if (W == 2) s_pay[ex] = curp[k]; s_hit[ex] = hit[k] ? 1 : 0; ++ex; }
-  __syncthreads();
-  const int64_t base = tile * kFusedTile + off;
-  for (uint32_t j = threadIdx.x; j < mine_tot; j += kFusedThreads) {
-    if (W == 2) inter[base + j] = s_pay[j];
-    hit8[base + j] = s_hit[j];
-  }
-}
-
-template <int W>
-__global__ void __launch_bounds__(kFusedThreads) join_probe_slice_emit_kernel(KeyCols kc, int64_t n, InlineRef t, int n_slices, const unsigned long long* __restrict__ inter,
-                                                                             const uint8_t* __restrict__ hit8, InlineOut oc, unsigned long long* __restrict__ tile_desc,
-                                                                             unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals) {
-  __shared__ unsigned long long s_pay[W == 2 ? kFusedTile : 1];
-  __shared__ uint32_t s_p[kFusedTile];
-  __shared__ unsigned long long s_w[kFusedThreads / 32][2];
-  __shared__ unsigned int s_tile;
-  __shared__ unsigned long long s_base;
-  if (threadIdx.x == 0) s_tile = atomicAdd(tile_counter, 1u);
-  __syncthreads();
-  const int64_t tile = s_tile;
-  const int64_t row0 = tile * kFusedTile + (int64_t)threadIdx.x * kFusedItems;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  int sl[kFusedItems];
-  unsigned long long lo = 0, hi = 0;    // rows of this thread per slice: 4 x 16-bit lanes per word
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    const int64_t i = row0 + k;
-    uint64_t tag;
-    sl[k] = -1;
-    if (i < n && load_tag(kc, i, &tag) && tag != kEmpty64) {
-      sl[k] = (int)__umul64hi(hash_u64(tag, kSeedJoin), (uint64_t)n_slices);
-      if (sl[k] < 4) lo += 1ull << (16 * sl[k]); else hi += 1ull << (16 * (sl[k] - 4));
-    }
-  }
-  unsigned long long ilo = lo, ihi = hi;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const unsigned long long a = __shfl_up_sync(0xffffffffu, ilo, d), b = __shfl_up_sync(0xffffffffu, ihi, d);
-    if (lane >= d) { ilo += a; ihi += b; }
-  }
-  if (lane == 31) { s_w[warp][0] = ilo; s_w[warp][1] = ihi; }
-  __syncthreads();
-  unsigned long long wlo = 0, whi = 0, tlo = 0, thi = 0;
-#pragma unroll
-  for (int w = 0; w < kFusedThreads / 32; ++w) {
-    const unsigned long long a = s_w[w][0], b = s_w[w][1];
-    if (w < warp) { wlo += a; whi += b; }
-    tlo += a; thi += b;
-  }
-  // start of every slice's run inside the tile (packed), then this thread's running position per slice
-  unsigned long long plo = 0, phi = 0;
-  {
-    uint32_t run = 0;
-#pragma unroll
-    for (int q = 0; q < kMaxSlices; ++q) {
-      if (q < 4) plo |= (unsigned long long)run << (16 * q); else phi |= (unsigned long long)run << (16 * (q - 4));
-      run += (uint32_t)((q < 4 ? tlo : thi) >> (16 * (q & 3))) & 0xFFFFu;
-    }
-  }
-  unsigned long long blo = plo + wlo + ilo - lo, bhi = phi + whi + ihi - hi;
-  bool hit[kFusedItems];
-  uint64_t pays[kFusedItems];
-  uint32_t m = 0;
-  const int64_t tbase = tile * kFusedTile;
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    hit[k] = false; pays[k] = 0;
-    if (sl[k] < 0) continue;
-    const int sh = 16 * (sl[k] & 3);
-    uint32_t r;
-    if (sl[k] < 4) { r = (uint32_t)(blo >> sh) & 0xFFFFu; blo += 1ull << sh; }
-    else { r = (uint32_t)(bhi >> sh) & 0xFFFFu; bhi += 1ull << sh; }
-    hit[k] = hit8[tbase + r] != 0;
-    if (W == 2 && hit[k]) pays[k] = inter[tbase + r];
-    m += hit[k] ? 1u : 0u;
-  }
-  uint32_t tot;
-  uint32_t ex = block_exclusive_scan<kFusedThreads, uint32_t>(m, &tot);
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k)
-    if (hit[k]) { if (W == 2) s_pay[ex] = pays[k]; s_p[ex] = (uint32_t)(row0 + k - tile * kFusedTile); ++ex; }
-  if (threadIdx.x < 32) {
-    unsigned long long exclusive = tile_lookback(tile, tot, tile_desc);
-    if (threadIdx.x == 0) {
-      s_base = exclusive;
-      if ((tile + 1) * (int64_t)kFusedTile >= n) totals[0] = exclusive + tot;
-      if (tot) atomicAdd(&totals[1], (unsigned long long)tot);
-    }
-  }
-  __syncthreads();
-  const unsigned long long base = s_base;
-  const int64_t prow0 = tile * kFusedTile;
-  if (oc.pidx_out) for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) oc.pidx_out[base + j] = (uint32_t)(prow0 + s_p[j]);
-  for (int c = 0; c < oc.n; ++c) {
-    if (oc.kind[c] == 0) {
-      switch (oc.width[c]) {
-        case 8: { const uint64_t* src = (const uint64_t*)oc.src[c]; uint64_t* dst = (uint64_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        case 4: { const uint32_t* src = (const uint32_t*)oc.src[c]; uint32_t* dst = (uint32_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        case 2: { const uint16_t* src = (const uint16_t*)oc.src[c]; uint16_t* dst = (uint16_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        case 1: { const uint8_t* src = (const uint8_t*)oc.src[c]; uint8_t* dst = (uint8_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        default: { const uint4* src = (const uint4*)oc.src[c]; uint4* dst = (uint4*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-      }
-    } else if (oc.kind[c] == 1 && W == 2) {
-      const int sh = oc.shift[c];
-      switch (oc.width[c]) {
-        case 8: { uint64_t* dst = (uint64_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = s_pay[j]; break; }
-        case 4: { uint32_t* dst = (uint32_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = (uint32_t)(s_pay[j] >> sh); break; }
-        case 2: { uint16_t* dst = (uint16_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = (uint16_t)(s_pay[j] >> sh); break; }
-        default: { uint8_t* dst = (uint8_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = (uint8_t)(s_pay[j] >> sh); break; }
-      }
-    }
-  }
-}
-
 constexpr int kStageCols = 4;   // probe-side output columns staged through shared memory (8 B each per row)
 
 // width-generic loads / stores of one value as 64 bits
@@ -847,9 +664,10 @@ __device__ __forceinline__ void store_w(void* p, int width, uint64_t i, uint64_t
 // probe column is one fully coalesced 2 KB wavefront.  Matched rows are ranked in row order with warp
 // ballots + one 32-entry scan, their output values (payload word + up to 4 probe-side columns, read while
 // the lines are hot) are staged in shared memory, the tile's output offset comes from the decoupled
-// look-back, and every output column is then written with fully coalesced stores.
+// look-back, and every output column is then written with fully coalesced stores.  The pipelined host probe
+// runs it on each staged chunk.
 template <int W>
-__global__ void __launch_bounds__(kFusedThreads) join_probe_inline_kernel(KeyCols kc, int64_t n, InlineRef t, InlineOut oc,
+__global__ void __launch_bounds__(kFusedThreads) join_probe_inline_staged_kernel(KeyCols kc, int64_t n, InlineRef t, InlineOut oc,
                                                                        unsigned long long* __restrict__ tile_desc, unsigned int* __restrict__ tile_counter,
                                                                        unsigned long long* __restrict__ totals) {
   __shared__ unsigned long long s_pay[W == 2 ? kFusedTile : 1];
@@ -952,121 +770,6 @@ __global__ void __launch_bounds__(kFusedThreads) join_probe_inline_kernel(KeyCol
         for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]];
       } else {
         for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) store_w(oc.dst[c], oc.width[c], base + j, load_w(oc.src[c], oc.width[c], prow0 + s_p[j]));
-      }
-    } else if (oc.kind[c] == 1 && W == 2) {
-      const int sh = oc.shift[c];
-      switch (oc.width[c]) {
-        case 8: { uint64_t* dst = (uint64_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = s_pay[j]; break; }
-        case 4: { uint32_t* dst = (uint32_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = (uint32_t)(s_pay[j] >> sh); break; }
-        case 2: { uint16_t* dst = (uint16_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = (uint16_t)(s_pay[j] >> sh); break; }
-        default: { uint8_t* dst = (uint8_t*)oc.dst[c] + base; for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = (uint8_t)(s_pay[j] >> sh); break; }
-      }
-    }
-  }
-}
-
-// Tile = 256 threads x 4 rows, rows interleaved (row = tile_base + k*256 + tid) so every global load of a
-// probe column is one fully coalesced 2 KB wavefront.  Matched rows are ranked in row order with warp
-// ballots + one 32-entry scan, their output values (payload word + up to 4 probe-side columns, read while
-// the lines are hot) are staged in shared memory, the tile's output offset comes from the decoupled
-// look-back, and every output column is then written with fully coalesced stores.
-template <int W>
-__global__ void __launch_bounds__(kFusedThreads) join_probe_inline_v2_kernel(KeyCols kc, int64_t n, InlineRef t, InlineOut oc,
-                                                                       unsigned long long* __restrict__ tile_desc, unsigned int* __restrict__ tile_counter,
-                                                                       unsigned long long* __restrict__ totals) {
-  __shared__ unsigned long long s_pay[W == 2 ? kFusedTile : 1];
-  __shared__ uint32_t s_p[kFusedTile];
-  __shared__ uint32_t s_cnt[kFusedItems * (kFusedThreads / 32) + 1];
-  __shared__ unsigned int s_tile;
-  __shared__ unsigned long long s_base;
-  if (threadIdx.x == 0) s_tile = atomicAdd(tile_counter, 1u);
-  __syncthreads();
-  const int64_t tile = s_tile;
-  const int64_t prow0 = tile * kFusedTile;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  uint64_t tags[kFusedItems], slot[kFusedItems], pays[kFusedItems], cur[kFusedItems], curp[kFusedItems];
-  bool live[kFusedItems], hit[kFusedItems];
-  // phase 1: keys, then first-slot loads, for all 4 rows before any is consumed (memory-level parallelism)
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    const int64_t i = prow0 + k * kFusedThreads + threadIdx.x;
-    live[k] = i < n && load_tag(kc, i, &tags[k]) && tags[k] != kEmpty64;
-    hit[k] = false; pays[k] = 0; slot[k] = 0;
-    if (live[k]) {
-      if (t.dense) { slot[k] = tags[k] - t.amin; if (slot[k] >= t.cap) live[k] = false; }
-      else slot[k] = __umul64hi(hash_u64(tags[k], kSeedJoin), t.cap);
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    cur[k] = kEmpty64; curp[k] = 0;
-    if (live[k]) {
-      if (W == 2) { const uint4 v = __ldcg((const uint4*)t.slots + slot[k]); cur[k] = (uint64_t)v.x | ((uint64_t)v.y << 32); curp[k] = (uint64_t)v.z | ((uint64_t)v.w << 32); }
-      else cur[k] = __ldcg((const unsigned long long*)t.slots + slot[k]);
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    if (!live[k]) continue;
-    while (true) {  // linear probing continues only on a foreign key (never in dense mode)
-      if (cur[k] == tags[k]) { hit[k] = true; pays[k] = curp[k]; break; }
-      if (cur[k] == kEmpty64 || t.dense) break;
-      if (++slot[k] == t.cap) slot[k] = 0;
-      if (W == 2) { const uint4 v = __ldcg((const uint4*)t.slots + slot[k]); cur[k] = (uint64_t)v.x | ((uint64_t)v.y << 32); curp[k] = (uint64_t)v.z | ((uint64_t)v.w << 32); }
-      else cur[k] = __ldcg((const unsigned long long*)t.slots + slot[k]);
-    }
-  }
-  // phase 2: rank the matches in row order: (k, warp) segments are consecutive row ranges
-  uint32_t bal[kFusedItems];
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    bal[k] = __ballot_sync(0xffffffffu, hit[k]);
-    if (lane == 0) s_cnt[k * (kFusedThreads / 32) + warp] = __popc(bal[k]);
-  }
-  __syncthreads();
-  if (warp == 0) {  // exclusive scan of the 32 segment counts
-    uint32_t c = s_cnt[lane], inc = c;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) { uint32_t nb = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += nb; }
-    s_cnt[lane] = inc - c;
-    if (lane == 31) s_cnt[32] = inc;
-  }
-  __syncthreads();
-  const uint32_t tot = s_cnt[32];
-  // phase 3: stage output values of the matched rows
-#pragma unroll
-  for (int k = 0; k < kFusedItems; ++k) {
-    if (!hit[k]) continue;
-    const uint32_t pos = s_cnt[k * (kFusedThreads / 32) + warp] + __popc(bal[k] & ((1u << lane) - 1u));
-    const int64_t i = prow0 + k * kFusedThreads + threadIdx.x;
-    if (W == 2) s_pay[pos] = pays[k];
-    s_p[pos] = (uint32_t)(i - prow0);
-  }
-  if (threadIdx.x < 32) {
-    unsigned long long exclusive = tile_lookback(tile, tot, tile_desc);
-    if (threadIdx.x == 0) {
-      s_base = exclusive;
-      if ((tile + 1) * (int64_t)kFusedTile >= n) totals[0] = exclusive + tot;
-      if (tot) atomicAdd(&totals[1], (unsigned long long)tot);
-    }
-  }
-  __syncthreads();
-  const unsigned long long base = s_base;
-  if (oc.pidx_out) for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) oc.pidx_out[base + j] = (uint32_t)(prow0 + s_p[j]);
-  // phase 4: coalesced column writes
-  for (int c = 0; c < oc.n; ++c) {
-    if (oc.kind[c] == 0) {
-      switch (oc.width[c]) {
-        case 8: { const uint64_t* src = (const uint64_t*)oc.src[c]; uint64_t* dst = (uint64_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        case 4: { const uint32_t* src = (const uint32_t*)oc.src[c]; uint32_t* dst = (uint32_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        case 2: { const uint16_t* src = (const uint16_t*)oc.src[c]; uint16_t* dst = (uint16_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        case 1: { const uint8_t* src = (const uint8_t*)oc.src[c]; uint8_t* dst = (uint8_t*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
-        default: { const uint4* src = (const uint4*)oc.src[c]; uint4* dst = (uint4*)oc.dst[c] + base;
-                  for (uint32_t j = threadIdx.x; j < tot; j += kFusedThreads) dst[j] = src[prow0 + s_p[j]]; break; }
       }
     } else if (oc.kind[c] == 1 && W == 2) {
       const int sh = oc.shift[c];
@@ -1412,12 +1115,11 @@ static void finish_build(dfgpu_hashjoin* j) {
     }
     if (ok) {
       const int W = pc.n ? 2 : 1;
-      static const int cap_pct = getenv("DFGPU_JOIN_CAP_PCT") ? atoi(getenv("DFGPU_JOIN_CAP_PCT")) : 250;  // table slots per 100 build rows
-      const uint64_t cap = j->use_array_map ? j->table.asize : ((std::max<uint64_t>(1024, (uint64_t)n * cap_pct / 100) + 3) & ~3ull);
+      const uint64_t cap = j->use_array_map ? j->table.asize : ((std::max<uint64_t>(1024, (uint64_t)n * kInlineSlotsPer100Rows / 100) + 3) & ~3ull);
       j->inline_slots.alloc(ctx, (size_t)cap * 8 * W);
       j->inline_slots.fill(0xFF);
       j->iref.slots = j->inline_slots.ptr; j->iref.cap = cap; j->iref.dense = j->use_array_map ? 1 : 0; j->iref.amin = j->table.amin;
-      j->iref.bucket = 0;   // bucket-aligned start slots were a round-1 experiment that only the v0 probe kernel honoured (ADVICE r1): retired
+      j->iref.bucket = 0;   // bucket-aligned start slots were a round-1 experiment that only join_probe_inline_kernel honoured (ADVICE r1): retired
       DF_CUDA(cudaMemsetAsync(j->counters.ptr, 0, 64, ctx->stream));
       {
         KernelTimer kt(ctx, "join_build");
@@ -1695,11 +1397,9 @@ static void push_probe(dfgpu_hashjoin* j, std::vector<DCol>&& cols) {
     }
     // ---- radix-partitioned probe (row order not required, table several times the L2): radix_probe.cuh ----
     {
-      static const int radix_env = getenv("DFGPU_JOIN_RADIX") ? atoi(getenv("DFGPU_JOIN_RADIX")) : 1;
-      static const int radix_mb = std::max(1, getenv("DFGPU_JOIN_RADIX_MB") ? atoi(getenv("DFGPU_JOIN_RADIX_MB")) : 16);   // sub-table per partition: a third of the 50 MB L2
       const size_t tbytes = (size_t)j->iref.cap * 8 * j->inline_words;
       const int force_parts = getenv("DFGPU_JOIN_RADIX_PARTS") ? atoi(getenv("DFGPU_JOIN_RADIX_PARTS")) : 0;   // tests force the path on small inputs
-      bool radix = radix_env && !j->opt.ordered_output && !j->iref.dense && !j->iref.bucket && !need_pidx && pk.n == 1 && pk.width[0] == 8 && !pk.valid[0] &&
+      bool radix = !j->opt.ordered_output && !j->iref.dense && !j->iref.bucket && !need_pidx && pk.n == 1 && pk.width[0] == 8 && !pk.valid[0] &&
                    ((uintptr_t)pk.ptr[0] % 16 == 0) && ((tbytes > (size_t)40 << 20 && n >= (1ll << 22)) || force_parts >= 2);
       // every probe-side output column must be the key column or ONE other plain 8-byte column (it rides in the 16-byte record)
       int carry = -1;
@@ -1716,7 +1416,7 @@ static void push_probe(dfgpu_hashjoin* j, std::vector<DCol>&& cols) {
       }
       if (radix) {
         int bits = 1;
-        const size_t want = force_parts >= 2 ? (size_t)force_parts : (tbytes + ((size_t)radix_mb << 20) - 1) / ((size_t)radix_mb << 20);
+        const size_t want = force_parts >= 2 ? (size_t)force_parts : (tbytes + ((size_t)kRadixSubTableMB << 20) - 1) / ((size_t)kRadixSubTableMB << 20);
         while ((1u << bits) < want && bits < 6) ++bits;
         const int P = 1 << bits;
         const unsigned long long* keys = (const unsigned long long*)pk.ptr[0];
@@ -1771,45 +1471,14 @@ static void push_probe(dfgpu_hashjoin* j, std::vector<DCol>&& cols) {
     desc.zero();
     unsigned long long* totals = (unsigned long long*)((char*)desc.ptr + (size_t)nt * 8);
     unsigned int* counter = (unsigned int*)(totals + 2);
-    // L2-sliced probe (table several times the L2, large batch).  Measured slower than the single-pass kernel (each extra key
-    // pass costs a full read of the keys and the slice does not stay L2-resident next to the key stream), so it is OFF unless DFGPU_JOIN_SLICED=1 / DFGPU_JOIN_SLICES=n; kept because the parity tests cover it.
-    // (environment read per call: the parity tests force the sliced path on small inputs with DFGPU_JOIN_SLICES=n)
-    const int sliced_env = getenv("DFGPU_JOIN_SLICED") ? atoi(getenv("DFGPU_JOIN_SLICED")) : 0;
-    const int slice_mb = std::max(1, getenv("DFGPU_JOIN_SLICE_MB") ? atoi(getenv("DFGPU_JOIN_SLICE_MB")) : 32);   // a slice well inside the 50 MB L2
-    const int forced_slices = getenv("DFGPU_JOIN_SLICES") ? atoi(getenv("DFGPU_JOIN_SLICES")) : 0;
-    const size_t table_bytes = (size_t)j->iref.cap * 8 * j->inline_words;
-    int n_slices = (int)std::min<size_t>(kMaxSlices, (table_bytes + (size_t)slice_mb * 1000000 - 1) / ((size_t)slice_mb * 1000000));
-    bool sliced = sliced_env && !j->iref.dense && !j->iref.bucket && n_slices >= 2 && n >= (1ll << 22);
-    if (forced_slices >= 2 && !j->iref.dense && !j->iref.bucket) { sliced = true; n_slices = std::min(forced_slices, kMaxSlices); }
-    if (sliced) {
-      DevBuf inter, hit8;
-      if (j->inline_words == 2) inter.alloc(ctx, (size_t)nt * kFusedTile * 8);
-      hit8.alloc(ctx, (size_t)nt * kFusedTile);
+    {
       KernelTimer kt(ctx, "join_probe");
-      for (int sidx = 0; sidx < n_slices; ++sidx) {
-        if (j->inline_words == 2) join_probe_slice_pass_kernel<2><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, sidx, n_slices, inter.as<unsigned long long>(), hit8.as<uint8_t>());
-        else join_probe_slice_pass_kernel<1><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, sidx, n_slices, nullptr, hit8.as<uint8_t>());
-      }
-      if (j->inline_words == 2) join_probe_slice_emit_kernel<2><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, n_slices, inter.as<unsigned long long>(), hit8.as<uint8_t>(), oc, desc.as<unsigned long long>(), counter, totals);
-      else join_probe_slice_emit_kernel<1><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, n_slices, nullptr, hit8.as<uint8_t>(), oc, desc.as<unsigned long long>(), counter, totals);
-      DF_LAUNCH_CHECK(ctx);
-    } else {
-      KernelTimer kt(ctx, "join_probe");
-      static const int variant = getenv("DFGPU_JOIN_VARIANT") ? atoi(getenv("DFGPU_JOIN_VARIANT")) : 0;
-      if (variant == 2) {
-        if (j->inline_words == 2) join_probe_inline_v2_kernel<2><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
-        else join_probe_inline_v2_kernel<1><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
-      } else if (variant == 0) {
-        if (j->iref.bloom) {
-          if (j->inline_words == 2) join_probe_inline_v0_kernel<2, true><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
-          else join_probe_inline_v0_kernel<1, true><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
-        } else {
-          if (j->inline_words == 2) join_probe_inline_v0_kernel<2, false><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
-          else join_probe_inline_v0_kernel<1, false><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
-        }
+      if (j->iref.bloom) {
+        if (j->inline_words == 2) join_probe_inline_kernel<2, true><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
+        else join_probe_inline_kernel<1, true><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
       } else {
-        if (j->inline_words == 2) join_probe_inline_kernel<2><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
-        else join_probe_inline_kernel<1><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
+        if (j->inline_words == 2) join_probe_inline_kernel<2, false><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
+        else join_probe_inline_kernel<1, false><<<(int)nt, kFusedThreads, 0, ctx->stream>>>(pk, n, j->iref, oc, desc.as<unsigned long long>(), counter, totals);
       }
       DF_LAUNCH_CHECK(ctx);
     }
@@ -2003,8 +1672,8 @@ static bool push_probe_host_pipelined(dfgpu_hashjoin* j, const dfgpu_column* hco
     unsigned int* counter = (unsigned int*)(totals + 2);
     {
       KernelTimer kt(ctx, "join_probe");
-      if (j->inline_words == 2) join_probe_inline_kernel<2><<<(int)ntl, kFusedThreads, 0, ctx->stream>>>(pk, len, j->iref, oc, desc[b].as<unsigned long long>(), counter, totals);
-      else join_probe_inline_kernel<1><<<(int)ntl, kFusedThreads, 0, ctx->stream>>>(pk, len, j->iref, oc, desc[b].as<unsigned long long>(), counter, totals);
+      if (j->inline_words == 2) join_probe_inline_staged_kernel<2><<<(int)ntl, kFusedThreads, 0, ctx->stream>>>(pk, len, j->iref, oc, desc[b].as<unsigned long long>(), counter, totals);
+      else join_probe_inline_staged_kernel<1><<<(int)ntl, kFusedThreads, 0, ctx->stream>>>(pk, len, j->iref, oc, desc[b].as<unsigned long long>(), counter, totals);
       DF_LAUNCH_CHECK(ctx);
     }
     DF_CUDA(cudaMemcpyAsync((char*)totals_host.ptr + i * 16, totals, 16, cudaMemcpyDeviceToHost, ctx->stream));

@@ -198,13 +198,13 @@ def test_gpu_large_join_properties(gpu_ctx):
     j.close()
 
 
-@pytest.mark.parametrize("n_slices", [2, 5, 8])
+@pytest.mark.parametrize("seed", [79, 82, 85])
 @pytest.mark.parametrize("with_payload", [True, False])
-def test_gpu_l2_sliced_probe_is_identical_to_single_pass(gpu_ctx, monkeypatch, n_slices, with_payload):
-    """The L2-sliced probe (slice passes + ordered emit, hash_join.cu) must give the reference's rows in the reference's
-    order exactly like the single-pass kernel: unique build keys, ~60 % hit rate, NULL probe keys, a ragged last tile and
-    several probe batches.  DFGPU_JOIN_SLICES forces the path on inputs far smaller than the L2."""
-    rng = np.random.default_rng(77 + n_slices)
+def test_gpu_ordered_inline_probe_keeps_reference_order(gpu_ctx, seed, with_payload):
+    """The single-pass ordered probe of the inline table (join_probe_inline_kernel, hash_join.cu) must give the reference's rows in
+    the reference's order: unique build keys, ~60 % hit rate, ~3 % NULL probe keys, a ragged last tile and several probe batches,
+    from device and from host input."""
+    rng = np.random.default_rng(seed)
     nb, npr = 30_000, 201_777
     bk = rng.permutation(100_000)[:nb].astype(np.int64) * 1_000_003 - 5
     build = [(bk, None), (rng.integers(-2**62, 2**62, nb).astype(np.int64), None)]
@@ -212,12 +212,12 @@ def test_gpu_l2_sliced_probe_is_identical_to_single_pass(gpu_ctx, monkeypatch, n
     probe = [(pk, rng.random(npr) > 0.03), (np.arange(npr, dtype=np.int64), None)]
     side, idx = ([0, 0, 1, 1], [0, 1, 0, 1]) if with_payload else ([0, 1, 1], [0, 0, 1])
     exp = O.hash_join(build, probe, [0], [0], side, idx, phj_threshold=0, phj_density=float("inf"))
-    monkeypatch.setenv("DFGPU_JOIN_SLICES", str(n_slices))
     for device in (True, False):
         got, h = gpu_hash_join(gpu_ctx, build, probe, [0], [0], side, idx, phj=(0, float("inf")), probe_batch_rows=70_001, device=device, return_handle=True)
         assert h.metric("array_map_created_count") == 0
+        assert h.metric("radix_partitioned_probes") == 0
         h.close()
-        assert_cols_equal(got, exp, ordered=True, what=f"sliced probe S={n_slices} payload={with_payload} device={device}")
+        assert_cols_equal(got, exp, ordered=True, what=f"ordered probe seed={seed} payload={with_payload} device={device}")
 
 
 def test_gpu_null_aware_validation(gpu_ctx):
