@@ -370,6 +370,15 @@ inline T read_scalar(dfgpu_ctx* ctx, const T* dptr) {
   return *h;
 }
 
+// Radix partition of n {key, val} rows (radix_probe.cuh, compiled once in hash_join.cu): 16-byte records grouped by the top hash bits of
+// the key, so that partition p holds exactly the keys of slot range [p cap / P, (p+1) cap / P) of any fastrange-addressed table
+// (slot = hi64(hash_u64(key, kSeedJoin) * cap)).  P = table_bytes / kRadixSubTableMB rounded up to a power of two in [2, kRadixMaxParts],
+// or force_parts when >= 2.  keys and vals 16-byte aligned; meta: kRadixMetaWords zeroed device words.  Returns log2(P).
+constexpr int kRadixSubTableMB = 16;   // table bytes per partition, a third of the 50 MB L2
+constexpr int kRadixMaxParts = 64, kRadixMetaWords = 3 * kRadixMaxParts + 1;
+int radix_partition(dfgpu_ctx* ctx, const unsigned long long* keys, const unsigned long long* vals, int64_t n, size_t table_bytes, int force_parts,
+                    void* out, unsigned long long* meta);
+
 // ------------------------------------------------------------------------------------------
 // device bit helpers (Arrow validity bitmaps are LSB-numbered)
 // ------------------------------------------------------------------------------------------

@@ -472,7 +472,6 @@ __global__ void __launch_bounds__(kFusedThreads) join_probe_fused_kernel(KeyCols
 // ------------------------------------------------------------------------------------------
 constexpr int kMaxPayloadCols = 8;
 constexpr int kInlineSlotsPer100Rows = 250;   // hashed inline table: 250 slots per 100 build rows
-constexpr int kRadixSubTableMB = 16;          // radix-partitioned probe: table bytes per partition, a third of the 50 MB L2
 struct PayloadCols { int n; const void* ptr[kMaxPayloadCols]; int width[kMaxPayloadCols]; int shift[kMaxPayloadCols]; };
 struct InlineRef { void* slots; uint64_t cap; int dense; uint64_t amin; int bucket; /* probe sequences start on a 4-slot boundary (one 64 B line for 16 B slots) */
                    const unsigned long long* bloom; uint64_t bloom_blocks; /* optional membership filter over the build keys (dfgpu_hashjoin_options.membership_filter) */ };
@@ -1415,30 +1414,15 @@ static void push_probe(dfgpu_hashjoin* j, std::vector<DCol>&& cols) {
         carry = src; ro.kind[c] = 1;
       }
       if (radix) {
-        int bits = 1;
-        const size_t want = force_parts >= 2 ? (size_t)force_parts : (tbytes + ((size_t)kRadixSubTableMB << 20) - 1) / ((size_t)kRadixSubTableMB << 20);
-        while ((1u << bits) < want && bits < 6) ++bits;
-        const int P = 1 << bits;
         const unsigned long long* keys = (const unsigned long long*)pk.ptr[0];
         const unsigned long long* vals = carry >= 0 ? (const unsigned long long*)cols[carry].values : keys;
-        DevBuf recs(ctx, (size_t)n * 16), meta(ctx, (size_t)(3 * kRadixMaxParts + 8) * 8);
+        DevBuf recs(ctx, (size_t)n * 16), meta(ctx, (size_t)(kRadixMetaWords + 2) * 8);
         meta.zero();
-        unsigned long long* counts = meta.as<unsigned long long>();
-        unsigned long long* cursor = counts + kRadixMaxParts;
-        unsigned long long* bounds = cursor + kRadixMaxParts;      // [P + 1]
-        unsigned long long* rtot = bounds + kRadixMaxParts + 1;    // output rows
+        unsigned long long* rtot = meta.as<unsigned long long>() + kRadixMetaWords;    // output rows
         unsigned int* rtile = (unsigned int*)(rtot + 1);
-        static bool attr_set = false;
-        if (!attr_set) { DF_CUDA(cudaFuncSetAttribute(radix_scatter_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kRadixTile * 8)); attr_set = true; }
         {
           KernelTimer kt(ctx, "radix_partition");
-          radix_hist_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(keys, n, bits, counts);
-          DF_LAUNCH_CHECK(ctx);
-          radix_prefix_kernel<<<1, 32, 0, ctx->stream>>>(counts, P, cursor, bounds);
-          DF_LAUNCH_CHECK(ctx);
-          const int64_t rtiles = (n + kRadixTile - 1) / kRadixTile;
-          radix_scatter_tma_kernel<<<(int)std::min<int64_t>(rtiles, kNumSMs * 3), kRadixThreads, 4 * kRadixTile * 8, ctx->stream>>>(keys, vals, n, bits, cursor, recs.as<RadixRec>());
-          DF_LAUNCH_CHECK(ctx);
+          radix_partition(ctx, keys, vals, n, tbytes, force_parts, recs.ptr, meta.as<unsigned long long>());
         }
         {
           KernelTimer kt(ctx, "join_probe");

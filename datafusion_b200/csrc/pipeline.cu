@@ -77,7 +77,8 @@ struct PipeParams {
   LookupDev target; int bkey_col, target_unique, n_bpay, bpay_src[kMaxBuildPay], bpay_shift[kMaxBuildPay], bpay_width[kMaxBuildPay];
   // aggregate sink (group id == record of stage `agg_stage`)
   int agg_stage, rows_word, n_aggs; AggDef agg[kMaxPipeAggs];
-  // unordered output sink
+  // unordered output sink; the partitioned aggregate sink (pipe_kernel VAR bit 128) writes its {key, value} records to out_dst[0] / out_dst[1],
+  // reserved through out_counter, at most target.cap of them
   int n_out, out_src[kMaxPipeCols], out_width[kMaxPipeCols]; void* out_dst[kMaxPipeCols]; unsigned long long* out_counter;
   ENode pool[kPoolNodes];
   // ring-fed phase A (pipe_kernel VAR bit 64): ring_stages > 0 when this batch qualifies (fill_params)
@@ -398,6 +399,9 @@ __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_
 //              TMA bulk copies in a ring of ring_stages warp tiles per warp in dynamic shared memory; lane 0 refills the ring S - 1 tiles
 //              ahead, so a warp in phase B keeps its next tiles in flight.  Phase B loads agg[0]'s column operands of the whole round
 //              before evaluating (replaces bit 0).  Blocks per SM and ring sizes: ring_smem.  Chosen by launch_pipe, not by DFGPU_PIPE_VAR.
+//   bit 7 (128) partitioned aggregate (with bit 6; pipeline_push decides, partitioned_parts): the aggregate stage's table exceeds L2, so
+//              phase B makes no lookup — it writes each survivor's {key, SUM argument} to the record buffer (out_dst, out_counter), and
+//              pipe_probe_agg_kernel probes them once they are radix-partitioned.  Rows past the buffer's end probe and RED right here.
 // DFGPU_PIPE_VAR selects the instantiation (aggregate sink; bits 1 and 5 also for the pack sink, bit 1 for the unordered-output sink); 0 is the
 // kernel without any of them, 11 the default.  Tried and removed: four instead of two survivors per lane and phase-B round; prefetching the
 // table record and the argument sectors already when a row passes the membership filter in phase A (the prefetches of five tiles queue up
@@ -530,7 +534,7 @@ __device__ __forceinline__ void dense_reduce_peers(unsigned peers, int op, unsig
 template <int SINK, bool DEC, int VAR = 0>
 __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PACK) || SINK == SINK_DENSE) ? 2 : 3) pipe_kernel(const PipeParams* __restrict__ gp, int64_t n, unsigned long long* __restrict__ counters /* [alive, inserted, fail, err] */) {
   constexpr int PB = kPhaseB, PBG = kPhaseBGroup, QC = kQueueCap;
-  constexpr bool RING = (VAR & 64) != 0;
+  constexpr bool RING = (VAR & 64) != 0, PART = (VAR & 128) != 0;
   __shared__ PipeParams sp;
   __shared__ uint32_t q_rows[kPipeWarps][QC];
   extern __shared__ __align__(128) unsigned char dyn_smem[];   // RING: mbarriers [warp][stage], then the rings [warp][stage][ring_bytes]
@@ -749,12 +753,12 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
       const unsigned int qbase = qn - take;   // consume from the tail: nothing has to move
       bool live[PB];
       int64_t row[PB];
-      uint64_t pay[kMaxStages][PB];
+      uint64_t pay[kMaxStages][PB], pkey[PB];   // pkey: PART, the aggregate stage's key
       unsigned long long* arec[PB];
 #pragma unroll
       for (int u = 0; u < PB; ++u) {
         const unsigned int e = u * 32 + lane;
-        live[u] = e < take; row[u] = live[u] ? (int64_t)q_row[qbase + e] : 0; arec[u] = nullptr;
+        live[u] = e < take; row[u] = live[u] ? (int64_t)q_row[qbase + e] : 0; arec[u] = nullptr; pkey[u] = 0;
       }
       if ((VAR & 1) && SINK == SINK_AGG) {
 #pragma unroll 1
@@ -800,11 +804,16 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
             if ((kc.valid && !bit_get(kc.valid, kc.voff + row[u])) || key[u] == kEmptyKey) look[u] = false;   // NULL keys never match
           }
           slot[u] = __umul64hi(lk_hash(key[u]), st.lk.cap); ck[u] = kEmptyKey; cp[u] = 0;
-          if (look[u]) {
+          if (look[u] && !PART) {
             const unsigned long long* r = st.lk.recs + slot[u] * (uint64_t)st.lk.stride;
             if (st.lk.has_payload) { const uint4 v = __ldcg((const uint4*)r); ck[u] = (uint64_t)v.x | ((uint64_t)v.y << 32); cp[u] = (uint64_t)v.z | ((uint64_t)v.w << 32); }
             else ck[u] = __ldcg(r);
           }
+        }
+        if (PART) {   // the aggregate stage, the only hash stage here: resolved by pipe_probe_agg_kernel (or the sink's fallback below)
+#pragma unroll
+          for (int u = 0; u < PB; ++u) { pkey[u] = key[u]; live[u] = look[u]; }
+          continue;
         }
 #pragma unroll
         for (int u = 0; u < PB; ++u) {
@@ -853,6 +862,39 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
         }
       }
       bool sunk = false;
+      if (PART && SINK == SINK_AGG) {
+        // {key, value} records through one reservation per warp and round; no table access.  A Bloom false positive costs one record
+        // (its key finds no partner later).  Reservations past the buffer's end (target.cap records) probe and RED here instead.
+        sunk = true;
+        const AggDef& ag0 = sp.agg[0];
+        unsigned int tot = 0, mypos[PB];
+#pragma unroll
+        for (int u = 0; u < PB; ++u) { const unsigned m = __ballot_sync(0xffffffffu, live[u]); mypos[u] = tot + __popc(m & ((1u << lane) - 1u)); tot += __popc(m); }
+        unsigned long long obase = 0;
+        if (lane == 0 && tot) obase = atomicAdd(sp.out_counter, (unsigned long long)tot);
+        obase = __shfl_sync(0xffffffffu, obase, 0);
+#pragma unroll
+        for (int u = 0; u < PB; ++u) {
+          if (!live[u]) continue;
+          const uint64_t ext[kMaxStages] = {0, 0, 0};   // the program reads no payload field (partitioned_parts)
+          const unsigned long long v = eval_int_gathered(sp.pool + ag0.start, ag0.n, row[u], ext, sp.n_gather, g[0][u], g[1][u]);
+          const unsigned long long o = obase + mypos[u];
+          if (o < sp.target.cap) {
+            ((unsigned long long*)sp.out_dst[0])[o] = pkey[u];
+            ((unsigned long long*)sp.out_dst[1])[o] = v;
+            continue;
+          }
+          const LookupDev& lk = sp.stage[sp.agg_stage].lk;
+          uint64_t slot = __umul64hi(lk_hash(pkey[u]), lk.cap);
+          while (true) {
+            unsigned long long* r = lk.recs + slot * (uint64_t)lk.stride;
+            const unsigned long long ck = __ldcg(r);
+            if (ck == pkey[u]) { red_add_u64(r + sp.rows_word, 1ull); red_add_u64(r + ag0.word, v); alive_cnt++; break; }
+            if (ck == kEmptyKey) break;
+            if (++slot == lk.cap) slot = 0;
+          }
+        }
+      }
       if ((VAR & 8) && SINK == SINK_AGG) {
         // one RED instruction per lane PAIR and row: the row counter and the sum word of a record share a sector, so the even lane adds
         // its row's count while the odd neighbour adds the same row's value (then the roles swap) — half the L2 reduction requests
@@ -1088,6 +1130,69 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
     if (s_flag[0]) atomicOr(&counters[2], (unsigned long long)s_flag[0]);
     if (s_flag[1]) atomicOr(&counters[3], (unsigned long long)s_flag[1]);
   }
+}
+
+// ------------------------------------------------------------------------------------------
+// partitioned aggregate, second half: the {key, value} records of pipe_kernel VAR bit 128, radix-partitioned (radix_partition), probe the
+// aggregate stage's table and RED into the matched record.  Tiles are taken in record order from one counter, so the running blocks
+// share one ~16 MB slot range of the table and its lookups and REDs are L2 hits instead of DRAM misses (radix_probe_kernel's scheme).
+// Matches add to counters[0], the sink's row count.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) pipe_probe_agg_kernel(const ulonglong2* __restrict__ recs, int64_t n, LookupDev t, int rows_word, int sum_word,
+                                                             unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ counters) {
+  constexpr int ITEMS = 4, TILE = 256 * ITEMS;
+  __shared__ unsigned int s_tile;
+  const int lane = threadIdx.x & 31;
+  const bool even = !(lane & 1);
+  const int64_t ntiles = (n + TILE - 1) / TILE;
+  unsigned int hits = 0;
+  while (true) {
+    __syncthreads();
+    if (threadIdx.x == 0) s_tile = atomicAdd(tile_counter, 1u);   // tiles in record order: the running blocks share one sub-table
+    __syncthreads();
+    const int64_t tile = s_tile;
+    if (tile >= ntiles) break;
+    unsigned long long key[ITEMS], val[ITEMS], slot[ITEMS], cur[ITEMS];
+    unsigned pend = 0, hit = 0;
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const int64_t i = tile * TILE + k * 256 + threadIdx.x;
+      key[k] = kEmptyKey; val[k] = 0; cur[k] = kEmptyKey;
+      if (i < n) { const int4 r = ld_stream_16(recs + i); key[k] = (uint64_t)(uint32_t)r.x | ((uint64_t)(uint32_t)r.y << 32); val[k] = (uint64_t)(uint32_t)r.z | ((uint64_t)(uint32_t)r.w << 32); }
+      slot[k] = __umul64hi(lk_hash(key[k]), t.cap);
+      if (i < n) { cur[k] = __ldcg(t.recs + slot[k] * (uint64_t)t.stride); pend |= 1u << k; }
+    }
+    // lockstep linear probing: the (rare) second probes of the thread's rows overlap
+    while (pend) {
+#pragma unroll
+      for (int k = 0; k < ITEMS; ++k) {
+        if (!((pend >> k) & 1u)) continue;
+        if (cur[k] == key[k]) { hit |= 1u << k; pend &= ~(1u << k); }
+        else if (cur[k] == kEmptyKey) pend &= ~(1u << k);
+        else {
+          if (++slot[k] == t.cap) slot[k] = 0;
+          cur[k] = __ldcg(t.recs + slot[k] * (uint64_t)t.stride);
+        }
+      }
+    }
+    // lane-paired REDs (pipe_kernel VAR bit 3): the even lane adds its row's count while the odd neighbour adds the same row's value
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const bool h = (hit >> k) & 1u;
+      hits += h ? 1u : 0u;
+      const unsigned long long rp = h ? (unsigned long long)(t.recs + slot[k] * (uint64_t)t.stride) : 0ull;
+      const unsigned long long prp = __shfl_xor_sync(0xffffffffu, rp, 1);
+      const unsigned long long pv = __shfl_xor_sync(0xffffffffu, val[k], 1);
+      const bool pl = __shfl_xor_sync(0xffffffffu, h ? 1 : 0, 1) != 0;
+      unsigned long long* const mine = (unsigned long long*)rp + rows_word;
+      unsigned long long* const theirs = (unsigned long long*)prp + sum_word;
+      if (even ? h : pl) red_add_u64(even ? mine : theirs, even ? 1ull : pv);
+      if (even ? pl : h) red_add_u64(even ? theirs : mine, even ? pv : 1ull);
+    }
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) hits += __shfl_xor_sync(0xffffffffu, hits, d);
+  if (lane == 0 && hits) atomicAdd(&counters[0], (unsigned long long)hits);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1436,7 +1541,7 @@ struct dfgpu_pipeline {
   bool finished = false;
   DevBuf params_dev, counters;
   std::deque<BatchPtr> outq;
-  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0, m_dense_block_launches = 0;
+  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0, m_dense_block_launches = 0, m_partitioned_launches = 0;
   std::string name;   // optional label: the kernel-timing family becomes "pipe:<name>" (dfgpu_kernel_time)
 };
 
@@ -1680,7 +1785,7 @@ static void check_errors(unsigned long long err) {
 }
 
 template <int SINK>
-static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, const char* timer_name) {
+static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, const char* timer_name, bool part = false) {
   dfgpu_ctx* ctx = p->ctx;
   const int64_t ntiles = (n + kPipeTile - 1) / kPipeTile;
   // programs that touch Decimal128 values run a second instantiation of the kernel (128-bit interpreter linked in): the integer
@@ -1692,18 +1797,21 @@ static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, cons
   const std::string tname = p->name.empty() ? std::string(timer_name) : "pipe:" + p->name;
   if constexpr (SINK == SINK_AGG || SINK == SINK_PACK) if (!dec && pp.ring_stages > 0 && !getenv("DFGPU_PIPE_VAR")) {
     constexpr int RV = SINK == SINK_AGG ? 64 | 8 : 64;   // ring + lane-paired REDs for the aggregate sink, ring alone for the pack sink
+    // the partitioned aggregate: ring + records instead of lookups
+    void (*kern)(const PipeParams*, int64_t, unsigned long long*) = SINK == SINK_AGG && part ? pipe_kernel<SINK_AGG, false, 64 | 128> : pipe_kernel<SINK, false, RV>;
     const int smem = kRingBarBytes + kPipeWarps * pp.ring_stages * pp.ring_bytes;
     // the attribute belongs to the current device: set on every launch (a host-side call), so any device and thread may launch
-    DF_CUDA(cudaFuncSetAttribute(pipe_kernel<SINK, false, RV>, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingBarBytes + ring_smem(SINK)));
+    DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kRingBarBytes + ring_smem(SINK)));
     int blocks_per_sm = 0;
-    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, pipe_kernel<SINK, false, RV>, kPipeThreads, smem));
+    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, smem));
     const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
     KernelTimer kt(ctx, tname.c_str());
-    pipe_kernel<SINK, false, RV><<<grid, kPipeThreads, smem, ctx->stream>>>(gp, n, cnt);
+    kern<<<grid, kPipeThreads, smem, ctx->stream>>>(gp, n, cnt);
     DF_LAUNCH_CHECK(ctx);
     p->m_ring_launches++;
     return;
   }
+  DF_CHECK(!part, DFGPU_ERR_INVALID, "internal: the partitioned aggregate needs the ring-fed pipeline kernel");
   static const int blocks_env = getenv("DFGPU_PIPE_BLOCKS_PER_SM") ? atoi(getenv("DFGPU_PIPE_BLOCKS_PER_SM")) : 0;
   int blocks_per_sm = blocks_env;
   if (blocks_per_sm <= 0) {   // persistent blocks: exactly one resident wave (a second wave would start after the first finished)
@@ -1842,6 +1950,25 @@ static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DensePar
   if (!dp.per_warp) p->m_dense_block_launches++;
 }
 
+// The partitioned aggregate (pipe_kernel VAR bit 128, then radix_partition and pipe_probe_agg_kernel) trades phase B's dependent DRAM
+// lookup + RED per survivor for streamed records and L2-resident probes.  It serves a batch that takes the ring kernel, whose aggregate
+// stage is the only hash stage phase B probes and exceeds L2 (the rule that gives it a Bloom filter), with one integer SUM over this
+// batch's columns: no payload field, no NULLs, no non-null counter — TPC-H Q3 over Int64 money.  Returns the stage's table bytes, 0 when
+// the batch keeps the direct probe.  force_parts >= 2 (a test hook) admits tables of any size.
+static size_t partitioned_table_bytes(const dfgpu_pipeline* p, const PipeParams& pp, int force_parts) {
+  if (pp.ring_stages == 0 || pipeline_has_decimal(p) || getenv("DFGPU_PIPE_VAR")) return 0;   // launch_pipe's ring kernel runs
+  if (pp.agg_stage < 0) return 0;
+  for (int s = 0; s < pp.n_stages; ++s)
+    if (s != pp.agg_stage && pp.stage[s].lk.mode == LK_HASH && pp.stage[s].kind != kStageMaybe) return 0;
+  const StageDev& st = pp.stage[pp.agg_stage];
+  if (st.kind != DFGPU_STAGE_INNER || st.lk.mode != LK_HASH || st.lk.cap == 0) return 0;
+  const AggDef& a = pp.agg[0];
+  if (pp.n_aggs != 1 || a.small != 2 || a.func != DFGPU_AGG_SUM || a.cls == C_F64 || a.cls == C_DEC || a.nn_word >= 0) return 0;
+  for (int i = 0; i < a.n; ++i) if (pp.pool[a.start + i].kind == kExprExt) return 0;
+  const size_t bytes = (size_t)st.lk.cap * st.lk.stride * 8;
+  return bytes > (40ull << 20) || force_parts >= 2 ? bytes : 0;
+}
+
 static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   DF_CHECK(!p->finished, DFGPU_ERR_STATE, "push after finish");
   DF_CHECK(p->sink != SINK_NONE, DFGPU_ERR_STATE, "pipeline: choose a sink before the first push");
@@ -1903,9 +2030,44 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   } else if (p->sink == SINK_AGG) {
     prepare_acc(p);
     fill_params(p, cols, &pp);
+    // test hooks: DFGPU_PIPE_RADIX_PARTS forces the partition count (and the partitioned path on small tables), DFGPU_PIPE_RADIX_CAP the
+    // record buffer's capacity
+    const int force_parts = getenv("DFGPU_PIPE_RADIX_PARTS") ? atoi(getenv("DFGPU_PIPE_RADIX_PARTS")) : 0;
+    const size_t part_bytes = partitioned_table_bytes(p, pp, force_parts);
+    DevBuf rkeys, rvals, recs, meta;   // released after read_counters' synchronise
+    if (part_bytes) {
+      // survivors are a fraction of the rows (Q3: ~5 %); the buffer holds one in eight, rows past it take the in-kernel fallback
+      int64_t cap = std::min<int64_t>(n, std::max<int64_t>(n / 8, 1 << 20));
+      if (getenv("DFGPU_PIPE_RADIX_CAP")) cap = std::min<int64_t>(cap, atoll(getenv("DFGPU_PIPE_RADIX_CAP")));
+      cap = std::max<int64_t>(cap, 1);
+      rkeys.alloc(ctx, (size_t)cap * 8); rvals.alloc(ctx, (size_t)cap * 8);
+      pp.out_dst[0] = rkeys.ptr; pp.out_dst[1] = rvals.ptr; pp.out_counter = p->counters.as<unsigned long long>() + 4; pp.target.cap = (uint64_t)cap;
+    }
     upload_params(p, pp);
     p->counters.zero();
-    launch_pipe<SINK_AGG>(p, pp, n, "pipeline_agg");
+    launch_pipe<SINK_AGG>(p, pp, n, "pipeline_agg", part_bytes != 0);
+    if (part_bytes) {
+      unsigned long long h8[8];
+      DF_CUDA(cudaMemcpyAsync(h8, p->counters.ptr, 64, cudaMemcpyDeviceToHost, ctx->stream));
+      DF_CUDA(cudaStreamSynchronize(ctx->stream));
+      check_errors(h8[3]);
+      const int64_t m = std::min<int64_t>((int64_t)h8[4], (int64_t)pp.target.cap);
+      if (m > 0) {
+        recs.alloc(ctx, (size_t)m * 16); meta.alloc(ctx, (size_t)(kRadixMetaWords + 1) * 8);
+        meta.zero();
+        {
+          KernelTimer kt(ctx, "pipe_partition");
+          radix_partition(ctx, rkeys.as<unsigned long long>(), rvals.as<unsigned long long>(), m, part_bytes, force_parts, recs.ptr, meta.as<unsigned long long>());
+        }
+        {
+          KernelTimer kt(ctx, "pipe_probe_agg");
+          pipe_probe_agg_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(recs.as<ulonglong2>(), m, pp.stage[pp.agg_stage].lk, pp.rows_word, pp.agg[0].word,
+                                                                      (unsigned int*)(meta.as<unsigned long long>() + kRadixMetaWords), p->counters.as<unsigned long long>());
+          DF_LAUNCH_CHECK(ctx);
+        }
+      }
+      p->m_partitioned_launches++;
+    }
     read_counters(p, h);
     check_errors(h[3]);
     p->m_sink_rows += (int64_t)h[0];
@@ -2573,6 +2735,7 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name) {
   if (s == "num_groups") return p->m_groups;
   if (s == "ring_launches") return p->m_ring_launches;   // launches of the ring-fed pipeline kernel
   if (s == "dense_block_launches") return p->m_dense_block_launches;   // dense sink launches with one accumulator copy per block (shared atomics)
+  if (s == "partitioned_launches") return p->m_partitioned_launches;   // aggregate sink pushes probed from radix-partitioned records
   return -1;
 }
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p) {

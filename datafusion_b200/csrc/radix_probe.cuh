@@ -1,4 +1,5 @@
-// radix_probe.cuh — intra-GPU radix-partitioned probe of the inline join table (included by hash_join.cu).
+// radix_probe.cuh — intra-GPU radix-partitioned probe of the inline join table (included by hash_join.cu only; radix_partition, declared
+// in common.cuh, also partitions the probe records of the fused pipeline's aggregate sink, pipeline.cu).
 //
 // Reference analogue: PartitionMode::Partitioned — both join inputs go through BatchPartitioner::Hash
 // (physical-plan/src/repartition/mod.rs:1097-1145) so that every partition's hash table is small enough to stay in
@@ -21,7 +22,7 @@
 
 namespace dfgpu {
 
-constexpr int kRadixTile = 2048, kRadixThreads = 256, kRadixPerThread = kRadixTile / kRadixThreads, kRadixMaxParts = 64;
+constexpr int kRadixTile = 2048, kRadixThreads = 256, kRadixPerThread = kRadixTile / kRadixThreads;   // kRadixMaxParts: common.cuh
 
 __device__ __forceinline__ int radix_part(uint64_t key, int bits) { return (int)(hash_u64(key, kSeedJoin) >> (64 - bits)); }
 
@@ -129,6 +130,27 @@ __global__ void __launch_bounds__(kRadixThreads) radix_scatter_tma_kernel(const 
     __syncthreads();
     if (threadIdx.x == 0) issue(tile + 2 * (int64_t)gridDim.x, s);   // refill this stage two tiles ahead
   }
+}
+
+// hist -> prefix -> TMA scatter (declared in common.cuh: the fused pipeline's aggregate sink partitions its probe records here too)
+int radix_partition(dfgpu_ctx* ctx, const unsigned long long* keys, const unsigned long long* vals, int64_t n, size_t table_bytes, int force_parts,
+                    void* out, unsigned long long* meta) {
+  int bits = 1;
+  const size_t want = force_parts >= 2 ? (size_t)force_parts : (table_bytes + ((size_t)kRadixSubTableMB << 20) - 1) / ((size_t)kRadixSubTableMB << 20);
+  while ((1u << bits) < want && bits < 6) ++bits;
+  unsigned long long* counts = meta;
+  unsigned long long* cursor = counts + kRadixMaxParts;
+  unsigned long long* bounds = cursor + kRadixMaxParts;      // [P + 1]
+  // the attribute belongs to the current device: set on every call, so any device and thread may partition
+  DF_CUDA(cudaFuncSetAttribute(radix_scatter_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kRadixTile * 8));
+  radix_hist_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(keys, n, bits, counts);
+  DF_LAUNCH_CHECK(ctx);
+  radix_prefix_kernel<<<1, 32, 0, ctx->stream>>>(counts, 1 << bits, cursor, bounds);
+  DF_LAUNCH_CHECK(ctx);
+  const int64_t rtiles = (n + kRadixTile - 1) / kRadixTile;
+  radix_scatter_tma_kernel<<<(int)std::min<int64_t>(rtiles, kNumSMs * 3), kRadixThreads, 4 * kRadixTile * 8, ctx->stream>>>(keys, vals, n, bits, cursor, (RadixRec*)out);
+  DF_LAUNCH_CHECK(ctx);
+  return bits;
 }
 
 struct RadixOut {

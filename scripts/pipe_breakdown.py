@@ -49,10 +49,13 @@ for name, mk in variants.items():
         for b in p.drain(host=False):
             b.release()
         t, n_ = ctx.kernel_time("pipe:v")
-        rows = p.metric("sink_rows")
+        # the partitioned aggregate (a table larger than L2: B2, B3): pass 1 is "pipe:v", then the partition and the probe-aggregate kernels
+        tp, _ = ctx.kernel_time("pipe_partition"); ta, _ = ctx.kernel_time("pipe_probe_agg")
+        rows, part = p.metric("sink_rows"), p.metric("partitioned_launches")
         p.close()
         if it:
-            ms.append(t / max(n_, 1))
-    out[name] = {"kernel_ms": round(min(ms), 3), "sink_rows": rows}
-    print(f"{name:75s} {min(ms):7.3f} ms   sink rows {rows}", flush=True)
+            ms.append((t / max(n_, 1), tp, ta))
+    best = min(ms, key=lambda m: sum(m))
+    out[name] = {"kernel_ms": round(best[0], 3), "partition_ms": round(best[1], 3), "probe_agg_ms": round(best[2], 3), "partitioned": part, "sink_rows": rows}
+    print(f"{name:75s} {best[0]:7.3f} ms" + (f" + partition {best[1]:.3f} + probe-aggregate {best[2]:.3f} ms" if part else "") + f"   sink rows {rows}", flush=True)
 json.dump(out, open("gpurun_out/r2_pipe_breakdown.json", "w"), indent=1)
