@@ -855,7 +855,7 @@ struct dfgpu_hashjoin {
   std::deque<BatchPtr> outq;
   // metrics (BuildProbeJoinMetrics, joins/utils.rs:1756-1778)
   int64_t m_build_rows = 0, m_build_batches = 0, m_input_rows = 0, m_input_batches = 0, m_output_rows = 0, m_output_batches = 0,
-          m_array_map = 0, m_probe_hits = 0, m_radix_probes = 0;
+          m_array_map = 0, m_probe_hits = 0, m_radix_probes = 0, m_pipelined_probes = 0;
   // wide keys (> 64 bits together, or a 16-byte Decimal128 key): the table is keyed by a 64-bit hash of the key columns (a hidden INT64
   // column appended to both sides) and key equality becomes a conjunct of the JoinFilter — the reference's own scheme: lookup by hash,
   // then equal_rows_arr on the candidate pairs (joins/utils.rs:2191-2257, hash_join/stream.rs lookup_join_hashmap)
@@ -1681,6 +1681,7 @@ static bool push_probe_host_pipelined(dfgpu_hashjoin* j, const dfgpu_column* hco
   j->m_input_rows += n;
   j->m_input_batches++;
   j->m_probe_hits += hits;
+  j->m_pipelined_probes++;
   j->probe_side_non_empty = true;
   if (out_rows > 0) emit_batch(j, std::move(hb));
   return true;
@@ -1902,10 +1903,11 @@ int dfgpu_hashjoin_next(dfgpu_hashjoin* j, int host, dfgpu_batch** out) {
   try {
     DF_CHECK(j && out, DFGPU_ERR_INVALID, "null argument");
     if (j->outq.empty()) { *out = nullptr; return DFGPU_END; }
+    // checked before the batch leaves the queue: a refused call must not lose its rows
+    DF_CHECK(host || !j->outq.front()->host, DFGPU_ERR_STATE, "this batch was produced on the host (pipelined host probe): call next(host=1)");
     BatchPtr b = std::move(j->outq.front());
     j->outq.pop_front();
     if (host && !b->host) { set_device(j->ctx); b = to_host_batch(j->ctx, *b); }
-    DF_CHECK(host || !b->host, DFGPU_ERR_STATE, "this batch was produced on the host (pipelined host probe): call next(host=1)");
     *out = b.release();
     return DFGPU_OK;
   } catch (const dfgpu::Error& e) { if (_ctx) _ctx->last_error = e.what(); return e.code; }
@@ -1923,6 +1925,7 @@ int64_t dfgpu_hashjoin_metric(dfgpu_hashjoin* j, const char* name) {
   if (s == "array_map_created_count") return j->m_array_map;
   if (s == "probe_hits") return j->m_probe_hits;
   if (s == "radix_partitioned_probes") return j->m_radix_probes;
+  if (s == "pipelined_host_probes") return j->m_pipelined_probes;   // host pushes probed by push_probe_host_pipelined
   if (s == "membership_filter_bytes") return (int64_t)j->bloom.bytes;
   if (s == "build_distinct_keys") return j->distinct;
   if (s == "build_unique") return j->unique ? 1 : 0;

@@ -325,8 +325,12 @@ int dfgpu_hashjoin_push_probe_host(dfgpu_hashjoin* j, const dfgpu_column* cols, 
 int dfgpu_hashjoin_push_probe_device(dfgpu_hashjoin* j, const dfgpu_column* cols, int32_t n_cols);
 int dfgpu_hashjoin_push_probe_arrow(dfgpu_hashjoin* j, const struct ArrowArray* batch, const struct ArrowSchema* schema);
 int dfgpu_hashjoin_finish_probe(dfgpu_hashjoin* j);  /* ExhaustedProbeSide → process_unmatched_build_batch, stream.rs:1002 */
+/* A host push probed by the pipelined host probe (see "pipelined_host_probes") yields a host batch: next with host = 0 returns
+ * DFGPU_ERR_STATE for it and leaves it queued for next with host = 1. */
 int dfgpu_hashjoin_next(dfgpu_hashjoin* j, int host, dfgpu_batch** out);
-/* "build_input_rows","input_rows","output_rows","array_map_created_count","probe_hits" … (joins/utils.rs:1756-1778, exec.rs:108) */
+/* "build_input_rows","input_rows","output_rows","array_map_created_count","probe_hits","radix_partitioned_probes",
+ * "pipelined_host_probes" (host pushes of >= 16 Mi rows probed chunk by chunk with overlapped copies) …
+ * (joins/utils.rs:1756-1778, exec.rs:108) */
 int64_t dfgpu_hashjoin_metric(dfgpu_hashjoin* j, const char* name);
 void dfgpu_hashjoin_destroy(dfgpu_hashjoin* j);
 
@@ -497,7 +501,7 @@ int dfgpu_pipeline_push_device(dfgpu_pipeline* p, const dfgpu_column* cols, int3
 int dfgpu_pipeline_push_arrow(dfgpu_pipeline* p, const struct ArrowArray* batch, const struct ArrowSchema* schema);
 int dfgpu_pipeline_finish(dfgpu_pipeline* p);
 int dfgpu_pipeline_next(dfgpu_pipeline* p, int host, dfgpu_batch** out);
-int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches","dense_block_launches" */
+int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches","dense_block_launches","partitioned_launches" */
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p);
 
 /* ===================================================================================== */
