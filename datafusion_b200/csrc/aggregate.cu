@@ -29,7 +29,7 @@ constexpr int kMaxAggs = 8;
 constexpr int kMaxProbe = 512;
 constexpr uint64_t kEmptyKey = 0xFFFFFFFFFFFFFFFFull;
 
-struct alignas(16) Key2 { unsigned long long lo, hi; };
+using Key2 = Rec128;   // a group key of up to 128 bits, or a Decimal128 accumulator pair (expr_dec.cuh)
 
 struct GroupCols {
   int n;
@@ -189,36 +189,12 @@ __host__ __device__ __forceinline__ double ordered_to_f64(uint64_t u) {
   return d;
 }
 
-__device__ __forceinline__ Key2 cas128(Key2* addr, Key2 cmp, Key2 val) {
-  Key2 old;
-  asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.global.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
-               : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
-  return old;
-}
-// a slot's Decimal128 {lo, hi} pair in one 128-bit access: never a mix of two CAS results
-__device__ __forceinline__ Key2 ld_pair(const Key2* addr) {
-  Key2 v;
-  asm volatile("{\n\t.reg .b128 t;\n\tld.relaxed.gpu.global.b128 t, [%2];\n\tmov.b128 {%0, %1}, t;\n\t}" : "=l"(v.lo), "=l"(v.hi) : "l"(addr) : "memory");
-  return v;
-}
-__device__ __forceinline__ bool lt_i128(Key2 a, Key2 b) { return (long long)a.hi < (long long)b.hi || (a.hi == b.hi && a.lo < b.lo); }
 // i128 add_wrapping as two 64-bit atomics: the carry out of the low word is a function of this add alone (old + lo overflowed), so the
 // high words sum to the right value in any interleaving
 __device__ __forceinline__ void add_i128(unsigned long long* lo_word, unsigned long long* hi_word, unsigned long long lo, unsigned long long hi) {
   const unsigned long long old = atomicAdd(lo_word, lo);
   const unsigned long long carry = (old + lo) < old ? 1ull : 0ull;
   if (hi + carry) atomicAdd(hi_word, hi + carry);
-}
-// Decimal128 MIN / MAX of the value at p into the slot w, signed i128 order.  Once a group has a few rows most values are not better than
-// the slot: one load, no atomic.  The load is one 128-bit access and the slot only ever improves, so "not better" than it is final.
-__device__ __forceinline__ void minmax_i128(Key2* w, const unsigned long long* p, bool is_min) {
-  const Key2 v{p[0], p[1]};
-  Key2 cur = ld_pair(w);
-  while (is_min ? lt_i128(v, cur) : lt_i128(cur, v)) {
-    const Key2 prev = cas128(w, cur, v);
-    if (prev.lo == cur.lo && prev.hi == cur.hi) break;
-    cur = prev;
-  }
 }
 
 // PAIR: the aggregate set has a Decimal128 MIN / MAX / AVG ({lo, hi} pair accumulators).  Only those update kernels compile their
@@ -252,7 +228,11 @@ __device__ __forceinline__ void apply_agg(const AggDev& a, int64_t row, uint64_t
     case DFGPU_AGG_MIN:
     case DFGPU_AGG_MAX: {
       const bool is_min = a.func == DFGPU_AGG_MIN;
-      if (PAIR && a.cls == 3) minmax_i128((Key2*)a.acc0 + slot, (const unsigned long long*)a.in0 + 2 * row, is_min);
+      if (PAIR && a.cls == 3) {
+        Key2* w = (Key2*)a.acc0 + slot;
+        const unsigned long long* p = (const unsigned long long*)a.in0 + 2 * row;
+        minmax_i128(w, Key2{p[0], p[1]}, is_min);
+      }
       else if (a.cls == 0) {
         long long v = load_as_i64(a.in0, a.in0_type, row);
         if (is_min) atomicMin((long long*)&a.acc0[slot], v); else atomicMax((long long*)&a.acc0[slot], v);

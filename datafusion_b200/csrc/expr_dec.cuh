@@ -55,6 +55,39 @@ __device__ __forceinline__ bool mul_ovf128(i128 a, i128 b, i128* r) {
 }
 __device__ __forceinline__ bool is_min128(i128 a) { return (u128)a == ((u128)1 << 127); }
 
+// ---- 16-byte {lo, hi} pairs in memory: Decimal128 accumulators (and 128-bit keys / record heads), always accessed as ONE 128-bit unit ----
+struct alignas(16) Rec128 { unsigned long long lo, hi; };
+// 128-bit compare-and-swap on a global address; GENERIC: on a generic one (shared memory as well)
+template <bool GENERIC = false>
+__device__ __forceinline__ Rec128 cas128(void* addr, Rec128 cmp, Rec128 val) {
+  Rec128 old;
+  if constexpr (GENERIC)
+    asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
+                 : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
+  else
+    asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.global.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
+                 : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
+  return old;
+}
+// a {lo, hi} pair in global memory in one 128-bit access: never a mix of two CAS results
+__device__ __forceinline__ Rec128 ld_pair(const void* addr) {
+  Rec128 v;
+  asm volatile("{\n\t.reg .b128 t;\n\tld.relaxed.gpu.global.b128 t, [%2];\n\tmov.b128 {%0, %1}, t;\n\t}" : "=l"(v.lo), "=l"(v.hi) : "l"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ bool lt_i128(Rec128 a, Rec128 b) { return (long long)a.hi < (long long)b.hi || (a.hi == b.hi && a.lo < b.lo); }
+// Decimal128 MIN / MAX of v into the 16-byte aligned pair at w (global memory), signed i128 order.  Once a group has a few rows most
+// values are not better than the pair: one load, no atomic.  The load is one 128-bit access and the pair only ever improves, so "not
+// better" than it is final (a torn read could show a value below anything ever stored and skip a needed update).
+__device__ __forceinline__ void minmax_i128(void* w, Rec128 v, bool is_min) {
+  Rec128 cur = ld_pair(w);
+  while (is_min ? lt_i128(v, cur) : lt_i128(cur, v)) {
+    const Rec128 prev = cas128(w, cur, v);
+    if (prev.lo == cur.lo && prev.hi == cur.hi) break;
+    cur = prev;
+  }
+}
+
 __device__ __forceinline__ i128 load_dec(const void* col, int64_t row) {
   const unsigned long long* p = (const unsigned long long*)col + 2 * row;   // 8-byte aligned is all Arrow promises for a sliced buffer
   return (i128)(((u128)p[1] << 64) | (u128)p[0]);

@@ -102,14 +102,6 @@ __device__ __forceinline__ unsigned long long ld_keep_u64(const unsigned long lo
   unsigned long long v; asm volatile("ld.global.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
 }
 
-struct alignas(16) Rec128 { unsigned long long lo, hi; };
-__device__ __forceinline__ Rec128 rec_cas128(void* addr, Rec128 cmp, Rec128 val) {
-  Rec128 old;
-  asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.global.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
-               : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
-  return old;
-}
-
 __device__ __forceinline__ uint64_t lk_hash(uint64_t key) { return hash_u64(key, kSeedJoin); }
 // Coarse first level for filters that do not fit L2 (a join's filter shared by 4-8 GPUs is hundreds of MB): 4 bits per key, two probe
 // bits in one 32-bit word.  It stays L2-resident and rejects ~85 % of the keys without a partner, so only ~1 probe in 4 pays the DRAM
@@ -148,7 +140,7 @@ __device__ __forceinline__ int lk_insert(const LookupDev& t, uint64_t key, uint6
   while (true) {
     unsigned long long* r = t.recs + s * (uint64_t)t.stride;
     unsigned long long prev;
-    if (t.has_payload) prev = rec_cas128(r, Rec128{kEmptyKey, 0ull}, Rec128{key, pay}).lo;
+    if (t.has_payload) prev = cas128(r, Rec128{kEmptyKey, 0ull}, Rec128{key, pay}).lo;
     else prev = atomicCAS(r, (unsigned long long)kEmptyKey, (unsigned long long)key);
     if (prev == kEmptyKey) break;
     if (prev == key) { rc = 1; break; }
@@ -270,6 +262,16 @@ __device__ __noinline__ void pipe_sum_dec(const ENode* nodes, int n, int64_t row
   const unsigned long long old = atomicAdd(acc, lo);
   const unsigned long long add_hi = hi + ((old + lo) < old ? 1ull : 0ull);
   if (add_hi) atomicAdd(acc + 1, add_hi);
+}
+// MIN / MAX over a Decimal128 argument, out of line like SUM: the {lo, hi} pair at acc (16-byte aligned in the record) is read in one
+// 128-bit load and replaced by a 128-bit CAS only when the value is better
+__device__ __noinline__ void pipe_minmax_dec(const ENode* nodes, int n, int64_t row, const uint64_t* ext, int* err_ok, unsigned long long* acc, unsigned long long* nn,
+                                             bool is_min) {
+  unsigned long long hi;
+  const unsigned long long lo = pipe_eval_dec(nodes, n, row, ext, err_ok, &hi);
+  if (!err_ok[1]) return;                                  // NULL inputs are skipped
+  if (nn) atomicAdd(nn, 1ull);
+  minmax_i128(acc, Rec128{lo, hi}, is_min);
 }
 
 __device__ __forceinline__ uint4 ld_stream_v4(const void* p, uint64_t pol) {
@@ -438,13 +440,6 @@ struct DenseParams {
 constexpr int kDenseParamsOff = (int)((sizeof(PipeParams) + 15) / 16 * 16);   // DenseParams behind PipeParams in the parameter buffer
 constexpr int kDenseAccOff = (int)((sizeof(DenseParams) + 15) / 16 * 16);     // dynamic shared memory: DenseParams, then the slots
 
-// 128-bit compare-and-swap on a generic address (shared memory in the row loop, global memory at the flush)
-__device__ __forceinline__ Rec128 cas128(void* addr, Rec128 cmp, Rec128 val) {
-  Rec128 old;
-  asm volatile("{\n\t.reg .b128 c, v, o;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 v, {%4, %5};\n\tatom.cas.b128 o, [%6], c, v;\n\tmov.b128 {%0, %1}, o;\n\t}"
-               : "=l"(old.lo), "=l"(old.hi) : "l"(cmp.lo), "l"(cmp.hi), "l"(val.lo), "l"(val.hi), "l"(addr) : "memory");
-  return old;
-}
 __device__ __forceinline__ bool lt128(unsigned long long alo, unsigned long long ahi, unsigned long long blo, unsigned long long bhi) {
   return (long long)ahi < (long long)bhi || (ahi == bhi && alo < blo);   // signed 128-bit a < b
 }
@@ -493,9 +488,10 @@ __device__ __forceinline__ void dense_update(int op, unsigned long long* w, unsi
       break;
     }
     case DO_MIN_128: case DO_MAX_128: {
-      Rec128 cur = cas128(w, Rec128{lo, hi}, Rec128{lo, hi});   // an atomic read of both words (stores only what is already there)
+      // w is a generic address: shared memory in the row loop, global memory at the flush
+      Rec128 cur = cas128<true>(w, Rec128{lo, hi}, Rec128{lo, hi});   // an atomic read of both words (stores only what is already there)
       while (dense_better(op, lo, hi, cur.lo, cur.hi)) {
-        const Rec128 prev = cas128(w, cur, Rec128{lo, hi});
+        const Rec128 prev = cas128<true>(w, cur, Rec128{lo, hi});
         if (prev.lo == cur.lo && prev.hi == cur.hi) break;
         cur = prev;
       }
@@ -1040,8 +1036,10 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
             uint64_t v;
             if (ag.small == 2) v = RING && a == 0 ? eval_int_gathered(sp.pool + ag.start, ag.n, row[u], ext, sp.n_gather, g[0][u], g[1][u])
                                                   : eval_int_fast(sp.pool + ag.start, ag.n, row[u], ext);
-            else if (DEC && ag.cls == C_DEC && ag.func == DFGPU_AGG_SUM) {
-              pipe_sum_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, ag.nn_word >= 0 ? rec + ag.nn_word : nullptr);
+            else if (DEC && ag.cls == C_DEC && ag.func != DFGPU_AGG_COUNT) {
+              unsigned long long* nn = ag.nn_word >= 0 ? rec + ag.nn_word : nullptr;   // AVG: its count word
+              if (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) pipe_minmax_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, nn, ag.func == DFGPU_AGG_MIN);
+              else pipe_sum_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, nn);   // SUM, and the sum of AVG
               continue;
             } else {
               if (RING) { atomicOr(&counters[3], (unsigned long long)kErrRingAgg); continue; }   // fill_ring admits integer programs and COUNT(*) only
@@ -1855,12 +1853,16 @@ static void prepare_acc(dfgpu_pipeline* p) {
   LookupDev t = lookup_dev(l);
   for (const PipeAgg& ag : p->aggs) {
     if (ag.func != DFGPU_AGG_MIN && ag.func != DFGPU_AGG_MAX) continue;
-    unsigned long long init;
+    unsigned long long init, init_hi = 0;
     const bool is_min = ag.func == DFGPU_AGG_MIN;
-    if (ag.cls == C_F64) { double d = is_min ? INFINITY : -INFINITY; memcpy(&init, &d, 8); }
+    if (ag.cls == C_DEC) { init = is_min ? ~0ull : 0ull; init_hi = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN; }   // i128::MAX / MIN
+    else if (ag.cls == C_F64) { double d = is_min ? INFINITY : -INFINITY; memcpy(&init, &d, 8); }
     else if (ag.cls == C_U64) init = is_min ? ~0ull : 0ull;
     else init = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN;
-    if (l->cap) { lookup_init_acc_kernel<<<grid_for((int64_t)l->cap, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, ag.word, init); DF_LAUNCH_CHECK(ctx); }
+    if (l->cap) {
+      lookup_init_acc_kernel<<<grid_for((int64_t)l->cap, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, ag.word, init); DF_LAUNCH_CHECK(ctx);
+      if (ag.cls == C_DEC) { lookup_init_acc_kernel<<<grid_for((int64_t)l->cap, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, ag.word + 1, init_hi); DF_LAUNCH_CHECK(ctx); }
+    }
   }
   p->acc_ready = true;
 }
@@ -2230,6 +2232,11 @@ static void pipeline_finish(dfgpu_pipeline* p) {
   const bool partial = p->agg_mode == DFGPU_AGG_PARTIAL;
   EmitCols ec;
   memset(&ec, 0, sizeof(ec));
+  // AVG over Decimal128 (emission kind 7): the error word is set when a group's value overflows
+  bool dec_avg = false;
+  for (const PipeAgg& ag : p->aggs) dec_avg = dec_avg || (ag.func == DFGPU_AGG_AVG && ag.cls == C_DEC);
+  DevBuf err;
+  if (dec_avg) { err.alloc(ctx, 8); err.zero(); ec.err = err.as<unsigned long long>(); }
   std::vector<DCol> out;
   const int key_col = p->stages[p->agg_stage].key_col;
   auto add = [&](int type, bool nullable, EmitCol e) {
@@ -2248,6 +2255,12 @@ static void pipeline_finish(dfgpu_pipeline* p) {
   add_agg_columns(p->aggs, p->rows_word, partial, add);
   lookup_emit_kernel<<<grid_for(groups, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), groups, p->rows_word, ec);
   DF_LAUNCH_CHECK(ctx);
+  if (dec_avg) {
+    unsigned long long h_err = 0;
+    DF_CUDA(cudaMemcpyAsync(&h_err, err.ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    if (h_err) throw Error(DFGPU_ERR_ARITH, "Arithmetic Overflow in AvgAccumulator");
+  }
   emit_sliced(p, out, groups);
 }
 
@@ -2543,6 +2556,9 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: the lookup reserves no accumulator words (n_acc_words)");
   const int rows_word = next++;
   std::vector<PipeAgg> new_aggs;   // committed only when every check has passed
+  // a Decimal128 MIN / MAX is a {lo, hi} pair updated by one 16-byte CAS: it sits on an even word of a record of an even number of words
+  auto is_pair = [](const PipeAgg& ag) { return ag.cls == C_DEC && (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX); };
+  bool pairs = false;
   for (int a = 0; a < n_aggs; ++a) {
     PipeAgg ag;
     ag.func = aggs[a].func;
@@ -2554,19 +2570,43 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
       ag.arg_type = ag.plan.root_type;
       ag.cls = cls_of(ag.arg_type);
       DF_CHECK(ag.cls != C_BOOL || ag.func == DFGPU_AGG_COUNT, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Boolean arguments only for COUNT");
-      if (ag.func == DFGPU_AGG_AVG) DF_CHECK(ag.arg_type == DFGPU_FLOAT64, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: AVG takes a Float64 argument (the planner casts)");
+      if (ag.func == DFGPU_AGG_AVG) {
+        DF_CHECK(ag.arg_type == DFGPU_FLOAT64 || ag.cls == C_DEC, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: AVG takes a Float64 (the planner casts) or Decimal128 argument");
+        DF_CHECK(ag.cls != C_DEC || mode != DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: AVG over Decimal128 runs in Single modes only");
+      }
       if ((ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX)) DF_CHECK(ag.arg_type != DFGPU_FLOAT32, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: MIN/MAX over Float32 stays on dfgpu_agg");
-      if (ag.cls == C_DEC) DF_CHECK(ag.func == DFGPU_AGG_SUM || ag.func == DFGPU_AGG_COUNT, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: SUM / COUNT over Decimal128 (MIN / MAX / AVG stay on the CPU operator)");
-      DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
-      ag.word = next++;
-      if (ag.cls == C_DEC && ag.func == DFGPU_AGG_SUM) { DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: a Decimal128 SUM takes two accumulator words (n_acc_words)"); next++; }
-      if (ag.func == DFGPU_AGG_AVG) { DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)"); ag.cnt_word = next++; ag.nn_word = ag.cnt_word; }
+      pairs = pairs || is_pair(ag);
     }
     new_aggs.push_back(std::move(ag));
   }
+  // accumulator words.  Without pairs: the row counter, then every aggregate's words in order.  With pairs: the row counter, at most one
+  // padding word to reach an even word, the pairs, then the other aggregates in order.  Spare words (the padding word first) become
+  // non-null counters.
+  auto take = [&](const char* what) { DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, what); return next++; };
+  int pad = -1;
+  if (pairs) {
+    DF_CHECK(l->stride % 2 == 0, DFGPU_ERR_UNSUPPORTED,
+             "pipeline aggregate: a Decimal128 MIN / MAX needs a record of an even number of words: a lookup without payload takes an odd n_acc_words");
+    if (next & 1) pad = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
+    for (auto& ag : new_aggs) {
+      if (!is_pair(ag)) continue;
+      ag.word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
+      take("pipeline aggregate: a Decimal128 MIN / MAX takes two accumulator words (n_acc_words)");
+    }
+  }
+  for (auto& ag : new_aggs) {
+    if (ag.func == DFGPU_AGG_COUNT_STAR || is_pair(ag)) continue;
+    ag.word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
+    if (ag.cls == C_DEC && ag.func == DFGPU_AGG_SUM) take("pipeline aggregate: a Decimal128 SUM takes two accumulator words (n_acc_words)");
+    if (ag.cls == C_DEC && ag.func == DFGPU_AGG_AVG) take("pipeline aggregate: a Decimal128 AVG takes three accumulator words (n_acc_words)");
+    if (ag.func == DFGPU_AGG_AVG) { ag.cnt_word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)"); ag.nn_word = ag.cnt_word; }
+  }
   // spare words become non-null counters (SUM / MIN / MAX of a nullable argument are NULL until a value arrives, accumulate.rs:164-188)
-  for (auto& ag : new_aggs)
-    if ((ag.func == DFGPU_AGG_SUM || ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) && next < budget) ag.nn_word = next++;
+  for (auto& ag : new_aggs) {
+    if (ag.func != DFGPU_AGG_SUM && ag.func != DFGPU_AGG_MIN && ag.func != DFGPU_AGG_MAX) continue;
+    if (pad >= 0) { ag.nn_word = pad; pad = -1; }
+    else if (next < budget) ag.nn_word = next++;
+  }
   p->rows_word = rows_word;
   p->group_cols.assign(group_cols, group_cols + n_group);
   p->aggs = std::move(new_aggs);

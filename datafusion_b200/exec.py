@@ -843,6 +843,28 @@ def _fuse_dense(plan: "GpuAggregateExec") -> Optional["GpuPipelineExec"]:
     return GpuPipelineExec(sc, sink="dense", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, key_range=ranges)
 
 
+def _acc_words(funcs: Sequence[str], types: Sequence[Optional[pa.DataType]], has_payload: bool) -> int:
+    """n_acc_words of the build lookup that a join-keyed aggregate sink accumulates into (dfgpu.h, dfgpu_pipeline_sink_aggregate): the
+    row counter; per aggregate 1 word (2 for AVG over Float64), and a Decimal128 SUM, MIN or MAX 2, a Decimal128 AVG 3; one non-null
+    counter per SUM, MIN and MAX.  A Decimal128 MIN / MAX pair is 16-byte aligned: one padding word, and a record of an even number of
+    words (key + accumulators) when the build has no payload."""
+    n, pairs = 1, False
+    for f, t in zip(funcs, types):
+        dec = t is not None and pa.types.is_decimal128(t)
+        if f == "avg":
+            n += 3 if dec else 2
+        elif f in ("sum", "min", "max"):
+            n += (2 if dec else 1) + 1
+            pairs = pairs or (dec and f != "sum")
+        else:
+            n += 1
+    if pairs:
+        n += 1
+        if not has_payload and n % 2 == 0:
+            n += 1
+    return n
+
+
 def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a): AggregateExec(Single / SinglePartitioned / Partial) over [ProjectionExec] over
     HashJoinExec(Inner) whose GROUP BY is the probe key plus build-side columns becomes ONE GpuPipelineExec; its build side (filters, semi
@@ -886,18 +908,21 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
         e = None if a.arg is None else exprs.get(a.arg)
         if a.arg is not None and e is None:
             return plan
-        if a.func == "avg" and e is not None and e.data_type(vs) != pa.float64():
-            return plan
         aggs.append((a.func, e, a.alias))
     try:
         for _, e, _ in aggs:
             if e is not None:
                 e.rpn(vs, [])                              # every referenced name must exist in the virtual schema
+        types = [None if e is None else e.data_type(vs) for _, e, _ in aggs]
     except KeyError:
         return plan
-    build.n_acc_words = 1 + sum(2 if f == "avg" else 1 for f, _, _ in aggs) + sum(1 for f, _, _ in aggs if f in ("sum", "min", "max"))
-    if build.n_acc_words > 12:
+    for (f, _, _), t in zip(aggs, types):
+        if f == "avg" and t is not None and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
+            return plan                                    # AVG(Decimal128) has no pinned Partial state
+    n_acc = _acc_words([f for f, _, _ in aggs], types, bool(build.payload))
+    if n_acc > 12:
         return plan
+    build.n_acc_words = n_acc
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
 
 

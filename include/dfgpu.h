@@ -414,7 +414,8 @@ typedef struct dfgpu_lookup_options {
   int64_t key_min, key_max;/* valid when has_key_range (column statistics, or dfgpu_column_minmax_device — the bounds
                             * collect_left_input tracks, exec.rs:2585-2619) */
   int32_t has_key_range;
-  int32_t n_acc_words;     /* 8-byte accumulator words reserved in every record for a downstream fused aggregation */
+  int32_t n_acc_words;     /* 8-byte accumulator words reserved in every record for a downstream fused aggregation (0..12; what each
+                            * aggregate costs: dfgpu_pipeline_sink_aggregate) */
   int32_t membership_filter; /* 1 = build a blocked Bloom filter next to the table, 0 = never, -1 = when the table exceeds L2 */
   int32_t filter_only;       /* 1 = membership filter WITHOUT a table (16 bits per expected_rows key): the pushed-down dynamic filter of a join
                               * whose exact probe happens downstream of an exchange; backs DFGPU_STAGE_MAYBE stages only */
@@ -470,6 +471,16 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
  *  aggregate : AggregateExec over the surviving rows; group_cols must be the probe key of one INNER stage plus payload
  *              fields of that stage (group id == build row; anything else -> DFGPU_ERR_UNSUPPORTED, use dfgpu_agg);
  *              mode = DFGPU_AGG_SINGLE* or DFGPU_AGG_PARTIAL (state columns as dfgpu_agg emits them);
+ *              the accumulators are words of the lookup's records (n_acc_words): 1 row counter, then per aggregate
+ *                COUNT(x), and SUM / MIN / MAX over a 64-bit type: 1;  AVG over Float64: 2;
+ *                Decimal128 SUM: 2;  Decimal128 MIN / MAX: 2, one 16-byte aligned {lo, hi} pair;  Decimal128 AVG: 3;
+ *              plus 1 non-null counter for a SUM / MIN / MAX whose argument can be NULL (without it such an argument is
+ *              DFGPU_ERR_UNSUPPORTED at the push); spare words become non-null counters.
+ *              Over Decimal128: COUNT, SUM, MIN, MAX in every mode; AVG -> Decimal128(min(38, p+4), min(38, s+4)) in Single
+ *              modes only (DFGPU_ERR_ARITH at finish when a group's value overflows, as in the dense sink).  A Decimal128 MIN /
+ *              MAX needs a record of an even number of words: with payload it always is; a lookup without payload needs an odd
+ *              n_acc_words (else DFGPU_ERR_UNSUPPORTED).  The pairs take even words after the row counter, behind at most one
+ *              padding word, which may serve as a non-null counter; without pairs the words are taken in aggregate order;
  *  output    : surviving rows, columns = out_cols of the virtual schema, input order preserved. */
 int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload);
 int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, int32_t n_group,

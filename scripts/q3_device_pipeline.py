@@ -148,14 +148,15 @@ def revenue_expr(l_types):
     return B(D.OP_MULTIPLY, C(1), B(D.OP_MINUS, L(100), C(2)))
 
 
-def run_q3_fused(ctx, customer, orders, lineitem):
+def run_q3_fused(ctx, customer, orders, lineitem, aggs=None, n_acc_words=None):
     """the same plan as three fused pipelines (dfgpu_pipeline): every table is read once, no intermediate batch touches HBM
 
         P1  customer : FilterExec(c_mktsegment = 1)                      -> build L1 = key set {c_custkey}   (dense range -> bitmap)
         P2  orders   : FilterExec(o_orderdate < CUT) -> RightSemi vs L1  -> build L2 = {o_orderkey -> (o_orderdate, o_shippriority)}
         P3  lineitem : FilterExec(l_shipdate > CUT)  -> Inner vs L2      -> AggregateExec gby [l_orderkey, o_orderdate, o_shippriority]
                                                                             SUM(l_extendedprice * (100 - l_discount))
-    The group keys are the join key plus build-side columns, so the group id is the build row and the sums live in L2's records."""
+    The group keys are the join key plus build-side columns, so the group id is the build row and the sums live in L2's records.
+    aggs / n_acc_words: other aggregates of P3 ([(func, nodes)]) and the accumulator words of L2 they need (default: the SUM)."""
     stages = {}
     kmin, kmax, _ = D.column_minmax_device(ctx, customer.cols[0])       # the bounds collect_left_input tracks (exec.rs:2585-2619)
     l1 = D.Lookup(ctx, D.INT64, [], key_range=(kmin, kmax))
@@ -165,14 +166,14 @@ def run_q3_fused(ctx, customer, orders, lineitem):
     stages["customer_building"] = p1.metric("sink_rows")
     p1.close()
     dec = D.type_base(lineitem.types[1]) == D.DECIMAL128                 # a Decimal128 SUM takes two accumulator words
-    l2 = D.Lookup(ctx, D.INT64, [D.INT32, D.INT32], n_acc_words=3 if dec else 2, membership_filter=-1)
+    l2 = D.Lookup(ctx, D.INT64, [D.INT32, D.INT32], n_acc_words=n_acc_words or (3 if dec else 2), membership_filter=-1)
     p2 = D.Pipeline(ctx, orders.types, B(D.OP_LT, C(2), L(CUT, D.INT32)), [(D.STAGE_SEMI, 1, l1)], name="orders")
     p2.sink_build(l2, 0, [2, 3])
     p2.push_device(orders.cols); p2.finish()
     stages["orders_of_building_customers"] = p2.metric("sink_rows")
     p2.close()
     p3 = D.Pipeline(ctx, lineitem.types, B(D.OP_GT, C(3), L(CUT, D.INT32)), [(D.STAGE_INNER, 0, l2)], name="lineitem")
-    p3.sink_aggregate([0, 4, 5], [(D.AGG_SUM, revenue_expr(lineitem.types))], D.AGG_SINGLE_PARTITIONED)
+    p3.sink_aggregate([0, 4, 5], aggs or [(D.AGG_SUM, revenue_expr(lineitem.types))], D.AGG_SINGLE_PARTITIONED)
     p3.push_device(lineitem.cols); p3.finish()
     res = p3.drain(host=False)
     stages["joined_rows"] = p3.metric("sink_rows")
