@@ -165,7 +165,8 @@ EXPORTS = [
     "dfgpu_comm_destroy", "dfgpu_exchange_create", "dfgpu_exchange_run", "dfgpu_exchange_columns", "dfgpu_exchange_destroy",
     "dfgpu_lookup_default_options", "dfgpu_lookup_create", "dfgpu_lookup_metric", "dfgpu_lookup_destroy", "dfgpu_lookup_clear",
     "dfgpu_lookup_filter_buffer", "dfgpu_lookup_filter_allreduce_peer", "dfgpu_pipeline_sink_output_unordered", "dfgpu_pipeline_set_name", "dfgpu_column_minmax_device", "dfgpu_column_sum_device",
-    "dfgpu_pipeline_create", "dfgpu_pipeline_sink_build", "dfgpu_pipeline_sink_aggregate", "dfgpu_pipeline_sink_aggregate_dense", "dfgpu_pipeline_sink_output",
+    "dfgpu_pipeline_create", "dfgpu_pipeline_sink_build", "dfgpu_pipeline_sink_aggregate", "dfgpu_pipeline_sink_aggregate_dense",
+    "dfgpu_pipeline_sink_aggregate_hash", "dfgpu_pipeline_sink_output",
     "dfgpu_pipeline_push_host", "dfgpu_pipeline_push_device", "dfgpu_pipeline_push_arrow", "dfgpu_pipeline_finish",
     "dfgpu_pipeline_next", "dfgpu_pipeline_metric", "dfgpu_pipeline_destroy",
     "dfgpu_dictionary_create", "dfgpu_dictionary_unify", "dfgpu_dictionary_code", "dfgpu_dictionary_size", "dfgpu_dictionary_value",
@@ -291,6 +292,7 @@ def load_library() -> C.CDLL:
     sig("dfgpu_pipeline_sink_build", C.c_int, [vp, vp, i32, P(i32), i32])
     sig("dfgpu_pipeline_sink_aggregate", C.c_int, [vp, P(i32), i32, P(PipelineAgg), i32, i32, i64])
     sig("dfgpu_pipeline_sink_aggregate_dense", C.c_int, [vp, P(i32), P(i64), P(i64), i32, P(PipelineAgg), i32, i32, i64])
+    sig("dfgpu_pipeline_sink_aggregate_hash", C.c_int, [vp, P(i32), P(i32), i32, P(PipelineAgg), i32, i32, i64, i64])
     sig("dfgpu_pipeline_sink_output", C.c_int, [vp, P(i32), i32, i64])
     sig("dfgpu_pipeline_set_name", C.c_int, [vp, C.c_char_p])
     sig("dfgpu_pipeline_push_host", C.c_int, [vp, P(Column), i32])
@@ -861,6 +863,18 @@ class Pipeline(_Operator):
         kmax = (C.c_int64 * max(len(key_range), 1))(*[int(hi) for _, hi in key_range])
         self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_aggregate_dense(self.h, _i32arr(group_cols), kmin, kmax, len(group_cols), arr, len(aggs),
                                                                         mode, batch_size))
+
+    def sink_aggregate_hash(self, group_cols, aggs, mode=AGG_SINGLE, batch_size=0, capacity_hint=0, nullable=None):
+        """GROUP BY any integer-like virtual columns packed into at most 128 bits (one extra bit per nullable column); the sink owns its
+        group table, capacity_hint (expected groups, 0 = unknown) sizes only the first one.  nullable: the declared nullability of each
+        group column (None = none is nullable).  aggs: [(func, nodes or None)]"""
+        group_cols = list(group_cols)
+        if nullable is not None and len(nullable) != len(group_cols):
+            raise ValueError("sink_aggregate_hash: one nullability flag per group column")
+        arr = self._agg_array(aggs)
+        nul = _i32arr([1 if x else 0 for x in nullable]) if nullable is not None else None
+        self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_aggregate_hash(self.h, _i32arr(group_cols), nul, len(group_cols), arr, len(aggs), mode,
+                                                                       batch_size, capacity_hint))
 
     def sink_output(self, out_cols, batch_size=0, ordered=True):
         fn = self.ctx.lib.dfgpu_pipeline_sink_output if ordered else self.ctx.lib.dfgpu_pipeline_sink_output_unordered

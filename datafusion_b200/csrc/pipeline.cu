@@ -44,7 +44,8 @@ constexpr int kPipeThreads = 256, kPipeItems = 4, kPipeTile = kPipeThreads * kPi
 enum LookupMode : int { LK_HASH = 0, LK_BITMAP = 1 };
 enum SinkKind : int { SINK_NONE = 0, SINK_COUNT = 1, SINK_BUILD = 2, SINK_AGG = 3, SINK_OUTPUT = 4, SINK_OUTPUT_ANY = 5 /* row order unspecified */,
                       SINK_PACK = 6 /* build sink, table size unknown: {key, payload} records to a staging buffer, inserted afterwards */,
-                      SINK_DENSE = 7 /* aggregate over group keys in small declared domains: slot arithmetic, shared-memory accumulators */ };
+                      SINK_DENSE = 7 /* aggregate over group keys in small declared domains: slot arithmetic, shared-memory accumulators */,
+                      SINK_HASH = 8 /* aggregate over a packed group key: find-or-claim in the sink's own table */ };
 constexpr int kStageMaybe = 3;   // DFGPU_STAGE_MAYBE
 constexpr int kPipeVarDefault = 11;   // pipe_kernel's VAR when DFGPU_PIPE_VAR is not set (H100 SXM at 400 W, Q3 SF100 lineitem pass: 17.5 ms; 43 20.4-20.9 ms)
 // ring-fed phase A: at most kMaxRing streamed columns, kMaxRingStages tiles per warp ring, the mbarriers in the first kRingBarBytes of the
@@ -437,8 +438,52 @@ struct DenseParams {
   // `column <cmp> literal` terms of the predicate's conjunction beyond PipeParams' kMaxTerms (TPC-H Q6 has five), tested after them
   int n_xterms, xterm_col[kDenseMaxXTerms], xterm_op[kDenseMaxXTerms], xterm_uns[kDenseMaxXTerms]; long long xterm_lit[kDenseMaxXTerms];
 };
-constexpr int kDenseParamsOff = (int)((sizeof(PipeParams) + 15) / 16 * 16);   // DenseParams behind PipeParams in the parameter buffer
+constexpr int kDenseParamsOff = (int)((sizeof(PipeParams) + 15) / 16 * 16);   // DenseParams (or HashParams) behind PipeParams in the parameter buffer
 constexpr int kDenseAccOff = (int)((sizeof(DenseParams) + 15) / 16 * 16);     // dynamic shared memory: DenseParams, then the slots
+
+// ------------------------------------------------------------------------------------------
+// hash-keyed aggregate sink (SINK_HASH): AggregateExec over a FilterExec (and probe stages) whose GROUP BY keys the join key does not
+// determine (TPC-H Q15's revenue0: l_suppkey; Q3 grouped by o_custkey).  The group columns of a row are packed into a 128-bit tag
+// {lo, hi} (each column at its width, one NULL bit per nullable column) and the sink finds or claims the record
+//   {tag_lo | tag_hi | row counter | accumulator words...}
+// of that tag in its own open-addressing table (one 16-byte CAS claims a slot); the accumulate block of the join-keyed sink then runs on
+// that record.  The table grows between launches: a claim beyond the budget (group_limit) or a probe longer than kHashMaxProbe defers
+// the row to the overflow list before it touches any accumulator, and the host grows the table and pushes the deferred rows again.
+// The one tag equal to the empty marker {~0, ~0} lives in the side record behind the cap regular slots.  HashParams sit behind
+// PipeParams in the parameter buffer, as DenseParams do, and are copied to dynamic shared memory.
+// ------------------------------------------------------------------------------------------
+constexpr int kHashMaxKeys = 8, kHashMaxWords = 16, kHashMaxProbe = 256;
+struct HashKey { int src /* virtual column */, shift /* bit offset in the tag */, bits, null_bit /* -1: declared non-nullable */; };
+struct HashParams {
+  int n_keys, stride /* words per record, even */, pad0, pad1;
+  HashKey key[kHashMaxKeys];
+  unsigned long long* recs; uint64_t cap;        // cap regular records, then the side record
+  unsigned long long* ngroups; uint64_t group_limit;   // claimed regular records; no claims at or beyond the limit
+  uint32_t* overflow; unsigned long long* overflow_count;   // deferred input rows of this launch
+};
+struct HashIdent { unsigned long long w[kHashMaxWords]; };   // initial value of each record word (tag words ~0, MIN / MAX identities)
+
+__device__ __forceinline__ uint64_t hash_tag_slot(uint64_t lo, uint64_t hi, uint64_t cap) { return __umul64hi(hash_combine(hash_u64(lo, kSeedAgg), hi), cap); }
+// the record of tag {lo, hi}, claimed when absent; nullptr when the row must be deferred (claim budget exhausted or probe too long)
+__device__ __forceinline__ unsigned long long* hash_find_or_claim(const HashParams& hp, uint64_t lo, uint64_t hi) {
+  if (lo == kEmptyKey && hi == kEmptyKey) return hp.recs + hp.cap * (uint64_t)hp.stride;   // the side record
+  uint64_t s = hash_tag_slot(lo, hi, hp.cap);
+#pragma unroll 1
+  for (int probe = 0; probe < kHashMaxProbe; ++probe) {
+    unsigned long long* r = hp.recs + s * (uint64_t)hp.stride;
+    const uint4 v = __ldcg((const uint4*)r);
+    const uint64_t clo = (uint64_t)v.x | ((uint64_t)v.y << 32), chi = (uint64_t)v.z | ((uint64_t)v.w << 32);
+    if (clo == lo && chi == hi) return r;
+    if (clo == kEmptyKey && chi == kEmptyKey) {
+      if (__ldcg(hp.ngroups) >= hp.group_limit) return nullptr;
+      const Rec128 prev = cas128(r, Rec128{kEmptyKey, kEmptyKey}, Rec128{lo, hi});
+      if (prev.lo == kEmptyKey && prev.hi == kEmptyKey) { atomicAdd(hp.ngroups, 1ull); return r; }
+      if (prev.lo == lo && prev.hi == hi) return r;
+    }
+    if (++s == hp.cap) s = 0;
+  }
+  return nullptr;
+}
 
 __device__ __forceinline__ bool lt128(unsigned long long alo, unsigned long long ahi, unsigned long long blo, unsigned long long bhi) {
   return (long long)ahi < (long long)bhi || (ahi == bhi && alo < blo);   // signed 128-bit a < b
@@ -545,6 +590,10 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
   if constexpr (SINK == SINK_DENSE) {   // dynamic shared memory: DenseParams, then this block's slots
     const uint32_t* src = (const uint32_t*)((const char*)gp + kDenseParamsOff);
     for (int i = threadIdx.x; i < (int)(sizeof(DenseParams) / 4); i += kPipeThreads) ((uint32_t*)dyn_smem)[i] = src[i];
+  }
+  if constexpr (SINK == SINK_HASH) {   // dynamic shared memory: HashParams
+    const uint32_t* src = (const uint32_t*)((const char*)gp + kDenseParamsOff);
+    for (int i = threadIdx.x; i < (int)(sizeof(HashParams) / 4); i += kPipeThreads) ((uint32_t*)dyn_smem)[i] = src[i];
   }
   __syncthreads();
   if constexpr (SINK == SINK_DENSE) {
@@ -993,6 +1042,37 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
           __syncwarp();   // per-warp copies: this round's stores are seen by the next round's leaders
         }
       }
+      if constexpr (SINK == SINK_HASH) {   // the record of each survivor's packed group tag; a deferred row leaves the round untouched
+        const HashParams& hp = *(const HashParams*)dyn_smem;
+#pragma unroll
+        for (int u = 0; u < PB; ++u) {
+          if (!live[u]) continue;
+          u128 tag = 0;
+#pragma unroll 1
+          for (int k = 0; k < hp.n_keys; ++k) {
+            const HashKey& hk = hp.key[k];
+            bool isnull = false;
+            uint64_t v;
+            if (hk.src < sp.n_cols) {
+              const ColRef& c = sp.col[hk.src];
+              isnull = c.valid && !bit_get(c.valid, c.voff + row[u]);
+              v = isnull ? 0ull : ld_stream_int(c.ptr, c.width, 0, row[u], pol_stream);
+            } else {
+              const ExtDef e = sp.ext[hk.src - sp.n_cols];
+              uint64_t wd = 0;
+#pragma unroll
+              for (int s = 0; s < kMaxStages; ++s) if (s == e.stage) wd = pay[s][u];
+              v = ext_field(wd, e.shift, e.width, DFGPU_UINT64);
+            }
+            if (isnull && hk.null_bit < 0) fail |= 4;   // a NULL in a column declared non-nullable
+            if (hk.bits < 64) v &= (1ull << hk.bits) - 1ull;
+            tag |= (u128)v << hk.shift;
+            if (isnull && hk.null_bit >= 0) tag |= (u128)1 << hk.null_bit;
+          }
+          arec[u] = hash_find_or_claim(hp, (uint64_t)tag, (uint64_t)(tag >> 64));
+          if (!arec[u]) { hp.overflow[atomicAdd(hp.overflow_count, 1ull)] = (uint32_t)row[u]; live[u] = false; }
+        }
+      }
 #pragma unroll
       for (int u = 0; u < PB; ++u) {
         if (SINK == SINK_OUTPUT_ANY || SINK == SINK_DENSE || sunk) break;
@@ -1027,7 +1107,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
             if (rc == 0) ins_cnt++;
             else if (rc == 2 || sp.target_unique) fail |= rc;
           }
-        } else if (SINK == SINK_AGG) {
+        } else if (SINK == SINK_AGG || SINK == SINK_HASH) {
           unsigned long long* rec = arec[u];
           red_add_u64(rec + sp.rows_word, 1ull);
           for (int a = 0; a < sp.n_aggs; ++a) {
@@ -1361,6 +1441,26 @@ __global__ void __launch_bounds__(256) lookup_insert_records_kernel(LookupDev t,
 __global__ void __launch_bounds__(256) lookup_init_acc_kernel(LookupDev t, int word, unsigned long long value) {
   for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < t.cap; s += (uint64_t)gridDim.x * blockDim.x) t.recs[s * (uint64_t)t.stride + word] = value;
 }
+// the hash sink's table: every record (the side record included) starts as its identity words
+__global__ void __launch_bounds__(256) hash_init_kernel(unsigned long long* recs, uint64_t n_recs, int stride, HashIdent id) {
+  const uint64_t total = n_recs * (uint64_t)stride;
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < total; i += (uint64_t)gridDim.x * blockDim.x) recs[i] = id.w[i % (uint64_t)stride];
+}
+// the hash sink's growth: the claimed regular records of the old table move to the (initialised) new one, every word as it is
+__global__ void __launch_bounds__(256) hash_rehash_kernel(const unsigned long long* __restrict__ old_recs, uint64_t old_cap, unsigned long long* new_recs, uint64_t new_cap, int stride) {
+  for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < old_cap; s += (uint64_t)gridDim.x * blockDim.x) {
+    const unsigned long long* r = old_recs + s * (uint64_t)stride;
+    const uint64_t lo = r[0], hi = r[1];
+    if (lo == kEmptyKey && hi == kEmptyKey) continue;
+    uint64_t d = hash_tag_slot(lo, hi, new_cap);
+    while (true) {
+      unsigned long long* q = new_recs + d * (uint64_t)stride;
+      const Rec128 prev = cas128(q, Rec128{kEmptyKey, kEmptyKey}, Rec128{lo, hi});
+      if (prev.lo == kEmptyKey && prev.hi == kEmptyKey) { for (int w = 2; w < stride; ++w) q[w] = r[w]; break; }
+      if (++d == new_cap) d = 0;
+    }
+  }
+}
 // records with rows_word > 0 -> occupancy bitmap (one ballot word per warp)
 __global__ void __launch_bounds__(256) lookup_groups_kernel(LookupDev t, int rows_word, uint32_t* __restrict__ words) {
   const uint64_t nw = (t.cap + 31) / 32;
@@ -1374,10 +1474,12 @@ __global__ void __launch_bounds__(256) lookup_groups_kernel(LookupDev t, int row
 }
 struct EmitCol {
   int kind /* 0 key, 1 payload field, 2 accumulator word, 3 AVG value, 4 count as u64, 5 Decimal128 sum / min / max (two words),
-              6 dense group key decoded from the slot number, 7 Decimal128 AVG value */, width, shift, word, nn_word, cnt_word, f64;
+              6 dense group key decoded from the slot number, 7 Decimal128 AVG value, 8 packed group field of a 128-bit tag in words 0 and 1 */,
+      width, shift, word, nn_word, cnt_word, f64;
   void* dst; uint32_t* valid;
   long long kmin; int kstride, kradix;   // kind 6: key = kmin + (slot / kstride) % kradix, NULL when that index is kradix - 1
   int avg_mul, avg_prec;                  // kind 7: sum * 10^avg_mul / count must fit Decimal128(avg_prec, _)
+  int tag_null;                           // kind 8: the field starts at bit `shift`; NULL when bit tag_null (>= 0) is set
 };
 struct EmitCols { int n; EmitCol c[kMaxPipeCols]; unsigned long long* err /* kind 7: set to 1 on overflow */; };
 __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uint32_t* __restrict__ slots, int64_t n, int rows_word, EmitCols ec) {
@@ -1415,6 +1517,12 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
             if (ok && !dec_avg((i128)(((u128)r[e.word + 1] << 64) | (u128)r[e.word]), cnt, e.avg_mul, e.avg_prec, &q)) atomicOr(ec.err, 1ull);
             ((unsigned long long*)e.dst)[2 * i] = (unsigned long long)(u128)q;
             ((unsigned long long*)e.dst)[2 * i + 1] = (unsigned long long)((u128)q >> 64);
+            break;
+          }
+          case 8: {
+            const u128 tag = ((u128)r[1] << 64) | (u128)r[0];
+            ok = e.tag_null < 0 || !(uint64_t)((tag >> e.tag_null) & 1u);
+            v = (uint64_t)(tag >> e.shift);   // the store below keeps the column's width: no sign extension needed
             break;
           }
           default: {   // AVG = sum / count over Float64 (functions-aggregate/src/average.rs)
@@ -1532,6 +1640,10 @@ struct dfgpu_pipeline {
   // dense-group aggregate sink (group_cols, aggs and agg_mode as above; the aggregates' words address a slot of dense_acc)
   std::vector<DenseKey> dense_keys; std::vector<int> dense_radix; std::vector<unsigned long long> dense_ident;
   int dense_slots = 0, dense_words = 0; DevBuf dense_acc;
+  // hash-keyed aggregate sink (group_cols, aggs, agg_mode and rows_word as above; the aggregates' words address a record of hash_recs)
+  std::vector<HashKey> hash_keys; std::vector<unsigned long long> hash_ident; int hash_stride = 0; int64_t hash_cap_hint = 0;
+  uint64_t hash_cap = 0; DevBuf hash_recs /* hash_cap records, then the side record */, hash_ngroups;
+  int64_t m_group_rehashes = 0, m_replayed_rows = 0;
   // output sink
   std::vector<int> out_cols; bool out_ordered = true;
   std::vector<std::vector<DCol>> out_parts; int64_t out_rows_pending = 0;
@@ -1748,7 +1860,7 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
       pp->bpay_src[c] = p->bpay_cols[c]; pp->bpay_shift[c] = p->target->pay_shift[c]; pp->bpay_width[c] = type_width(p->target->pay_types[c]);
       if (p->bpay_cols[c] < (int)cols.size()) DF_CHECK(!cols[p->bpay_cols[c]].validity, DFGPU_ERR_UNSUPPORTED, "pipeline: nullable build payload columns stay on the unfused join");
     }
-  } else if (p->sink == SINK_AGG) {
+  } else if (p->sink == SINK_AGG || p->sink == SINK_HASH) {
     pp->agg_stage = p->agg_stage; pp->rows_word = p->rows_word; pp->n_aggs = (int)p->aggs.size();
     for (size_t a = 0; a < p->aggs.size(); ++a) {
       const PipeAgg& ag = p->aggs[a];
@@ -1971,6 +2083,100 @@ static size_t partitioned_table_bytes(const dfgpu_pipeline* p, const PipeParams&
   return bytes > (40ull << 20) || force_parts >= 2 ? bytes : 0;
 }
 
+// ---- hash-keyed aggregate sink ----
+// (re)allocate the table with new_cap regular records: every record starts as the identity words, then the claimed records and the
+// side record of the old table move over
+static void hash_grow(dfgpu_pipeline* p, uint64_t new_cap) {
+  dfgpu_ctx* ctx = p->ctx;
+  DF_CHECK(new_cap < 0xFFFFFFFEull, DFGPU_ERR_UNSUPPORTED, "pipeline hash aggregate: the group table would exceed 2^32 records");
+  const int st = p->hash_stride;
+  HashIdent id;
+  memset(&id, 0, sizeof(id));
+  for (int w = 0; w < st; ++w) id.w[w] = p->hash_ident[w];
+  DevBuf nrecs(ctx, (size_t)(new_cap + 1) * st * 8);
+  hash_init_kernel<<<grid_for((int64_t)(new_cap + 1) * st, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(nrecs.as<unsigned long long>(), new_cap + 1, st, id);
+  DF_LAUNCH_CHECK(ctx);
+  if (p->hash_cap > 0) {
+    hash_rehash_kernel<<<grid_for((int64_t)p->hash_cap, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(p->hash_recs.as<unsigned long long>(), p->hash_cap,
+                                                                                                  nrecs.as<unsigned long long>(), new_cap, st);
+    DF_LAUNCH_CHECK(ctx);
+    DF_CUDA(cudaMemcpyAsync(nrecs.as<unsigned long long>() + new_cap * st, p->hash_recs.as<unsigned long long>() + p->hash_cap * st, (size_t)st * 8,
+                            cudaMemcpyDeviceToDevice, ctx->stream));
+    p->m_group_rehashes++;
+  }
+  p->hash_recs = std::move(nrecs); p->hash_cap = new_cap;
+}
+
+// One push in row chunks (the overflow list holds one chunk's row numbers).  Before a chunk the table grows x4 once groups x 2 > capacity;
+// after a launch that deferred rows the table grows x4 and those rows, gathered into one compact batch, go through the same kernel again
+// (each round raises the claim budget to 5/8 of four times the capacity, above the groups already claimed, so every round claims more).
+static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t n) {
+  dfgpu_ctx* ctx = p->ctx;
+  DF_CHECK(n < 0xFFFFFFFFll, DFGPU_ERR_UNSUPPORTED, "pipeline: a batch must have < 2^32-1 rows");
+  if (!p->hash_recs.ptr) {
+    p->hash_ngroups.alloc(ctx, 8);
+    p->hash_ngroups.zero();
+    hash_grow(p, std::max<uint64_t>(1024, (uint64_t)p->hash_cap_hint * 2));
+  }
+  const size_t pbytes = kDenseParamsOff + sizeof(HashParams);
+  if (p->params_dev.bytes < pbytes) p->params_dev.alloc(ctx, pbytes);
+  // programs that touch Decimal128 values run the instantiation with the 128-bit interpreter
+  void (*kern)(const PipeParams*, int64_t, unsigned long long*) = pipeline_has_decimal(p) ? pipe_kernel<SINK_HASH, true> : pipe_kernel<SINK_HASH, false>;
+  int blocks_per_sm = 0;
+  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, sizeof(HashParams)));
+  const std::string tname = p->name.empty() ? std::string("pipeline_hash") : "pipe:" + p->name;
+  constexpr int64_t kMaxChunk = 1ll << 26;
+  int64_t chunk = std::max<int64_t>((int64_t)p->hash_cap / 2, 1 << 20);
+  DevBuf overflow;
+  unsigned long long groups = 0;
+  DF_CUDA(cudaMemcpyAsync(&groups, p->hash_ngroups.ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  for (int64_t done = 0; done < n; done += chunk, chunk = std::min(chunk * 4, kMaxChunk)) {
+    const int64_t m = std::min(chunk, n - done);
+    if (groups * 2 > p->hash_cap) hash_grow(p, p->hash_cap * 4);
+    if (overflow.bytes < (size_t)m * 4) overflow.alloc(ctx, (size_t)m * 4);
+    std::vector<DCol> batch;
+    for (const DCol& c : cols) batch.push_back(m == n ? c : slice_column(c, done, m));
+    int64_t rows = m;
+    while (true) {
+      PipeParams pp;
+      fill_params(p, batch, &pp);
+      pp.ring_stages = 0;
+      HashParams hp;
+      memset(&hp, 0, sizeof(hp));
+      hp.n_keys = (int)p->hash_keys.size(); hp.stride = p->hash_stride;
+      for (size_t k = 0; k < p->hash_keys.size(); ++k) hp.key[k] = p->hash_keys[k];
+      hp.recs = p->hash_recs.as<unsigned long long>(); hp.cap = p->hash_cap;
+      hp.ngroups = p->hash_ngroups.as<unsigned long long>(); hp.group_limit = p->hash_cap / 8 * 5;   // the claim budget, as dfgpu_agg's
+      hp.overflow = overflow.as<uint32_t>(); hp.overflow_count = p->counters.as<unsigned long long>() + 4;
+      DF_CUDA(cudaMemcpyAsync(p->params_dev.ptr, &pp, sizeof(PipeParams), cudaMemcpyHostToDevice, ctx->stream));
+      DF_CUDA(cudaMemcpyAsync((char*)p->params_dev.ptr + kDenseParamsOff, &hp, sizeof(HashParams), cudaMemcpyHostToDevice, ctx->stream));
+      p->counters.zero();
+      const int grid = (int)std::min<int64_t>((rows + kPipeTile - 1) / kPipeTile, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
+      {
+        KernelTimer kt(ctx, tname.c_str());
+        kern<<<grid, kPipeThreads, sizeof(HashParams), ctx->stream>>>((const PipeParams*)p->params_dev.ptr, rows, p->counters.as<unsigned long long>());
+        DF_LAUNCH_CHECK(ctx);
+      }
+      unsigned long long h8[8];
+      DF_CUDA(cudaMemcpyAsync(h8, p->counters.ptr, 64, cudaMemcpyDeviceToHost, ctx->stream));
+      DF_CUDA(cudaMemcpyAsync(&groups, p->hash_ngroups.ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
+      DF_CUDA(cudaStreamSynchronize(ctx->stream));   // also: `pp` and `hp` live on this stack frame
+      check_errors(h8[3]);
+      if (h8[2] & 4) throw Error(DFGPU_ERR_INVALID, "pipeline hash aggregate: a group column declared non-nullable holds a NULL");
+      p->m_sink_rows += (int64_t)h8[0];
+      const int64_t deferred = (int64_t)h8[4];
+      if (deferred == 0) break;
+      hash_grow(p, p->hash_cap * 4);   // x4 per round: the deferred rows may hold few groups, so their count does not size the table
+      std::vector<DCol> replay;
+      for (const DCol& c : batch) replay.push_back(take_column(ctx, c, overflow.as<uint32_t>(), deferred, false));
+      batch = std::move(replay);
+      rows = deferred;
+      p->m_replayed_rows += deferred;
+    }
+  }
+}
+
 static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   DF_CHECK(!p->finished, DFGPU_ERR_STATE, "push after finish");
   DF_CHECK(p->sink != SINK_NONE, DFGPU_ERR_STATE, "pipeline: choose a sink before the first push");
@@ -2073,6 +2279,8 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     read_counters(p, h);
     check_errors(h[3]);
     p->m_sink_rows += (int64_t)h[0];
+  } else if (p->sink == SINK_HASH) {
+    hash_push(p, cols, n);
   } else if (p->sink == SINK_DENSE) {
     prepare_dense(p);
     fill_params(p, cols, &pp);
@@ -2217,15 +2425,22 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     return;
   }
   if (p->sink == SINK_DENSE) { dense_finish(p); return; }
-  if (p->sink != SINK_AGG) return;
-  dfgpu_lookup* l = p->stages[p->agg_stage].lookup;
-  if (l->cap == 0) return;
-  LookupDev t = lookup_dev(l);
-  const uint64_t nw = (l->cap + 31) / 32;
+  if (p->sink != SINK_AGG && p->sink != SINK_HASH) return;
+  LookupDev t;
+  if (p->sink == SINK_AGG) {
+    dfgpu_lookup* l = p->stages[p->agg_stage].lookup;
+    if (l->cap == 0) return;
+    t = lookup_dev(l);
+  } else {   // the hash sink's table: the regular records, then the side record
+    if (!p->hash_recs.ptr) return;
+    memset(&t, 0, sizeof(t));
+    t.recs = p->hash_recs.as<unsigned long long>(); t.cap = p->hash_cap + 1; t.stride = p->hash_stride;
+  }
+  const uint64_t nw = (t.cap + 31) / 32;
   DevBuf words(ctx, (size_t)nw * 4 + 8), idx;
   lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, p->rows_word, words.as<uint32_t>());
   DF_LAUNCH_CHECK(ctx);
-  const int64_t groups = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)l->cap, 1, &idx);
+  const int64_t groups = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)t.cap, 1, &idx);
   p->m_groups = groups;
   if (groups == 0) return;
   // output schema: group columns, then one (Single) or the state (Partial) columns per aggregate
@@ -2238,7 +2453,7 @@ static void pipeline_finish(dfgpu_pipeline* p) {
   DevBuf err;
   if (dec_avg) { err.alloc(ctx, 8); err.zero(); ec.err = err.as<unsigned long long>(); }
   std::vector<DCol> out;
-  const int key_col = p->stages[p->agg_stage].key_col;
+  const int key_col = p->sink == SINK_AGG ? p->stages[p->agg_stage].key_col : -1;
   auto add = [&](int type, bool nullable, EmitCol e) {
     DF_CHECK(ec.n < kMaxPipeCols, DFGPU_ERR_UNSUPPORTED, "pipeline: too many output columns");
     DCol d = alloc_col(ctx, type, groups, nullable);
@@ -2247,7 +2462,14 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     ec.c[ec.n++] = e;
     out.push_back(std::move(d));
   };
+  for (size_t k = 0; k < p->hash_keys.size(); ++k) {   // hash sink: the fields of the packed tag
+    const HashKey& hk = p->hash_keys[k];
+    EmitCol e; memset(&e, 0, sizeof(e));
+    e.kind = 8; e.shift = hk.shift; e.tag_null = hk.null_bit;
+    add(p->vtypes[hk.src], hk.null_bit >= 0, e);
+  }
   for (int g : p->group_cols) {
+    if (p->sink == SINK_HASH) break;
     EmitCol e; memset(&e, 0, sizeof(e));
     if (g == key_col) { e.kind = 0; add(p->in_types[g], false, e); }
     else { const ExtDef& x = p->exts[g - (int)p->in_types.size()]; e.kind = 1; e.shift = x.shift; add(x.type, false, e); }
@@ -2312,6 +2534,67 @@ static void dense_finish(dfgpu_pipeline* p) {
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
   if (h_err) throw Error(DFGPU_ERR_ARITH, "Arithmetic Overflow in AvgAccumulator");
   emit_sliced(p, out, groups);
+}
+
+// the aggregates of the join-keyed and the hash-keyed sink: functions, argument programs and the types each accepts
+static std::vector<PipeAgg> parse_pipe_aggs(const dfgpu_pipeline* p, const dfgpu_pipeline_agg* aggs, int n_aggs, int mode) {
+  DF_CHECK(n_aggs >= 0 && n_aggs <= kMaxPipeAggs && (n_aggs == 0 || aggs), DFGPU_ERR_UNSUPPORTED, "pipeline: 0..4 aggregates");
+  std::vector<PipeAgg> out;
+  for (int a = 0; a < n_aggs; ++a) {
+    PipeAgg ag;
+    ag.func = aggs[a].func;
+    DF_CHECK(ag.func >= DFGPU_AGG_SUM && ag.func <= DFGPU_AGG_COUNT_STAR, DFGPU_ERR_INVALID, "pipeline aggregate: unknown function");
+    if (ag.func != DFGPU_AGG_COUNT_STAR) {
+      DF_CHECK(aggs[a].expr && aggs[a].n_nodes > 0, DFGPU_ERR_INVALID, "pipeline aggregate: missing argument expression");
+      ag.plan = plan_expr(p->vtypes.data(), (int)p->vtypes.size(), aggs[a].expr, aggs[a].n_nodes);
+      ag.has_expr = true;
+      ag.arg_type = ag.plan.root_type;
+      ag.cls = cls_of(ag.arg_type);
+      DF_CHECK(ag.cls != C_BOOL || ag.func == DFGPU_AGG_COUNT, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Boolean arguments only for COUNT");
+      if (ag.func == DFGPU_AGG_AVG) {
+        DF_CHECK(ag.arg_type == DFGPU_FLOAT64 || ag.cls == C_DEC, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: AVG takes a Float64 (the planner casts) or Decimal128 argument");
+        DF_CHECK(ag.cls != C_DEC || mode != DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: AVG over Decimal128 runs in Single modes only");
+      }
+      if ((ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX)) DF_CHECK(ag.arg_type != DFGPU_FLOAT32, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: MIN/MAX over Float32 stays on dfgpu_agg");
+    }
+    out.push_back(std::move(ag));
+  }
+  return out;
+}
+
+// accumulator words of a record, taken from word `next` (the row counter already taken) up to `budget` (exclusive); `next` ends past the
+// last word taken.  Without pairs: every aggregate's words in order.  With pairs (a Decimal128 MIN / MAX is a {lo, hi} pair updated by one
+// 16-byte CAS, so it sits on an even word of a record of an even number of words, `even_record`): at most one padding word to reach an
+// even word, the pairs, then the other aggregates in order.  Spare words (the padding word first) become non-null counters.
+static void layout_agg_words(std::vector<PipeAgg>& aggs, int& next, int budget, bool even_record) {
+  auto is_pair = [](const PipeAgg& ag) { return ag.cls == C_DEC && (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX); };
+  bool pairs = false;
+  for (const auto& ag : aggs) pairs = pairs || (ag.has_expr && is_pair(ag));
+  auto take = [&](const char* what) { DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, what); return next++; };
+  int pad = -1;
+  if (pairs) {
+    DF_CHECK(even_record, DFGPU_ERR_UNSUPPORTED,
+             "pipeline aggregate: a Decimal128 MIN / MAX needs a record of an even number of words: a lookup without payload takes an odd n_acc_words");
+    if (next & 1) pad = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
+    for (auto& ag : aggs) {
+      if (!is_pair(ag)) continue;
+      ag.word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
+      take("pipeline aggregate: a Decimal128 MIN / MAX takes two accumulator words (n_acc_words)");
+    }
+  }
+  for (auto& ag : aggs) {
+    if (ag.func == DFGPU_AGG_COUNT_STAR || is_pair(ag)) continue;
+    ag.word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
+    if (ag.cls == C_DEC && ag.func == DFGPU_AGG_SUM) take("pipeline aggregate: a Decimal128 SUM takes two accumulator words (n_acc_words)");
+    if (ag.cls == C_DEC && ag.func == DFGPU_AGG_AVG) take("pipeline aggregate: a Decimal128 AVG takes three accumulator words (n_acc_words)");
+    if (ag.func == DFGPU_AGG_AVG) { ag.cnt_word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)"); ag.nn_word = ag.cnt_word; }
+  }
+  // spare words become non-null counters (SUM / MIN / MAX of a nullable argument are NULL until a value arrives, accumulate.rs:164-188)
+  for (auto& ag : aggs) {
+    if (ag.func != DFGPU_AGG_SUM && ag.func != DFGPU_AGG_MIN && ag.func != DFGPU_AGG_MAX) continue;
+    if (pad >= 0) { ag.nn_word = pad; pad = -1; }
+    else if (next < budget) ag.nn_word = next++;
+  }
 }
 
 }  // namespace dfgpu
@@ -2552,66 +2835,61 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   dfgpu_lookup* l = p->stages[stage].lookup;
   DF_CHECK(!l->acc_claimed, DFGPU_ERR_STATE, "pipeline aggregate: the lookup's accumulators are already in use");
   const int base = 1 + (l->has_payload ? 1 : 0);
-  int next = base, budget = base + l->opt.n_acc_words;
-  DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: the lookup reserves no accumulator words (n_acc_words)");
+  int next = base;
+  DF_CHECK(next < base + l->opt.n_acc_words, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: the lookup reserves no accumulator words (n_acc_words)");
   const int rows_word = next++;
-  std::vector<PipeAgg> new_aggs;   // committed only when every check has passed
-  // a Decimal128 MIN / MAX is a {lo, hi} pair updated by one 16-byte CAS: it sits on an even word of a record of an even number of words
-  auto is_pair = [](const PipeAgg& ag) { return ag.cls == C_DEC && (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX); };
-  bool pairs = false;
-  for (int a = 0; a < n_aggs; ++a) {
-    PipeAgg ag;
-    ag.func = aggs[a].func;
-    DF_CHECK(ag.func >= DFGPU_AGG_SUM && ag.func <= DFGPU_AGG_COUNT_STAR, DFGPU_ERR_INVALID, "pipeline aggregate: unknown function");
-    if (ag.func != DFGPU_AGG_COUNT_STAR) {
-      DF_CHECK(aggs[a].expr && aggs[a].n_nodes > 0, DFGPU_ERR_INVALID, "pipeline aggregate: missing argument expression");
-      ag.plan = plan_expr(p->vtypes.data(), (int)p->vtypes.size(), aggs[a].expr, aggs[a].n_nodes);
-      ag.has_expr = true;
-      ag.arg_type = ag.plan.root_type;
-      ag.cls = cls_of(ag.arg_type);
-      DF_CHECK(ag.cls != C_BOOL || ag.func == DFGPU_AGG_COUNT, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Boolean arguments only for COUNT");
-      if (ag.func == DFGPU_AGG_AVG) {
-        DF_CHECK(ag.arg_type == DFGPU_FLOAT64 || ag.cls == C_DEC, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: AVG takes a Float64 (the planner casts) or Decimal128 argument");
-        DF_CHECK(ag.cls != C_DEC || mode != DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: AVG over Decimal128 runs in Single modes only");
-      }
-      if ((ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX)) DF_CHECK(ag.arg_type != DFGPU_FLOAT32, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: MIN/MAX over Float32 stays on dfgpu_agg");
-      pairs = pairs || is_pair(ag);
-    }
-    new_aggs.push_back(std::move(ag));
-  }
-  // accumulator words.  Without pairs: the row counter, then every aggregate's words in order.  With pairs: the row counter, at most one
-  // padding word to reach an even word, the pairs, then the other aggregates in order.  Spare words (the padding word first) become
-  // non-null counters.
-  auto take = [&](const char* what) { DF_CHECK(next < budget, DFGPU_ERR_UNSUPPORTED, what); return next++; };
-  int pad = -1;
-  if (pairs) {
-    DF_CHECK(l->stride % 2 == 0, DFGPU_ERR_UNSUPPORTED,
-             "pipeline aggregate: a Decimal128 MIN / MAX needs a record of an even number of words: a lookup without payload takes an odd n_acc_words");
-    if (next & 1) pad = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
-    for (auto& ag : new_aggs) {
-      if (!is_pair(ag)) continue;
-      ag.word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
-      take("pipeline aggregate: a Decimal128 MIN / MAX takes two accumulator words (n_acc_words)");
-    }
-  }
-  for (auto& ag : new_aggs) {
-    if (ag.func == DFGPU_AGG_COUNT_STAR || is_pair(ag)) continue;
-    ag.word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)");
-    if (ag.cls == C_DEC && ag.func == DFGPU_AGG_SUM) take("pipeline aggregate: a Decimal128 SUM takes two accumulator words (n_acc_words)");
-    if (ag.cls == C_DEC && ag.func == DFGPU_AGG_AVG) take("pipeline aggregate: a Decimal128 AVG takes three accumulator words (n_acc_words)");
-    if (ag.func == DFGPU_AGG_AVG) { ag.cnt_word = take("pipeline aggregate: not enough accumulator words in the lookup (n_acc_words)"); ag.nn_word = ag.cnt_word; }
-  }
-  // spare words become non-null counters (SUM / MIN / MAX of a nullable argument are NULL until a value arrives, accumulate.rs:164-188)
-  for (auto& ag : new_aggs) {
-    if (ag.func != DFGPU_AGG_SUM && ag.func != DFGPU_AGG_MIN && ag.func != DFGPU_AGG_MAX) continue;
-    if (pad >= 0) { ag.nn_word = pad; pad = -1; }
-    else if (next < budget) ag.nn_word = next++;
-  }
+  std::vector<PipeAgg> new_aggs = parse_pipe_aggs(p, aggs, n_aggs, mode);   // committed only when every check has passed
+  layout_agg_words(new_aggs, next, base + l->opt.n_acc_words, l->stride % 2 == 0);
   p->rows_word = rows_word;
   p->group_cols.assign(group_cols, group_cols + n_group);
   p->aggs = std::move(new_aggs);
   l->acc_claimed = true;
   p->agg_stage = stage; p->agg_mode = mode; p->batch_size = batch_size; p->sink = SINK_AGG;
+  DF_API_END
+}
+
+int dfgpu_pipeline_sink_aggregate_hash(dfgpu_pipeline* p, const int32_t* group_cols, const int32_t* group_nullable, int32_t n_group,
+                                       const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size, int64_t capacity_hint) {
+  DF_API_BEGIN(p ? p->ctx : nullptr)
+  DF_CHECK(p && group_cols && n_group >= 1, DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  DF_CHECK(n_group <= kHashMaxKeys, DFGPU_ERR_UNSUPPORTED, "pipeline hash aggregate: 1..8 group columns");
+  DF_CHECK(mode == DFGPU_AGG_SINGLE || mode == DFGPU_AGG_SINGLE_PARTITIONED || mode == DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Single / SinglePartitioned / Partial");
+  DF_CHECK(capacity_hint >= 0, DFGPU_ERR_INVALID, "pipeline hash aggregate: negative capacity_hint");
+  for (auto& st : p->stages) DF_CHECK(st.kind != DFGPU_STAGE_MAYBE, DFGPU_ERR_UNSUPPORTED, "pipeline hash aggregate: a MAYBE stage's false positives would be counted");
+  // the packed tag: each column at its width, then its NULL bit when it is nullable; at most 128 bits
+  std::vector<HashKey> keys(n_group);
+  int bit = 0;
+  for (int g = 0; g < n_group; ++g) {
+    const int c = group_cols[g];
+    DF_CHECK(c >= 0 && c < (int)p->vtypes.size(), DFGPU_ERR_INVALID, "pipeline hash aggregate: group column out of range");
+    DF_CHECK(key_type_ok(p->vtypes[c]), DFGPU_ERR_UNSUPPORTED, "pipeline hash aggregate: group keys must be integer-like columns of <= 64 bits");
+    keys[g].src = c; keys[g].bits = 8 * type_width(p->vtypes[c]); keys[g].shift = bit;
+    bit += keys[g].bits;
+    keys[g].null_bit = (group_nullable && group_nullable[g]) ? bit++ : -1;
+  }
+  DF_CHECK(bit <= 128, DFGPU_ERR_UNSUPPORTED, "pipeline hash aggregate: the group key is wider than 128 bits — use the unfused dfgpu_agg");
+  std::vector<PipeAgg> new_aggs = parse_pipe_aggs(p, aggs, n_aggs, mode);
+  int next = 3;   // words 0 and 1: the tag; word 2: the row counter
+  layout_agg_words(new_aggs, next, kHashMaxWords, true);
+  p->hash_stride = next + (next & 1);
+  p->hash_ident.assign(p->hash_stride, 0ull);
+  p->hash_ident[0] = p->hash_ident[1] = kEmptyKey;
+  for (const PipeAgg& ag : new_aggs) {   // MIN / MAX identities
+    if (ag.func != DFGPU_AGG_MIN && ag.func != DFGPU_AGG_MAX) continue;
+    const bool is_min = ag.func == DFGPU_AGG_MIN;
+    unsigned long long& lo = p->hash_ident[ag.word];
+    if (ag.cls == C_DEC) { lo = is_min ? ~0ull : 0ull; p->hash_ident[ag.word + 1] = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN; }
+    else if (ag.cls == C_F64) { const double d = is_min ? INFINITY : -INFINITY; memcpy(&lo, &d, 8); }
+    else if (ag.cls == C_U64) lo = is_min ? ~0ull : 0ull;
+    else lo = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN;
+  }
+  p->hash_keys = std::move(keys);
+  p->hash_cap_hint = capacity_hint;
+  p->rows_word = 2;
+  p->group_cols.assign(group_cols, group_cols + n_group);
+  p->aggs = std::move(new_aggs);
+  p->agg_mode = mode; p->batch_size = batch_size; p->sink = SINK_HASH;
   DF_API_END
 }
 
@@ -2776,6 +3054,8 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name) {
   if (s == "ring_launches") return p->m_ring_launches;   // launches of the ring-fed pipeline kernel
   if (s == "dense_block_launches") return p->m_dense_block_launches;   // dense sink launches with one accumulator copy per block (shared atomics)
   if (s == "partitioned_launches") return p->m_partitioned_launches;   // aggregate sink pushes probed from radix-partitioned records
+  if (s == "group_rehashes") return p->m_group_rehashes;               // hash aggregate sink: times its group table grew
+  if (s == "replayed_rows") return p->m_replayed_rows;                 // hash aggregate sink: rows deferred by the claim budget and pushed again
   return -1;
 }
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p) {

@@ -689,9 +689,10 @@ class GpuPipelineExec(ExecutionPlan):
 
     def __init__(self, scan: _Scan, sink: str, key: Optional[str] = None, payload: Sequence[str] = (), group_by: Sequence[str] = (),
                  aggs: Sequence[Tuple[str, Optional[Expr], str]] = (), mode: str = "Single", out_schema: Optional[pa.Schema] = None,
-                 key_range: Sequence[Tuple[int, int]] = ()):
+                 key_range: Sequence[Tuple[int, int]] = (), nullable: Sequence[bool] = ()):
         self.scan, self.sink, self.key, self.payload, self.group_by, self.aggs, self.mode = scan, sink, key, list(payload), list(group_by), list(aggs), mode
         self.key_range = list(key_range)   # dense sink: the declared (min, max) of every group column
+        self.nullable = list(nullable)     # hash sink: the declared nullability of every group column
         self.schema = out_schema if out_schema is not None else pa.schema([])
         self.n_acc_words = 0
         self._metrics = {}
@@ -740,14 +741,14 @@ class GpuPipelineExec(ExecutionPlan):
         return D.Pipeline(ctx.gpu, [type_id(f.type) for f in ssch], nodes, stages), keep
 
     def execute(self, ctx):
-        assert self.sink in ("aggregate", "dense"), "build pipelines are driven by their consumer"
+        assert self.sink in ("aggregate", "dense", "hash"), "build pipelines are driven by their consumer"
         vs = self.scan.virtual_schema()
         pipe, keep = self._make_pipeline(ctx)
         try:
             aggs = []
             for func, expr, _ in self.aggs:
                 if expr is None:
-                    aggs.append((D.AGG_COUNT_STAR if self.sink == "dense" else _AGG_FUNCS[func], None))
+                    aggs.append((D.AGG_COUNT_STAR if self.sink in ("dense", "hash") else _AGG_FUNCS[func], None))
                 else:
                     nodes: list = []
                     expr.rpn(vs, nodes)
@@ -755,6 +756,8 @@ class GpuPipelineExec(ExecutionPlan):
             gcols = [vs.get_field_index(g) for g in self.group_by]
             if self.sink == "dense":
                 pipe.sink_aggregate_dense(gcols, self.key_range, aggs, _AGG_MODES[self.mode], 0)
+            elif self.sink == "hash":
+                pipe.sink_aggregate_hash(gcols, aggs, _AGG_MODES[self.mode], 0, 0, self.nullable)
             else:
                 pipe.sink_aggregate(gcols, aggs, _AGG_MODES[self.mode], 0)
             for rb in self.scan.source.execute(ctx):
@@ -924,6 +927,64 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
         return plan
     build.n_acc_words = n_acc
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
+
+
+def fuse_hash_aggregates(plan: ExecutionPlan) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_pipelines: its result when that rule fuses; otherwise an
+    AggregateExec(Single / SinglePartitioned / Partial) with at least one GROUP BY column over [ProjectionExec] over an Inner join chain or a
+    FilterExec (as _as_scan accepts them) becomes ONE GpuPipelineExec with the hash-keyed sink (dfgpu_pipeline_sink_aggregate_hash: TPC-H
+    Q15's revenue0, Q3 grouped by o_custkey).  Every group key must be a plain integer-like column of the virtual schema, the packed key
+    (each column at its width, one more bit per nullable column) at most 128 bits; no FILTER clause, at most 4 aggregates, and the argument
+    types the library accepts.  Anything else, a bare scan included, is returned unchanged (dfgpu_agg runs)."""
+    fused = fuse_pipelines(plan)
+    if fused is not plan:
+        return fused
+    if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial") or not plan.group_by:
+        return plan
+    below, proj = plan.input, None
+    if isinstance(below, GpuProjectionExec):
+        proj, below = below, below.input
+    if not ((isinstance(below, GpuHashJoinExec) and below.join_type == "Inner") or isinstance(below, GpuFilterExec)):
+        return plan
+    sc = _as_scan(below)
+    if sc is None:
+        return plan
+    vs = sc.virtual_schema()
+    exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
+    group, nullable, bits = [], [], 0
+    for g in plan.group_by:
+        e = exprs.get(g)
+        if not isinstance(e, Column) or e.name not in sc.visible or vs.get_field_index(e.name) < 0:
+            return plan
+        f = vs.field(e.name)
+        if not (pa.types.is_integer(f.type) or pa.types.is_date32(f.type) or pa.types.is_date64(f.type) or pa.types.is_timestamp(f.type)):
+            return plan
+        bits += D.WIDTH[type_id(f.type)] * 8 + (1 if f.nullable else 0)
+        group.append(e.name)
+        nullable.append(f.nullable)
+    if bits > 128 or len(plan.aggr_expr) > 4:
+        return plan
+    aggs = []
+    for a in plan.aggr_expr:
+        if a.filter is not None:
+            return plan
+        e = None if a.arg is None else exprs.get(a.arg)
+        if a.arg is not None and e is None:
+            return plan
+        if e is not None:
+            try:
+                e.rpn(vs, [])                              # every referenced name must exist in the virtual schema
+                t = e.data_type(vs)
+            except KeyError:
+                return plan
+            if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
+                return plan                                # AVG(Decimal128) has no pinned Partial state
+            if a.func in ("min", "max") and t == pa.float32():
+                return plan
+            if pa.types.is_boolean(t) and a.func != "count":
+                return plan
+        aggs.append((a.func, e, a.alias))
+    return GpuPipelineExec(sc, sink="hash", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, nullable=nullable)
 
 
 def collect(plan: ExecutionPlan, ctx: Optional[TaskContext] = None) -> List[pa.RecordBatch]:

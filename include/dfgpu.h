@@ -500,6 +500,30 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
 #define DFGPU_DENSE_MAX_GROUPS 256
 int dfgpu_pipeline_sink_aggregate_dense(dfgpu_pipeline* p, const int32_t* group_cols, const int64_t* key_min, const int64_t* key_max,
                                         int32_t n_group, const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size);
+/* hash aggregate: AggregateExec over the surviving rows whose GROUP BY keys the join key does not determine (TPC-H Q15's revenue0:
+ * l_suppkey; Q3 grouped by o_custkey).  The sink owns its group table.
+ *  group_cols: 1..8 virtual columns (input columns or payload fields of INNER stages), integer-like, <= 8 bytes (Int8..Int64,
+ *    UInt8..UInt64, Date32, Date64, Timestamp; dictionary-coded strings as their Int32 codes).  group_nullable[g] is the column's
+ *    declared nullability (DataFusion's Field::is_nullable); NULL = none is nullable.  The columns are packed into a 128-bit tag,
+ *    each at its width followed by one NULL bit when it is nullable; a key wider than 128 bits is DFGPU_ERR_UNSUPPORTED (dfgpu_agg
+ *    carries wide keys).  NULL is a group of its own; a NULL in a column declared non-nullable is DFGPU_ERR_INVALID at the push.
+ *  aggs: the functions, limits and result / state types of dfgpu_pipeline_sink_aggregate (<= 4; COUNT(*), COUNT, SUM, MIN, MAX, AVG
+ *    over Float64 and Decimal128; Decimal128 AVG in Single modes only; MIN / MAX over Float32 rejected).  The sink sizes the record
+ *    words itself: {tag_lo | tag_hi | row counter | the aggregates' words as dfgpu_pipeline_sink_aggregate lays them out, every SUM /
+ *    MIN / MAX with a non-null counter}.
+ *  mode: DFGPU_AGG_SINGLE, DFGPU_AGG_SINGLE_PARTITIONED or DFGPU_AGG_PARTIAL (the state columns dfgpu_agg emits: its Final consumes them).
+ *  MAYBE stages are rejected (their false positives would be counted).
+ *  Output: one row per group, group columns then aggregates, in slot order (unspecified), sliced by batch_size.
+ *  capacity_hint: the expected number of groups (0 = unknown); it sizes the first table only, results never depend on it.
+ *  Growth: a push runs in row chunks of at most 2^26 rows (the first one max(2^20, capacity / 2) rows, then x4); before a chunk the
+ *    table grows x4 when groups x 2 > capacity.  Inside the kernel claims stop at 5/8 of the capacity: a row whose group cannot be
+ *    claimed is deferred (its row number goes to an overflow list bounded by the chunk's rows) before it touches any accumulator; the
+ *    table grows x4 and the deferred rows are pushed again until none is left.  A table beyond 2^32 records is DFGPU_ERR_UNSUPPORTED.
+ *  Metrics: "num_groups", "sink_rows" (every surviving row once, replayed rows included), "group_rehashes" (times the table grew),
+ *    "replayed_rows" (rows deferred and pushed again). */
+int dfgpu_pipeline_sink_aggregate_hash(dfgpu_pipeline* p, const int32_t* group_cols, const int32_t* group_nullable, int32_t n_group,
+                                       const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size,
+                                       int64_t capacity_hint);
 int dfgpu_pipeline_sink_output(dfgpu_pipeline* p, const int32_t* out_cols, int32_t n_out, int64_t batch_size);
 /* the same, row order unspecified (what a RepartitionExec consumer sees anyway, repartition/mod.rs:1320-1400): runs on the two-phase
  * kernel and is several times faster than the ordered sink on selective pipelines */
@@ -512,7 +536,8 @@ int dfgpu_pipeline_push_device(dfgpu_pipeline* p, const dfgpu_column* cols, int3
 int dfgpu_pipeline_push_arrow(dfgpu_pipeline* p, const struct ArrowArray* batch, const struct ArrowSchema* schema);
 int dfgpu_pipeline_finish(dfgpu_pipeline* p);
 int dfgpu_pipeline_next(dfgpu_pipeline* p, int host, dfgpu_batch** out);
-int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches","dense_block_launches","partitioned_launches" */
+int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches","dense_block_launches","partitioned_launches",
+                                                                      "group_rehashes","replayed_rows" */
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p);
 
 /* ===================================================================================== */
