@@ -378,6 +378,8 @@ constexpr int kRadixSubTableMB = 16;   // table bytes per partition, a third of 
 constexpr int kRadixMaxParts = 64, kRadixMetaWords = 3 * kRadixMaxParts + 1;
 int radix_partition(dfgpu_ctx* ctx, const unsigned long long* keys, const unsigned long long* vals, int64_t n, size_t table_bytes, int force_parts,
                     void* out, unsigned long long* meta);
+// The same for n rows that are already 16-byte {key, val} records (recs 16-byte aligned): each 2048-row tile arrives by one bulk copy.
+int radix_partition_records(dfgpu_ctx* ctx, const void* recs, int64_t n, size_t table_bytes, int force_parts, void* out, unsigned long long* meta);
 
 // ------------------------------------------------------------------------------------------
 // device bit helpers (Arrow validity bitmaps are LSB-numbered)

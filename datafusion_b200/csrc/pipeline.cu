@@ -1437,6 +1437,56 @@ __global__ void __launch_bounds__(256) lookup_insert_records_kernel(LookupDev t,
   fail = __any_sync(0xffffffffu, fail & 1) | (__any_sync(0xffffffffu, fail & 2) << 1);
   if ((threadIdx.x & 31) == 0) { if (ins) atomicAdd(&counters[1], (unsigned long long)ins); if (fail) atomicOr(&counters[2], (unsigned long long)fail); }
 }
+// the same insert for records radix-partitioned by slot range (radix_partition_records), with the same counters.  Tiles are taken in
+// record order from one counter (pipe_probe_agg_kernel's scheme), so the running blocks insert into one ~16 MB slot range of the table at
+// a time and its sectors come from DRAM about once.  A thread first prefetches the start slots of its tile's four records into L2, so
+// their misses overlap instead of stalling one 128-bit CAS after the other.  The caller detaches the membership filter from `t`
+// (lookup_filter_records_kernel sets it): lk_insert then makes no filter update.
+__global__ void __launch_bounds__(256) lookup_insert_part_kernel(LookupDev t, const ulonglong2* __restrict__ recs, int64_t n, int unique,
+                                                                 unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ counters /* [_, inserted, fail] */) {
+  constexpr int ITEMS = 4, TILE = 256 * ITEMS;
+  __shared__ unsigned int s_tile;
+  const int64_t ntiles = (n + TILE - 1) / TILE;
+  unsigned int ins = 0; int fail = 0;
+  while (true) {
+    __syncthreads();
+    if (threadIdx.x == 0) s_tile = atomicAdd(tile_counter, 1u);   // tiles in record order: the running blocks share one slot range
+    __syncthreads();
+    const int64_t tile = s_tile;
+    if (tile >= ntiles) break;
+    ulonglong2 r[ITEMS];
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const int64_t i = tile * TILE + k * 256 + threadIdx.x;
+      if (i < n) { const int4 v = ld_stream_16(recs + i); r[k].x = (uint64_t)(uint32_t)v.x | ((uint64_t)(uint32_t)v.y << 32); r[k].y = (uint64_t)(uint32_t)v.z | ((uint64_t)(uint32_t)v.w << 32); }
+    }
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k)
+      if (tile * TILE + k * 256 + threadIdx.x < n) asm volatile("prefetch.global.L2 [%0];" :: "l"(t.recs + __umul64hi(lk_hash(r[k].x), t.cap) * (uint64_t)t.stride));
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      if (tile * TILE + k * 256 + threadIdx.x >= n) continue;
+      const int rc = lk_insert(t, r[k].x, r[k].y);
+      if (rc == 0) ins++;
+      else if (rc == 2 || unique) fail |= rc;
+    }
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) ins += __shfl_xor_sync(0xffffffffu, ins, d);
+  fail = __any_sync(0xffffffffu, fail & 1) | (__any_sync(0xffffffffu, fail & 2) << 1);
+  if ((threadIdx.x & 31) == 0) { if (ins) atomicAdd(&counters[1], (unsigned long long)ins); if (fail) atomicOr(&counters[2], (unsigned long long)fail); }
+}
+// the membership filter of n packed records, set in a sweep of its own: inside lookup_insert_part_kernel its random updates would compete
+// with the table's slot range for L2, while here the filter (Q3 SF100: 29 MB) stays in L2 and the records stream past it at evict-first
+// priority.  The bits equal lk_insert's: a duplicate key sets the bits its first copy set, and the reserved all-ones key, which lk_insert
+// rejects, sets none.
+__global__ void __launch_bounds__(256) lookup_filter_records_kernel(LookupDev t, const ulonglong2* __restrict__ recs, int64_t n) {
+  const uint64_t pol = policy_evict_first();
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint64_t key = ld_stream_int(recs + i, 8, 0, 0, pol);
+    if (key != kEmptyKey) filter_set(t, key);
+  }
+}
 // accumulator identities for MIN / MAX (SUM / COUNT start at the zero the table was initialised with)
 __global__ void __launch_bounds__(256) lookup_init_acc_kernel(LookupDev t, int word, unsigned long long value) {
   for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < t.cap; s += (uint64_t)gridDim.x * blockDim.x) t.recs[s * (uint64_t)t.stride + word] = value;
@@ -1651,7 +1701,8 @@ struct dfgpu_pipeline {
   bool finished = false;
   DevBuf params_dev, counters;
   std::deque<BatchPtr> outq;
-  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0, m_dense_block_launches = 0, m_partitioned_launches = 0;
+  int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0, m_dense_block_launches = 0, m_partitioned_launches = 0,
+          m_partitioned_inserts = 0;
   std::string name;   // optional label: the kernel-timing family becomes "pipe:<name>" (dfgpu_kernel_time)
 };
 
@@ -1670,6 +1721,10 @@ static LookupDev lookup_dev(const dfgpu_lookup* l) {
 
 static bool key_type_ok(int t) { int w = type_width(t); return w >= 1 && w <= 8 && !type_is_float(t) && t != DFGPU_BOOL; }
 
+// A lookup table larger than this does not stay in the 50 MB L2: it gets a Bloom filter (membership_filter < 0), and the fused pipeline
+// partitions its build records (pipeline_push) and the probe records of its aggregate sink (partitioned_table_bytes) by slot range.
+constexpr size_t kL2TableBytes = 40ull << 20;
+
 // (re)allocate a hash lookup for at least `rows` records at load factor <= 0.5; existing records are rehashed
 static void lookup_reserve(dfgpu_lookup* l, int64_t rows) {
   if (l->mode != LK_HASH || l->filter_only) return;
@@ -1683,7 +1738,7 @@ static void lookup_reserve(dfgpu_lookup* l, int64_t rows) {
   DF_LAUNCH_CHECK(ctx);
   uint64_t nblocks = 0;
   const size_t table_bytes = (size_t)new_cap * l->stride * 8;
-  if (l->opt.membership_filter == 1 || (l->opt.membership_filter < 0 && table_bytes > (40ull << 20))) {   // a table that does not fit the 50 MB L2
+  if (l->opt.membership_filter == 1 || (l->opt.membership_filter < 0 && table_bytes > kL2TableBytes)) {
     nblocks = std::max<uint64_t>(1024, new_cap / 8);   // 16 bits per key at load factor 0.5
     nbloom.alloc(ctx, (size_t)nblocks * 8);
     nbloom.zero();
@@ -2080,7 +2135,7 @@ static size_t partitioned_table_bytes(const dfgpu_pipeline* p, const PipeParams&
   if (pp.n_aggs != 1 || a.small != 2 || a.func != DFGPU_AGG_SUM || a.cls == C_F64 || a.cls == C_DEC || a.nn_word >= 0) return 0;
   for (int i = 0; i < a.n; ++i) if (pp.pool[a.start + i].kind == kExprExt) return 0;
   const size_t bytes = (size_t)st.lk.cap * st.lk.stride * 8;
-  return bytes > (40ull << 20) || force_parts >= 2 ? bytes : 0;
+  return bytes > kL2TableBytes || force_parts >= 2 ? bytes : 0;
 }
 
 // ---- hash-keyed aggregate sink ----
@@ -2215,10 +2270,35 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
       const int64_t packed = (int64_t)h8[4];
       lookup_reserve(t, t->rows + packed);
       p->counters.zero();
-      if (packed > 0) {
+      const int unique = (t->has_payload || t->opt.n_acc_words > 0) ? 1 : 0;
+      // a table larger than L2 takes its records one slot range at a time: partitioned first, like the aggregate sink's probe records
+      // (DFGPU_PIPE_RADIX_PARTS, a test hook, forces P and this path on small tables)
+      const size_t table_bytes = (size_t)t->cap * t->stride * 8;
+      const int force_parts = getenv("DFGPU_PIPE_RADIX_PARTS") ? atoi(getenv("DFGPU_PIPE_RADIX_PARTS")) : 0;
+      DevBuf parts, meta;   // released after read_counters' synchronise
+      if (packed > 0 && (table_bytes > kL2TableBytes || force_parts >= 2)) {
+        parts.alloc(ctx, (size_t)packed * 16); meta.alloc(ctx, (size_t)(kRadixMetaWords + 1) * 8);
+        meta.zero();
+        {
+          KernelTimer kt(ctx, "lookup_partition");
+          radix_partition_records(ctx, recs.ptr, packed, table_bytes, force_parts, parts.ptr, meta.as<unsigned long long>());
+        }
+        recs.release();
+        KernelTimer kt(ctx, "lookup_insert");   // both kernels: the time of the insert the unpartitioned path makes in one
+        LookupDev d = lookup_dev(t);
+        if (d.bloom) {
+          lookup_filter_records_kernel<<<grid_for(packed, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(d, parts.as<ulonglong2>(), packed);
+          DF_LAUNCH_CHECK(ctx);
+          d.bloom = nullptr; d.coarse = nullptr;
+        }
+        lookup_insert_part_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(d, parts.as<ulonglong2>(), packed, unique, (unsigned int*)(meta.as<unsigned long long>() + kRadixMetaWords),
+                                                                     p->counters.as<unsigned long long>());
+        DF_LAUNCH_CHECK(ctx);
+        p->m_partitioned_inserts++;
+      } else if (packed > 0) {
         KernelTimer kt(ctx, "lookup_insert");
-        lookup_insert_records_kernel<<<grid_for(packed, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(lookup_dev(t), (const ulonglong2*)recs.ptr, packed,
-                                                                                                   (t->has_payload || t->opt.n_acc_words > 0) ? 1 : 0, p->counters.as<unsigned long long>());
+        lookup_insert_records_kernel<<<grid_for(packed, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(lookup_dev(t), (const ulonglong2*)recs.ptr, packed, unique,
+                                                                                                   p->counters.as<unsigned long long>());
         DF_LAUNCH_CHECK(ctx);
       }
       read_counters(p, h);
@@ -3054,6 +3134,7 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name) {
   if (s == "ring_launches") return p->m_ring_launches;   // launches of the ring-fed pipeline kernel
   if (s == "dense_block_launches") return p->m_dense_block_launches;   // dense sink launches with one accumulator copy per block (shared atomics)
   if (s == "partitioned_launches") return p->m_partitioned_launches;   // aggregate sink pushes probed from radix-partitioned records
+  if (s == "partitioned_inserts") return p->m_partitioned_inserts;     // build sink pushes inserted from radix-partitioned records
   if (s == "group_rehashes") return p->m_group_rehashes;               // hash aggregate sink: times its group table grew
   if (s == "replayed_rows") return p->m_replayed_rows;                 // hash aggregate sink: rows deferred by the claim budget and pushed again
   return -1;

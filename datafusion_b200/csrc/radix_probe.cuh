@@ -1,5 +1,6 @@
 // radix_probe.cuh — intra-GPU radix-partitioned probe of the inline join table (included by hash_join.cu only; radix_partition, declared
-// in common.cuh, also partitions the probe records of the fused pipeline's aggregate sink, pipeline.cu).
+// in common.cuh, also partitions the probe records of the fused pipeline's aggregate sink, and radix_partition_records the packed build
+// records of its lookups, pipeline.cu).
 //
 // Reference analogue: PartitionMode::Partitioned — both join inputs go through BatchPartitioner::Hash
 // (physical-plan/src/repartition/mod.rs:1097-1145) so that every partition's hash table is small enough to stay in
@@ -26,21 +27,36 @@ constexpr int kRadixTile = 2048, kRadixThreads = 256, kRadixPerThread = kRadixTi
 
 __device__ __forceinline__ int radix_part(uint64_t key, int bits) { return (int)(hash_u64(key, kSeedJoin) >> (64 - bits)); }
 
-__global__ void __launch_bounds__(256) radix_hist_kernel(const unsigned long long* __restrict__ keys, int64_t n, int bits, unsigned long long* __restrict__ counts) {
+// The partition kernels read their rows from one of two layouts: RECS = false, a key array and a value array; RECS = true, interleaved
+// 16-byte {key, value} records (row i: key at keys[2 i], value at keys[2 i + 1]; vals unused), the fused pipeline's packed build rows.
+template <bool RECS>
+__device__ __forceinline__ void radix_hist_body(const unsigned long long* __restrict__ keys, int64_t n, int bits, unsigned long long* __restrict__ counts) {
   __shared__ unsigned int s_cnt[kRadixMaxParts];
   if (threadIdx.x < kRadixMaxParts) s_cnt[threadIdx.x] = 0;
   __syncthreads();
-  // two keys per 128-bit load
+  // two rows per iteration: one 128-bit load of two keys, or two of two records
   const int64_t n2 = n / 2;
   for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n2; i += (int64_t)gridDim.x * blockDim.x) {
-    const int4 v = ld_stream_16(keys + 2 * i);
-    const uint64_t a = (uint64_t)(uint32_t)v.x | ((uint64_t)(uint32_t)v.y << 32), b = (uint64_t)(uint32_t)v.z | ((uint64_t)(uint32_t)v.w << 32);
+    uint64_t a, b;
+    if constexpr (RECS) {
+      const int4 u = ld_stream_16(keys + 4 * i), v = ld_stream_16(keys + 4 * i + 2);
+      a = (uint64_t)(uint32_t)u.x | ((uint64_t)(uint32_t)u.y << 32); b = (uint64_t)(uint32_t)v.x | ((uint64_t)(uint32_t)v.y << 32);
+    } else {
+      const int4 v = ld_stream_16(keys + 2 * i);
+      a = (uint64_t)(uint32_t)v.x | ((uint64_t)(uint32_t)v.y << 32); b = (uint64_t)(uint32_t)v.z | ((uint64_t)(uint32_t)v.w << 32);
+    }
     atomicAdd(&s_cnt[radix_part(a, bits)], 1u);
     atomicAdd(&s_cnt[radix_part(b, bits)], 1u);
   }
-  if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&s_cnt[radix_part(keys[n - 1], bits)], 1u);
+  if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&s_cnt[radix_part(keys[RECS ? 2 * (n - 1) : n - 1], bits)], 1u);
   __syncthreads();
   if (threadIdx.x < (1 << bits) && s_cnt[threadIdx.x]) atomicAdd(&counts[threadIdx.x], (unsigned long long)s_cnt[threadIdx.x]);
+}
+__global__ void __launch_bounds__(256) radix_hist_kernel(const unsigned long long* __restrict__ keys, int64_t n, int bits, unsigned long long* __restrict__ counts) {
+  radix_hist_body<false>(keys, n, bits, counts);
+}
+__global__ void __launch_bounds__(256) radix_hist_records_kernel(const unsigned long long* __restrict__ recs, int64_t n, int bits, unsigned long long* __restrict__ counts) {
+  radix_hist_body<true>(recs, n, bits, counts);
 }
 
 // exclusive prefix of the P counts -> partition start offsets (cursor[p] = start[p], bounds[p] = start, bounds[P] = n)
@@ -54,10 +70,11 @@ __global__ void radix_prefix_kernel(const unsigned long long* __restrict__ count
 
 struct alignas(16) RadixRec { unsigned long long key, val; };
 
-// Dynamic shared memory: 2 stages x { keys[2048] | vals[2048] } (2 x 32 KB); a stage is reused in place as the 2048 sorted
-// 16-byte records once every thread holds its 8 rows in registers.
-__global__ void __launch_bounds__(kRadixThreads) radix_scatter_tma_kernel(const unsigned long long* __restrict__ keys, const unsigned long long* __restrict__ vals, int64_t n, int bits,
-                                                                         unsigned long long* __restrict__ cursor, RadixRec* __restrict__ out) {
+// Dynamic shared memory: 2 stages x { keys[2048] | vals[2048] } or 2 x { records[2048] } (2 x 32 KB, one bulk copy per array); a
+// stage is reused in place as the 2048 sorted 16-byte records once every thread holds its 8 rows in registers.
+template <bool RECS>
+__device__ __forceinline__ void radix_scatter_body(const unsigned long long* __restrict__ keys, const unsigned long long* __restrict__ vals, int64_t n, int bits,
+                                                   unsigned long long* __restrict__ cursor, RadixRec* __restrict__ out) {
   extern __shared__ __align__(128) unsigned char smem[];
   __shared__ __align__(8) uint64_t s_bar[2];
   __shared__ unsigned int s_cnt[kRadixMaxParts], s_start[kRadixMaxParts + 1];
@@ -71,8 +88,12 @@ __global__ void __launch_bounds__(kRadixThreads) radix_scatter_tma_kernel(const 
   auto issue = [&](int64_t tile, int s) {
     if (tile < ntiles && (tile + 1) * (int64_t)kRadixTile <= n) {
       mbar_expect_tx(&s_bar[s], 2u * kRadixTile * 8u);
-      tma_load_1d(stage_keys[s], keys + tile * kRadixTile, kRadixTile * 8u, &s_bar[s]);
-      tma_load_1d(stage_keys[s] + kRadixTile, vals + tile * kRadixTile, kRadixTile * 8u, &s_bar[s]);
+      if constexpr (RECS) {
+        tma_load_1d(stage_keys[s], keys + 2 * tile * kRadixTile, kRadixTile * 16u, &s_bar[s]);
+      } else {
+        tma_load_1d(stage_keys[s], keys + tile * kRadixTile, kRadixTile * 8u, &s_bar[s]);
+        tma_load_1d(stage_keys[s] + kRadixTile, vals + tile * kRadixTile, kRadixTile * 8u, &s_bar[s]);
+      }
     }
   };
   int64_t tile = blockIdx.x;
@@ -87,12 +108,19 @@ __global__ void __launch_bounds__(kRadixThreads) radix_scatter_tma_kernel(const 
       mbar_wait(&s_bar[s], phase[s]);
       phase[s] ^= 1;
 #pragma unroll
-      for (int i = 0; i < kRadixPerThread; ++i) { k[i] = stage_keys[s][threadIdx.x + i * kRadixThreads]; v[i] = stage_keys[s][kRadixTile + threadIdx.x + i * kRadixThreads]; }
+      for (int i = 0; i < kRadixPerThread; ++i) {
+        if constexpr (RECS) {   // 16-byte shared loads (addressed from smem itself: stage_keys[s] would be a generic pointer)
+          const ulonglong2 r = ((const ulonglong2*)(smem + s * (2 * kRadixTile * 8)))[threadIdx.x + i * kRadixThreads];
+          k[i] = r.x; v[i] = r.y;
+        }
+        else { k[i] = stage_keys[s][threadIdx.x + i * kRadixThreads]; v[i] = stage_keys[s][kRadixTile + threadIdx.x + i * kRadixThreads]; }
+      }
     } else {
 #pragma unroll
       for (int i = 0; i < kRadixPerThread; ++i) {
         const int r = threadIdx.x + i * kRadixThreads;
-        k[i] = r < rows ? keys[tile * kRadixTile + r] : 0ull; v[i] = r < rows ? vals[tile * kRadixTile + r] : 0ull;
+        if constexpr (RECS) { k[i] = r < rows ? keys[2 * (tile * kRadixTile + r)] : 0ull; v[i] = r < rows ? keys[2 * (tile * kRadixTile + r) + 1] : 0ull; }
+        else { k[i] = r < rows ? keys[tile * kRadixTile + r] : 0ull; v[i] = r < rows ? vals[tile * kRadixTile + r] : 0ull; }
       }
     }
     if (threadIdx.x < P) s_cnt[threadIdx.x] = 0;
@@ -131,10 +159,18 @@ __global__ void __launch_bounds__(kRadixThreads) radix_scatter_tma_kernel(const 
     if (threadIdx.x == 0) issue(tile + 2 * (int64_t)gridDim.x, s);   // refill this stage two tiles ahead
   }
 }
+__global__ void __launch_bounds__(kRadixThreads) radix_scatter_tma_kernel(const unsigned long long* __restrict__ keys, const unsigned long long* __restrict__ vals, int64_t n, int bits,
+                                                                         unsigned long long* __restrict__ cursor, RadixRec* __restrict__ out) {
+  radix_scatter_body<false>(keys, vals, n, bits, cursor, out);
+}
+__global__ void __launch_bounds__(kRadixThreads) radix_scatter_records_kernel(const unsigned long long* __restrict__ recs, int64_t n, int bits, unsigned long long* __restrict__ cursor,
+                                                                             RadixRec* __restrict__ out) {
+  radix_scatter_body<true>(recs, nullptr, n, bits, cursor, out);
+}
 
-// hist -> prefix -> TMA scatter (declared in common.cuh: the fused pipeline's aggregate sink partitions its probe records here too)
-int radix_partition(dfgpu_ctx* ctx, const unsigned long long* keys, const unsigned long long* vals, int64_t n, size_t table_bytes, int force_parts,
-                    void* out, unsigned long long* meta) {
+// hist -> prefix -> TMA scatter of either layout (recs: keys holds interleaved {key, value} records)
+static int radix_partition_impl(dfgpu_ctx* ctx, bool recs, const unsigned long long* keys, const unsigned long long* vals, int64_t n, size_t table_bytes, int force_parts,
+                                void* out, unsigned long long* meta) {
   int bits = 1;
   const size_t want = force_parts >= 2 ? (size_t)force_parts : (table_bytes + ((size_t)kRadixSubTableMB << 20) - 1) / ((size_t)kRadixSubTableMB << 20);
   while ((1u << bits) < want && bits < 6) ++bits;
@@ -142,15 +178,27 @@ int radix_partition(dfgpu_ctx* ctx, const unsigned long long* keys, const unsign
   unsigned long long* cursor = counts + kRadixMaxParts;
   unsigned long long* bounds = cursor + kRadixMaxParts;      // [P + 1]
   // the attribute belongs to the current device: set on every call, so any device and thread may partition
-  DF_CUDA(cudaFuncSetAttribute(radix_scatter_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kRadixTile * 8));
-  radix_hist_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(keys, n, bits, counts);
+  DF_CUDA(cudaFuncSetAttribute(recs ? (const void*)radix_scatter_records_kernel : (const void*)radix_scatter_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * kRadixTile * 8));
+  if (recs) radix_hist_records_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(keys, n, bits, counts);
+  else radix_hist_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(keys, n, bits, counts);
   DF_LAUNCH_CHECK(ctx);
   radix_prefix_kernel<<<1, 32, 0, ctx->stream>>>(counts, 1 << bits, cursor, bounds);
   DF_LAUNCH_CHECK(ctx);
   const int64_t rtiles = (n + kRadixTile - 1) / kRadixTile;
-  radix_scatter_tma_kernel<<<(int)std::min<int64_t>(rtiles, kNumSMs * 3), kRadixThreads, 4 * kRadixTile * 8, ctx->stream>>>(keys, vals, n, bits, cursor, (RadixRec*)out);
+  const int grid = (int)std::min<int64_t>(rtiles, kNumSMs * 3);
+  if (recs) radix_scatter_records_kernel<<<grid, kRadixThreads, 4 * kRadixTile * 8, ctx->stream>>>(keys, n, bits, cursor, (RadixRec*)out);
+  else radix_scatter_tma_kernel<<<grid, kRadixThreads, 4 * kRadixTile * 8, ctx->stream>>>(keys, vals, n, bits, cursor, (RadixRec*)out);
   DF_LAUNCH_CHECK(ctx);
   return bits;
+}
+
+// declared in common.cuh: the fused pipeline's aggregate sink partitions its probe records here too
+int radix_partition(dfgpu_ctx* ctx, const unsigned long long* keys, const unsigned long long* vals, int64_t n, size_t table_bytes, int force_parts,
+                    void* out, unsigned long long* meta) {
+  return radix_partition_impl(ctx, false, keys, vals, n, table_bytes, force_parts, out, meta);
+}
+int radix_partition_records(dfgpu_ctx* ctx, const void* recs, int64_t n, size_t table_bytes, int force_parts, void* out, unsigned long long* meta) {
+  return radix_partition_impl(ctx, true, (const unsigned long long*)recs, nullptr, n, table_bytes, force_parts, out, meta);
 }
 
 struct RadixOut {

@@ -537,7 +537,10 @@ int dfgpu_pipeline_push_arrow(dfgpu_pipeline* p, const struct ArrowArray* batch,
 int dfgpu_pipeline_finish(dfgpu_pipeline* p);
 int dfgpu_pipeline_next(dfgpu_pipeline* p, int host, dfgpu_batch** out);
 int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches","dense_block_launches","partitioned_launches",
-                                                                      "group_rehashes","replayed_rows" */
+                                                                      "group_rehashes","replayed_rows",
+                                                                      "partitioned_inserts": build sink pushes whose records went into a
+                                                                      table larger than 40 MB (more than L2 holds) radix-partitioned by
+                                                                      slot range, one L2-sized range at a time */
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p);
 
 /* ===================================================================================== */

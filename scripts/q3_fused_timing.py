@@ -22,7 +22,7 @@ for name, fn in (("fused", Q.run_q3_fused), ("unfused", Q.run_q3)):
         for b in res: b.release()
     ctx.record(e1)
     ms = ctx.elapsed_ms(e0, e1) / 5
-    kt = {k: ctx.kernel_time(k) for k in ("pipe:lineitem", "pipe:orders", "pipeline_count", "pipeline_build", "lookup_insert", "pipeline_agg", "pipeline_output", "join_probe", "join_build", "filter_fused", "agg_update")}
+    kt = {k: ctx.kernel_time(k) for k in ("pipe:lineitem", "pipe:orders", "pipeline_count", "pipeline_build", "lookup_partition", "lookup_insert", "pipeline_agg", "pipeline_output", "join_probe", "join_build", "filter_fused", "agg_update")}
     ctx.set_kernel_timing(False)
     out[name] = {"ms": ms, "stages": st, "fingerprint": fp, "kernel_ms": {k: v[0] / max(v[1], 1) for k, v in kt.items() if v[1]}, "kernel_n": {k: v[1] for k, v in kt.items() if v[1]}}
 print(json.dumps(out, indent=1))
