@@ -1511,20 +1511,27 @@ __global__ void __launch_bounds__(256) hash_rehash_kernel(const unsigned long lo
     }
   }
 }
-// records with rows_word > 0 -> occupancy bitmap (one ballot word per warp)
-__global__ void __launch_bounds__(256) lookup_groups_kernel(LookupDev t, int rows_word, uint32_t* __restrict__ words) {
+// the records to emit -> occupancy bitmap (one ballot word per warp).  sel 0: rows_word > 0 (the records a row reached);
+// 1: occupied records with rows_word == 0 (LEFT_ANTI: the build rows no probe row reached); 2: every occupied record (LEFT)
+__global__ void __launch_bounds__(256) lookup_groups_kernel(LookupDev t, int rows_word, int sel, uint32_t* __restrict__ words) {
   const uint64_t nw = (t.cap + 31) / 32;
   const int lane = threadIdx.x & 31;
   for (uint64_t w = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5; w < nw; w += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
     const uint64_t s = w * 32 + lane;
-    const bool occ = s < t.cap && t.recs[s * (uint64_t)t.stride + rows_word] != 0ull;
+    bool occ = false;
+    if (s < t.cap) {
+      const unsigned long long* r = t.recs + s * (uint64_t)t.stride;
+      const bool hit = r[rows_word] != 0ull;
+      occ = sel == 0 ? hit : (r[0] != kEmptyKey && (sel == 2 || !hit));
+    }
     const uint32_t b = __ballot_sync(0xffffffffu, occ);
     if (lane == 0) words[w] = b;
   }
 }
 struct EmitCol {
   int kind /* 0 key, 1 payload field, 2 accumulator word, 3 AVG value, 4 count as u64, 5 Decimal128 sum / min / max (two words),
-              6 dense group key decoded from the slot number, 7 Decimal128 AVG value, 8 packed group field of a 128-bit tag in words 0 and 1 */,
+              6 dense group key decoded from the slot number, 7 Decimal128 AVG value, 8 packed group field of a 128-bit tag in words 0 and 1,
+              9 COUNT(*) of a LEFT join's build row: the row counter, at least 1 (the NULL-padded row of a record no probe row reached) */,
       width, shift, word, nn_word, cnt_word, f64;
   void* dst; uint32_t* valid;
   long long kmin; int kstride, kradix;   // kind 6: key = kmin + (slot / kstride) % kradix, NULL when that index is kradix - 1
@@ -1549,6 +1556,7 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
           case 1: v = r[1] >> e.shift; break;
           case 2: v = r[e.word]; ok = e.nn_word >= 0 ? r[e.nn_word] != 0ull : true; break;
           case 4: v = r[e.word]; break;
+          case 9: v = max(r[e.word], 1ull); break;
           case 5:
             ok = e.nn_word >= 0 ? r[e.nn_word] != 0ull : true;
             ((unsigned long long*)e.dst)[2 * i] = ok ? r[e.word] : 0ull;
@@ -1670,6 +1678,7 @@ struct dfgpu_lookup {
   DevBuf recs, bloom, bits;
   uint64_t cap = 0, bloom_blocks = 0, coarse_words = 0, kmin = 0, ksize = 0;   // the coarse level lives behind the exact blocks in `bloom`
   int64_t rows = 0, rehashes = 0;
+  int64_t null_keys = 0;   // build rows pushed with a NULL key (counted before the predicate): never inserted, so a LEFT / LEFT_ANTI stage cannot emit them
   bool acc_claimed = false, filter_only = false;
 };
 
@@ -1687,6 +1696,7 @@ struct dfgpu_pipeline {
   dfgpu_lookup* target = nullptr; int bkey_col = -1; std::vector<int> bpay_cols;
   // aggregate sink
   std::vector<int> group_cols; std::vector<PipeAgg> aggs; int agg_mode = DFGPU_AGG_SINGLE, agg_stage = -1, rows_word = -1; bool acc_ready = false;
+  int left_kind = 0;   // DFGPU_STAGE_LEFT / DFGPU_STAGE_LEFT_ANTI when the last stage is one (it is then agg_stage), else 0
   // dense-group aggregate sink (group_cols, aggs and agg_mode as above; the aggregates' words address a slot of dense_acc)
   std::vector<DenseKey> dense_keys; std::vector<int> dense_radix; std::vector<unsigned long long> dense_ident;
   int dense_slots = 0, dense_words = 0; DevBuf dense_acc;
@@ -1901,7 +1911,9 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
   pp->first_hash = -1;
   for (size_t s = 0; s < p->stages.size(); ++s) if (p->stages[s].lookup->mode == LK_HASH && p->stages[s].kind != DFGPU_STAGE_MAYBE && pp->first_hash < 0) pp->first_hash = (int)s;
   for (size_t s = 0; s < p->stages.size(); ++s) {
-    pp->stage[s].kind = p->stages[s].kind; pp->stage[s].key_col = p->stages[s].key_col; pp->stage[s].lk = lookup_dev(p->stages[s].lookup);
+    // a LEFT / LEFT_ANTI stage probes as an INNER one: the build rows no probe row reached are found in the records at finish
+    const int kind = p->stages[s].kind;
+    pp->stage[s].kind = kind == DFGPU_STAGE_LEFT || kind == DFGPU_STAGE_LEFT_ANTI ? DFGPU_STAGE_INNER : kind; pp->stage[s].key_col = p->stages[s].key_col; pp->stage[s].lk = lookup_dev(p->stages[s].lookup);
   }
   pp->n_ext = (int)p->exts.size();
   for (size_t e = 0; e < p->exts.size(); ++e) pp->ext[e] = p->exts[e];
@@ -2126,7 +2138,7 @@ static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DensePar
 // the batch keeps the direct probe.  force_parts >= 2 (a test hook) admits tables of any size.
 static size_t partitioned_table_bytes(const dfgpu_pipeline* p, const PipeParams& pp, int force_parts) {
   if (pp.ring_stages == 0 || pipeline_has_decimal(p) || getenv("DFGPU_PIPE_VAR")) return 0;   // launch_pipe's ring kernel runs
-  if (pp.agg_stage < 0) return 0;
+  if (pp.agg_stage < 0 || p->left_kind) return 0;
   for (int s = 0; s < pp.n_stages; ++s)
     if (s != pp.agg_stage && pp.stage[s].lk.mode == LK_HASH && pp.stage[s].kind != kStageMaybe) return 0;
   const StageDev& st = pp.stage[pp.agg_stage];
@@ -2232,10 +2244,32 @@ static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t 
   }
 }
 
+// A LEFT / LEFT_ANTI join emits its build rows with a NULL key too, but the build sink never inserts them
+static void check_left_build(const dfgpu_pipeline* p) {
+  if (p->left_kind)
+    DF_CHECK(p->stages[p->agg_stage].lookup->null_keys == 0, DFGPU_ERR_UNSUPPORTED,
+             "pipeline: a LEFT / LEFT_ANTI stage needs a build side without NULL keys (they are not in the lookup) — use dfgpu_hashjoin");
+}
+
+// rows of a build push whose key is NULL, from the key column's validity (before the predicate: an upper bound of the rows dropped for it)
+static int64_t count_null_keys(dfgpu_ctx* ctx, const DCol& c) {
+  if (!c.validity || c.length == 0) return 0;
+  DevBuf mm(ctx, 24);
+  mm.zero();
+  col_minmax_kernel<<<grid_for(c.length, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(col_ref(c), c.length, type_is_unsigned_int(c.type) ? 1 : 0,
+                                                                                  mm.as<unsigned long long>());
+  DF_LAUNCH_CHECK(ctx);
+  unsigned long long h[3];
+  DF_CUDA(cudaMemcpyAsync(h, mm.ptr, 24, cudaMemcpyDeviceToHost, ctx->stream));
+  DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  return c.length - (int64_t)h[2];
+}
+
 static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   DF_CHECK(!p->finished, DFGPU_ERR_STATE, "push after finish");
   DF_CHECK(p->sink != SINK_NONE, DFGPU_ERR_STATE, "pipeline: choose a sink before the first push");
   DF_CHECK(cols.size() == p->in_types.size(), DFGPU_ERR_INVALID, "pipeline input column count mismatch");
+  check_left_build(p);
   dfgpu_ctx* ctx = p->ctx;
   set_device(ctx);
   const int64_t n = cols.empty() ? 0 : cols[0].length;
@@ -2252,6 +2286,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   unsigned long long h[4];
   if (p->sink == SINK_BUILD) {
     dfgpu_lookup* t = p->target;
+    t->null_keys += count_null_keys(ctx, cols[p->bkey_col]);
     if (t->mode == LK_HASH && !t->filter_only && (uint64_t)(t->rows + n) * 2 > t->cap) {
       // the batch may not fit at load factor 0.5 and nobody knows how many rows survive: ONE pass evaluates the pipeline and leaves
       // the survivors as packed {key, payload} records; the table is sized for exactly that many and the records are inserted by a
@@ -2452,24 +2487,28 @@ static void emit_sliced(dfgpu_pipeline* p, std::vector<DCol>& merged, int64_t ro
   }
 }
 
-// one column (Single) or the state columns (Partial) per aggregate, read from the accumulator words the aggregate addresses
+// one column (Single) or the state columns (Partial) per aggregate, read from the accumulator words the aggregate addresses.  `left`: the
+// records are a LEFT join's build rows, and one no probe row reached stands for its NULL-padded row: COUNT(*) 1, COUNT(x) 0 and every other
+// value NULL (the arguments propagate NULL).  Such a record's row counter is 0, so the counter serves as the non-null counter of a SUM /
+// MIN / MAX that has none; AVG's count is 0 anyway.
 template <class Add>
-static void add_agg_columns(const std::vector<PipeAgg>& aggs, int rows_word, bool partial, Add& add) {
+static void add_agg_columns(const std::vector<PipeAgg>& aggs, int rows_word, bool partial, bool left, Add& add) {
   for (const PipeAgg& ag : aggs) {
     EmitCol e; memset(&e, 0, sizeof(e));
     e.nn_word = -1;
     const int sum_type = ag.cls == C_F64 ? DFGPU_FLOAT64 : (ag.cls == C_U64 ? DFGPU_UINT64 : DFGPU_INT64);   // sum.rs:232-261
+    const int nn_word = left && ag.nn_word < 0 ? rows_word : ag.nn_word;
     switch (ag.func) {
-      case DFGPU_AGG_COUNT_STAR: e.kind = 4; e.word = rows_word; add(DFGPU_INT64, false, e); break;
+      case DFGPU_AGG_COUNT_STAR: e.kind = left ? 9 : 4; e.word = rows_word; add(DFGPU_INT64, false, e); break;
       case DFGPU_AGG_COUNT: e.kind = 4; e.word = ag.word; add(DFGPU_INT64, false, e); break;
       case DFGPU_AGG_SUM:
         if (ag.cls == C_DEC) {   // Sum::return_type: Decimal128(min(38, p + 10), s) (sum.rs:247-249); the Partial state has the same type
-          e.kind = 5; e.word = ag.word; e.nn_word = ag.nn_word;
-          add(dec_type(std::min(38, dec_precision(ag.arg_type) + 10), dec_scale(ag.arg_type)), ag.nn_word >= 0, e);
-        } else { e.kind = 2; e.word = ag.word; e.nn_word = ag.nn_word; add(sum_type, ag.nn_word >= 0, e); }
+          e.kind = 5; e.word = ag.word; e.nn_word = nn_word;
+          add(dec_type(std::min(38, dec_precision(ag.arg_type) + 10), dec_scale(ag.arg_type)), nn_word >= 0, e);
+        } else { e.kind = 2; e.word = ag.word; e.nn_word = nn_word; add(sum_type, nn_word >= 0, e); }
         break;
       case DFGPU_AGG_MIN: case DFGPU_AGG_MAX:   // the argument's type; Decimal128 takes two words
-        e.kind = ag.cls == C_DEC ? 5 : 2; e.word = ag.word; e.nn_word = ag.nn_word; add(ag.arg_type, ag.nn_word >= 0, e);
+        e.kind = ag.cls == C_DEC ? 5 : 2; e.word = ag.word; e.nn_word = nn_word; add(ag.arg_type, nn_word >= 0, e);
         break;
       case DFGPU_AGG_AVG:
         if (ag.cls == C_DEC) {   // Avg::return_type: Decimal128(min(38, p + 4), min(38, s + 4)) (average.rs); Single modes only
@@ -2506,6 +2545,7 @@ static void pipeline_finish(dfgpu_pipeline* p) {
   }
   if (p->sink == SINK_DENSE) { dense_finish(p); return; }
   if (p->sink != SINK_AGG && p->sink != SINK_HASH) return;
+  check_left_build(p);
   LookupDev t;
   if (p->sink == SINK_AGG) {
     dfgpu_lookup* l = p->stages[p->agg_stage].lookup;
@@ -2518,7 +2558,8 @@ static void pipeline_finish(dfgpu_pipeline* p) {
   }
   const uint64_t nw = (t.cap + 31) / 32;
   DevBuf words(ctx, (size_t)nw * 4 + 8), idx;
-  lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, p->rows_word, words.as<uint32_t>());
+  const int sel = p->left_kind == DFGPU_STAGE_LEFT ? 2 : (p->left_kind == DFGPU_STAGE_LEFT_ANTI ? 1 : 0);
+  lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, p->rows_word, sel, words.as<uint32_t>());
   DF_LAUNCH_CHECK(ctx);
   const int64_t groups = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)t.cap, 1, &idx);
   p->m_groups = groups;
@@ -2554,7 +2595,7 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     if (g == key_col) { e.kind = 0; add(p->in_types[g], false, e); }
     else { const ExtDef& x = p->exts[g - (int)p->in_types.size()]; e.kind = 1; e.shift = x.shift; add(x.type, false, e); }
   }
-  add_agg_columns(p->aggs, p->rows_word, partial, add);
+  add_agg_columns(p->aggs, p->rows_word, partial, p->left_kind == DFGPU_STAGE_LEFT, add);
   lookup_emit_kernel<<<grid_for(groups, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), groups, p->rows_word, ec);
   DF_LAUNCH_CHECK(ctx);
   if (dec_avg) {
@@ -2583,7 +2624,7 @@ static void dense_finish(dfgpu_pipeline* p) {
   } else {
     const uint64_t nw = (t.cap + 31) / 32;
     DevBuf words(ctx, (size_t)nw * 4 + 8);
-    lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, 0, words.as<uint32_t>());
+    lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, 0, 0, words.as<uint32_t>());
     DF_LAUNCH_CHECK(ctx);
     groups = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)t.cap, 1, &idx);
   }
@@ -2606,7 +2647,7 @@ static void dense_finish(dfgpu_pipeline* p) {
     e.kind = 6; e.kmin = (long long)p->dense_keys[k].kmin; e.kstride = (int)p->dense_keys[k].stride; e.kradix = p->dense_radix[k];
     add(p->vtypes[p->group_cols[k]], true, e);
   }
-  add_agg_columns(p->aggs, 0, p->agg_mode == DFGPU_AGG_PARTIAL, add);
+  add_agg_columns(p->aggs, 0, p->agg_mode == DFGPU_AGG_PARTIAL, false, add);
   lookup_emit_kernel<<<grid_for(groups, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), groups, 0, ec);
   DF_LAUNCH_CHECK(ctx);
   unsigned long long h_err = 0;
@@ -2677,6 +2718,39 @@ static void layout_agg_words(std::vector<PipeAgg>& aggs, int& next, int budget, 
   }
 }
 
+static bool is_left_kind(int kind) { return kind == DFGPU_STAGE_LEFT || kind == DFGPU_STAGE_LEFT_ANTI; }
+
+// a LEFT / LEFT_ANTI stage emits its build rows from the join-keyed aggregate sink's records; every other sink is UNSUPPORTED
+static void check_no_left_stage(const dfgpu_pipeline* p) {
+  for (const auto& st : p->stages)
+    DF_CHECK(!is_left_kind(st.kind), DFGPU_ERR_UNSUPPORTED, "pipeline: a LEFT / LEFT_ANTI stage runs only with the join-keyed aggregate sink grouped on it");
+}
+
+// LEFT: a build row no probe row reached is emitted as one NULL-padded row without evaluating anything, so an aggregate argument must be
+// NULL on that row: it reads at least one probe-side input column, no payload field of the LEFT stage (that is the padded row's own
+// value), and every node propagates NULL (no IS [NOT] NULL, IS [NOT] DISTINCT FROM, AND, OR)
+static void check_left_args(const dfgpu_pipeline* p, const std::vector<PipeAgg>& aggs, int stage) {
+  const int nin = (int)p->in_types.size();
+  for (const PipeAgg& ag : aggs) {
+    if (!ag.has_expr) continue;
+    bool probe_col = false;
+    for (const auto& nd : ag.plan.nodes) {
+      bool ok = true;
+      if (nd.kind == DFGPU_EXPR_COLUMN) {
+        if (nd.a < nin) probe_col = true;
+        else ok = p->exts[nd.a - nin].stage != stage;
+      } else if (nd.kind == DFGPU_EXPR_BINARY) {
+        ok = nd.a != DFGPU_OP_AND && nd.a != DFGPU_OP_OR && nd.a != DFGPU_OP_IS_DISTINCT_FROM && nd.a != DFGPU_OP_IS_NOT_DISTINCT_FROM;
+      } else {
+        ok = nd.kind == DFGPU_EXPR_LITERAL || nd.kind == DFGPU_EXPR_CAST || nd.kind == DFGPU_EXPR_NEGATIVE || nd.kind == DFGPU_EXPR_NOT;
+      }
+      DF_CHECK(ok, DFGPU_ERR_UNSUPPORTED,
+               "pipeline aggregate: under a LEFT stage an argument must propagate NULL and read no build-side column — use dfgpu_hashjoin + dfgpu_agg");
+    }
+    DF_CHECK(probe_col, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: under a LEFT stage every argument reads a probe-side input column");
+  }
+}
+
 }  // namespace dfgpu
 
 extern "C" {
@@ -2743,6 +2817,7 @@ int64_t dfgpu_lookup_metric(dfgpu_lookup* l, const char* name) {
   if (s == "filter_bytes") return (int64_t)l->bloom.bytes;
   if (s == "rehashes") return l->rehashes;
   if (s == "stride_bytes") return l->stride * 8;
+  if (s == "null_keys") return l->null_keys;
   return -1;
 }
 int dfgpu_lookup_clear(dfgpu_lookup* l) {
@@ -2756,7 +2831,7 @@ int dfgpu_lookup_clear(dfgpu_lookup* l) {
     if (l->cap) { lookup_init_kernel<<<grid_for((int64_t)l->cap * l->stride, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(l->recs.as<unsigned long long>(), l->cap, l->stride); DF_LAUNCH_CHECK(ctx); }
     if (l->bloom.ptr) l->bloom.zero();
   }
-  l->rows = 0;
+  l->rows = 0; l->null_keys = 0;
   DF_API_END
 }
 int dfgpu_lookup_filter_buffer(dfgpu_lookup* l, void** words_dev, uint64_t* n_bytes) {
@@ -2851,7 +2926,7 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
   for (int s = 0; s < n_stages; ++s) {
     const dfgpu_pipeline_stage& st = stages[s];
     DF_CHECK(st.lookup, DFGPU_ERR_INVALID, "pipeline: stage without a lookup");
-    DF_CHECK(st.kind >= DFGPU_STAGE_INNER && st.kind <= DFGPU_STAGE_MAYBE, DFGPU_ERR_INVALID, "pipeline: unknown stage kind");
+    DF_CHECK(st.kind >= DFGPU_STAGE_INNER && st.kind <= DFGPU_STAGE_LEFT_ANTI, DFGPU_ERR_INVALID, "pipeline: unknown stage kind");
     DF_CHECK(!st.lookup->filter_only || st.kind == DFGPU_STAGE_MAYBE, DFGPU_ERR_INVALID, "pipeline: a filter-only lookup can only back a MAYBE stage");
     DF_CHECK(st.key_col >= 0 && st.key_col < n_cols, DFGPU_ERR_INVALID, "pipeline: stage key column out of range");
     const int kt = input_types[st.key_col], lt = st.lookup->key_type;
@@ -2859,7 +2934,7 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
              "pipeline: probe key type differs from the lookup's key type");
     DF_CHECK(st.lookup->ctx->device == ctx->device, DFGPU_ERR_INVALID, "pipeline: lookup lives on another device");
     p->stages.push_back(st);
-    if (st.kind == DFGPU_STAGE_INNER)
+    if (st.kind == DFGPU_STAGE_INNER || st.kind == DFGPU_STAGE_LEFT || st.kind == DFGPU_STAGE_LEFT_ANTI)
       for (size_t f = 0; f < st.lookup->pay_types.size(); ++f) {
         DF_CHECK(p->exts.size() < (size_t)kMaxExt, DFGPU_ERR_UNSUPPORTED, "pipeline: at most 8 payload fields");
         ExtDef e; e.stage = s; e.shift = st.lookup->pay_shift[f]; e.width = type_width(st.lookup->pay_types[f]); e.type = st.lookup->pay_types[f];
@@ -2875,6 +2950,7 @@ int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t k
   DF_API_BEGIN(p ? p->ctx : nullptr)
   DF_CHECK(p && target, DFGPU_ERR_INVALID, "null argument");
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  check_no_left_stage(p);
   DF_CHECK(key_col >= 0 && key_col < (int)p->in_types.size(), DFGPU_ERR_INVALID, "pipeline build sink: the key must be an input column");
   const int kt = p->in_types[key_col];
   DF_CHECK(type_width(kt) == type_width(target->key_type) && type_is_signed_int(kt) == type_is_signed_int(target->key_type), DFGPU_ERR_INVALID,
@@ -2896,11 +2972,19 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
   DF_CHECK(n_aggs >= 0 && n_aggs <= kMaxPipeAggs && (n_aggs == 0 || aggs), DFGPU_ERR_UNSUPPORTED, "pipeline: 0..4 aggregates");
   DF_CHECK(mode == DFGPU_AGG_SINGLE || mode == DFGPU_AGG_SINGLE_PARTITIONED || mode == DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Single / SinglePartitioned / Partial");
+  // a LEFT / LEFT_ANTI stage must be the last one, and the records grouped on are its own
+  const int n_stages = (int)p->stages.size();
+  int left = -1;
+  for (int s = 0; s < n_stages; ++s) {
+    if (!is_left_kind(p->stages[s].kind)) continue;
+    DF_CHECK(s == n_stages - 1, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: a LEFT / LEFT_ANTI stage must be the last stage");
+    left = s;
+  }
   // functional dependence: every group column is the probe key of ONE inner stage or a payload field of that stage
   const int nin = (int)p->in_types.size();
   int stage = -1;
-  for (size_t s = 0; s < p->stages.size() && stage < 0; ++s) {
-    if (p->stages[s].kind != DFGPU_STAGE_INNER) continue;
+  for (int s = 0; s < n_stages && stage < 0; ++s) {
+    if (left >= 0 ? s != left : p->stages[s].kind != DFGPU_STAGE_INNER) continue;
     bool has_key = false, ok = true;
     for (int g = 0; g < n_group; ++g) {
       const int c = group_cols[g];
@@ -2919,11 +3003,15 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   DF_CHECK(next < base + l->opt.n_acc_words, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: the lookup reserves no accumulator words (n_acc_words)");
   const int rows_word = next++;
   std::vector<PipeAgg> new_aggs = parse_pipe_aggs(p, aggs, n_aggs, mode);   // committed only when every check has passed
+  const int left_kind = left >= 0 ? p->stages[left].kind : 0;
+  DF_CHECK(left_kind != DFGPU_STAGE_LEFT_ANTI || n_aggs == 0, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: a LEFT_ANTI stage emits its build rows without aggregates");
+  if (left_kind == DFGPU_STAGE_LEFT) check_left_args(p, new_aggs, left);
   layout_agg_words(new_aggs, next, base + l->opt.n_acc_words, l->stride % 2 == 0);
   p->rows_word = rows_word;
   p->group_cols.assign(group_cols, group_cols + n_group);
   p->aggs = std::move(new_aggs);
   l->acc_claimed = true;
+  p->left_kind = left_kind;
   p->agg_stage = stage; p->agg_mode = mode; p->batch_size = batch_size; p->sink = SINK_AGG;
   DF_API_END
 }
@@ -2933,6 +3021,7 @@ int dfgpu_pipeline_sink_aggregate_hash(dfgpu_pipeline* p, const int32_t* group_c
   DF_API_BEGIN(p ? p->ctx : nullptr)
   DF_CHECK(p && group_cols && n_group >= 1, DFGPU_ERR_INVALID, "null argument");
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  check_no_left_stage(p);
   DF_CHECK(n_group <= kHashMaxKeys, DFGPU_ERR_UNSUPPORTED, "pipeline hash aggregate: 1..8 group columns");
   DF_CHECK(mode == DFGPU_AGG_SINGLE || mode == DFGPU_AGG_SINGLE_PARTITIONED || mode == DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Single / SinglePartitioned / Partial");
   DF_CHECK(capacity_hint >= 0, DFGPU_ERR_INVALID, "pipeline hash aggregate: negative capacity_hint");
@@ -2978,6 +3067,7 @@ int dfgpu_pipeline_sink_aggregate_dense(dfgpu_pipeline* p, const int32_t* group_
   DF_API_BEGIN(p ? p->ctx : nullptr)
   DF_CHECK(p && n_group >= 0 && (n_group == 0 || (group_cols && key_min && key_max)), DFGPU_ERR_INVALID, "null argument");
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  check_no_left_stage(p);
   DF_CHECK(n_group <= kDenseMaxKeys, DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: 0..8 group columns");
   DF_CHECK(n_aggs >= 0 && n_aggs <= kDenseMaxAggs && (n_aggs == 0 || aggs), DFGPU_ERR_UNSUPPORTED, "pipeline dense aggregate: 0..8 aggregates");
   DF_CHECK(mode == DFGPU_AGG_SINGLE || mode == DFGPU_AGG_SINGLE_PARTITIONED || mode == DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Single / SinglePartitioned / Partial");
@@ -3061,6 +3151,7 @@ int dfgpu_pipeline_sink_output(dfgpu_pipeline* p, const int32_t* out_cols, int32
   DF_API_BEGIN(p ? p->ctx : nullptr)
   DF_CHECK(p && out_cols && n_out >= 1 && n_out <= kMaxPipeCols, DFGPU_ERR_INVALID, "pipeline output: 1..16 columns");
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  check_no_left_stage(p);
   for (int c = 0; c < n_out; ++c) {
     DF_CHECK(out_cols[c] >= 0 && out_cols[c] < (int)p->vtypes.size(), DFGPU_ERR_INVALID, "pipeline output: column out of range");
     DF_CHECK(type_width(p->vtypes[out_cols[c]]) <= 8, DFGPU_ERR_UNSUPPORTED, "pipeline output: 16-byte columns leave through dfgpu_filter / dfgpu_hashjoin");

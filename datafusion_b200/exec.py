@@ -251,12 +251,14 @@ def _rename(rb: pa.RecordBatch, schema: pa.Schema) -> pa.RecordBatch:
     return pa.RecordBatch.from_arrays(cols, schema=schema)
 
 
-def _drain(op, schema) -> Iterator[pa.RecordBatch]:
+def _drain(op, schema, project: Optional[Sequence[int]] = None) -> Iterator[pa.RecordBatch]:
+    """the operator's output batches as `schema`; `project`: the columns of each batch that form it (None = all, in order)"""
     while True:
         b = op.next(host=True)
         if b is None:
             return
-        yield _rename(b.to_arrow(), schema)
+        rb = b.to_arrow()
+        yield _rename(rb if project is None else rb.select(list(project)), schema)
 
 
 # ---------------------------------------------------------------------------------------------
@@ -627,7 +629,7 @@ class _Scan:
     def virtual_schema(self) -> pa.Schema:
         fields = list(self.source.schema)
         for kind, _, build in self.stages:
-            if kind == D.STAGE_INNER:
+            if kind in (D.STAGE_INNER, D.STAGE_LEFT, D.STAGE_LEFT_ANTI):
                 fields += [build.scan_field(n) for n in build.payload]
         return pa.schema(fields)
 
@@ -689,10 +691,11 @@ class GpuPipelineExec(ExecutionPlan):
 
     def __init__(self, scan: _Scan, sink: str, key: Optional[str] = None, payload: Sequence[str] = (), group_by: Sequence[str] = (),
                  aggs: Sequence[Tuple[str, Optional[Expr], str]] = (), mode: str = "Single", out_schema: Optional[pa.Schema] = None,
-                 key_range: Sequence[Tuple[int, int]] = (), nullable: Sequence[bool] = ()):
+                 key_range: Sequence[Tuple[int, int]] = (), nullable: Sequence[bool] = (), project: Optional[Sequence[int]] = None):
         self.scan, self.sink, self.key, self.payload, self.group_by, self.aggs, self.mode = scan, sink, key, list(payload), list(group_by), list(aggs), mode
         self.key_range = list(key_range)   # dense sink: the declared (min, max) of every group column
         self.nullable = list(nullable)     # hash sink: the declared nullability of every group column
+        self.project = None if project is None else list(project)   # the emitted columns that form the output (a LeftSemi / LeftAnti join's projection)
         self.schema = out_schema if out_schema is not None else pa.schema([])
         self.n_acc_words = 0
         self._metrics = {}
@@ -764,7 +767,7 @@ class GpuPipelineExec(ExecutionPlan):
                 pipe.push_arrow(rb)
             pipe.finish()
             bs = ctx.config.batch_size
-            for rb in _drain(pipe, self.schema):
+            for rb in _drain(pipe, self.schema, self.project):
                 for s in range(0, rb.num_rows, bs):
                     yield rb.slice(s, bs)
             self._metrics = {k: pipe.metric(k) for k in ("input_rows", "sink_rows", "num_groups")}
@@ -873,7 +876,13 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     HashJoinExec(Inner) whose GROUP BY is the probe key plus build-side columns becomes ONE GpuPipelineExec; its build side (filters, semi
     joins, column projections) becomes build pipelines.  The same AggregateExec over [ProjectionExec] over FilterExec over a source, with
     no join, becomes a GpuPipelineExec with the dense sink when its GROUP BY columns have small known bounds (_fuse_dense: TPC-H Q1, Q6).
-    Anything else is returned unchanged (the unfused Gpu*Exec operators run)."""
+    Left joins (the build side kept): the same AggregateExec over HashJoinExec(Left) grouped on the build key plus build columns
+    (_fuse_left: TPC-H Q13), and a top-level HashJoinExec(LeftSemi / LeftAnti) (_fuse_left_filter: Q18, Q20, Q22) become a GpuPipelineExec
+    with the join-keyed sink.  Their rows come out in slot order: the reference does not keep the build side's order either
+    (maintains_input_order is false for it).  Anything else is returned unchanged (the unfused Gpu*Exec operators run)."""
+    if isinstance(plan, GpuHashJoinExec) and plan.join_type in ("LeftSemi", "LeftAnti"):
+        fused = _fuse_left_filter(plan)
+        return plan if fused is None else fused
     if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial"):
         return plan
     dense = _fuse_dense(plan)
@@ -884,6 +893,9 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     below, proj = plan.input, None
     if isinstance(below, GpuProjectionExec):
         proj, below = below, below.input
+    if isinstance(below, GpuHashJoinExec) and below.join_type == "Left":
+        fused = _fuse_left(plan, below, proj)
+        return plan if fused is None else fused
     if not isinstance(below, GpuHashJoinExec) or below.join_type != "Inner":
         return plan
     sc = _as_scan(below)
@@ -927,6 +939,96 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
         return plan
     build.n_acc_words = n_acc
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
+
+
+def _left_join_scan(join: GpuHashJoinExec, kind: int) -> Optional[_Scan]:
+    """The probe chain of a Left / LeftSemi / LeftAnti join with the join as its last stage (kind), or None.  Conditions: one key, no
+    JoinFilter, NullEqualsNothing, not null-aware; the right side is an _as_scan chain probing on one of its source columns; the left side
+    is a fusable build whose key field is declared non-nullable (a NULL build key is never in the lookup, but Left / LeftAnti emit its row)
+    and has the probe key's type.  The build's payload is every other left column."""
+    if len(join.on) != 1 or join.filter is not None or join.null_aware or join.null_equality != "NullEqualsNothing":
+        return None
+    bkey, pkey = join.on[0]
+    sc = _as_scan(join.right)
+    ls = join.left.schema
+    if sc is None or len(sc.stages) >= 3 or sc.source.schema.get_field_index(pkey) < 0 or ls.get_field_index(bkey) < 0:
+        return None
+    kf = ls.field(bkey)
+    if kf.nullable or kf.type != sc.source.schema.field(pkey).type:
+        return None
+    build = _as_build(join.left, bkey, [f.name for f in ls if f.name != bkey])
+    if build is None:
+        return None
+    sc.stages.append((kind, pkey, build))
+    return sc
+
+
+def _fuse_left(plan: "GpuAggregateExec", join: GpuHashJoinExec, proj: Optional[GpuProjectionExec]) -> Optional["GpuPipelineExec"]:
+    """AggregateExec over [ProjectionExec] over HashJoinExec(Left) -> the join-keyed sink over a LEFT stage, or None.  GROUP BY the build
+    key (not the probe key: NULL on a padded row) plus build columns; every aggregate COUNT(*) or an argument over right-side columns that
+    reads a probe source column and propagates NULL, so that it is NULL on a build row's padded row."""
+    sc = _left_join_scan(join, D.STAGE_LEFT)
+    if sc is None:
+        return None
+    _, pkey, build = sc.stages[-1]
+    vs = sc.virtual_schema()
+    exprs = {name: e for e, name in proj.exprs} if proj is not None else {f.name: Column(f.name) for f in join.schema}
+    group = []
+    for g in plan.group_by:
+        e = exprs.get(g)
+        if not isinstance(e, Column) or (e.name != build.key and e.name not in build.payload):
+            return None
+        group.append(pkey if e.name == build.key else e.name)
+    if pkey not in group:
+        return None
+    n_src, left_payload = len(sc.source.schema), range(len(vs) - len(build.payload), len(vs))
+    aggs, types = [], []
+    for a in plan.aggr_expr:
+        if a.filter is not None:
+            return None
+        if a.arg is None:
+            aggs.append(("count_star", None, a.alias)); types.append(None)
+            continue
+        e = exprs.get(a.arg)
+        if e is None:
+            return None
+        nodes: list = []
+        try:
+            e.rpn(vs, nodes)                               # the build key is not in the virtual schema
+            t = e.data_type(vs)
+        except KeyError:
+            return None
+        if not any(n[0] == D.EXPR_COLUMN and n[1] < n_src for n in nodes):
+            return None
+        for n in nodes:
+            if (n[0] == D.EXPR_COLUMN and n[1] in left_payload) or n[0] in (D.EXPR_IS_NULL, D.EXPR_IS_NOT_NULL) or \
+                    (n[0] == D.EXPR_BINARY and n[1] in (D.OP_AND, D.OP_OR, D.OP_IS_DISTINCT_FROM, D.OP_IS_NOT_DISTINCT_FROM)):
+                return None
+        if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
+            return None                                    # AVG(Decimal128) has no pinned Partial state
+        if a.func in ("min", "max") and t == pa.float32():
+            return None
+        aggs.append((a.func, e, a.alias)); types.append(t)
+    n_acc = _acc_words([f for f, _, _ in aggs], types, bool(build.payload))
+    if n_acc > 12:
+        return None
+    build.n_acc_words = n_acc
+    return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
+
+
+def _fuse_left_filter(join: GpuHashJoinExec) -> Optional["GpuPipelineExec"]:
+    """HashJoinExec(LeftSemi / LeftAnti) -> the join-keyed sink without aggregates, grouped on every left column, or None.  LeftSemi is an
+    INNER stage over the unique build keys (the records a probe row reached), LeftAnti a LEFT_ANTI stage (the records none reached)."""
+    sc = _left_join_scan(join, D.STAGE_INNER if join.join_type == "LeftSemi" else D.STAGE_LEFT_ANTI)
+    if sc is None:
+        return None
+    _, pkey, build = sc.stages[-1]
+    group = [pkey if f.name == build.key else f.name for f in join.left.schema]
+    build.n_acc_words = _acc_words([], [], bool(build.payload))
+    project = [i for _, i in join.column_indices]          # the join's projection: left columns only
+    if project == list(range(len(group))):
+        project = None
+    return GpuPipelineExec(sc, sink="aggregate", group_by=group, mode="Single", out_schema=join.schema, project=project)
 
 
 def fuse_hash_aggregates(plan: ExecutionPlan) -> ExecutionPlan:

@@ -403,8 +403,8 @@ void dfgpu_agg_destroy(dfgpu_agg* a);
  *                 optional accumulator words per record for an aggregation whose group keys are functionally
  *                 determined by the join key (group id == build row).
  * dfgpu_pipeline= source batch -> predicate -> probe stage(s) -> sink.
- * "virtual columns" of a pipeline: the input columns [0, n_cols) followed by the payload fields of every INNER
- * stage in stage order; expressions, group columns, build payloads and outputs address this space. */
+ * "virtual columns" of a pipeline: the input columns [0, n_cols) followed by the payload fields of every INNER, LEFT and
+ * LEFT_ANTI stage in stage order; expressions, group columns, build payloads and outputs address this space. */
 /* ===================================================================================== */
 typedef struct dfgpu_lookup dfgpu_lookup;
 typedef struct dfgpu_pipeline dfgpu_pipeline;
@@ -436,7 +436,9 @@ int dfgpu_lookup_filter_buffer(dfgpu_lookup* l, void** words_dev, uint64_t* n_by
  * kernel, no NCCL payload (NCCL has no bitwise OR).  The caller places a barrier before (all filters built) and after (all slices
  * merged) the call.  Reference analogue: SharedBuildAccumulator merging per-partition bounds / membership (shared_bounds.rs). */
 int dfgpu_lookup_filter_allreduce_peer(dfgpu_lookup* l, void* const* peer_words, int32_t rank, int32_t n_ranks);
-int64_t dfgpu_lookup_metric(dfgpu_lookup* l, const char* name); /* "rows","capacity","mode"(0 hash,1 bitmap),"table_bytes","filter_bytes","rehashes" */
+int64_t dfgpu_lookup_metric(dfgpu_lookup* l, const char* name); /* "rows","capacity","mode"(0 hash,1 bitmap),"table_bytes","filter_bytes","rehashes",
+                                                                  "null_keys": rows pushed into the build sink with a NULL key (never
+                                                                  inserted), counted from the key column before the predicate */
 void dfgpu_lookup_destroy(dfgpu_lookup* l);
 /* min / max / non-null count of one integer column (device resident): feeds dfgpu_lookup_options.key_min/key_max */
 int dfgpu_column_minmax_device(dfgpu_ctx* ctx, const dfgpu_column* col, int64_t* min_out, int64_t* max_out, int64_t* valid_out);
@@ -447,11 +449,16 @@ int dfgpu_column_sum_device(dfgpu_ctx* ctx, const dfgpu_column* col, uint64_t* s
 
 enum dfgpu_stage_kind {
   DFGPU_STAGE_INNER = 0, DFGPU_STAGE_SEMI = 1, DFGPU_STAGE_ANTI = 2,
-  DFGPU_STAGE_MAYBE = 3   /* membership pre-filter only (may have false positives, never false negatives): the dynamic filter a downstream
+  DFGPU_STAGE_MAYBE = 3,  /* membership pre-filter only (may have false positives, never false negatives): the dynamic filter a downstream
                            * join pushes into this scan (joins/hash_join/shared_bounds.rs); the exact join runs after the exchange */
+  DFGPU_STAGE_LEFT = 4,   /* Left join (every build row, NULL-padded when no probe row matches) and LeftAnti join (the build rows no     */
+  DFGPU_STAGE_LEFT_ANTI = 5 /* probe row matches): the last stage only, with dfgpu_pipeline_sink_aggregate grouped on it (see there); the
+                           * probe runs as for INNER (unmatched probe rows are dropped, the payload fields are virtual columns) */
 };
 typedef struct dfgpu_pipeline_stage {
-  int32_t kind;          /* dfgpu_stage_kind: the pipeline input is the PROBE (right) side — Inner / RightSemi / RightAnti */
+  int32_t kind;          /* dfgpu_stage_kind: the pipeline input is the PROBE (right) side — Inner / RightSemi / RightAnti, and Left /
+                          * LeftAnti (LEFT / LEFT_ANTI) through the join-keyed aggregate sink.  LeftSemi is an INNER stage + the join-keyed
+                          * aggregate sink with no aggregates, grouped on the key and payload of a lookup with unique keys */
   int32_t key_col;       /* input column holding the probe key (NULL keys never match, utils.rs:2146-2155) */
   dfgpu_lookup* lookup;  /* must be completely built before the first push */
 } dfgpu_pipeline_stage;
@@ -468,8 +475,8 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
 /* exactly one sink, chosen before the first push:
  *  build     : surviving rows become records of `target` (key = virtual column key_col, payload = payload_cols in
  *              the order of the lookup's payload_types) — the pipeline IS the build side of the next join;
- *  aggregate : AggregateExec over the surviving rows; group_cols must be the probe key of one INNER stage plus payload
- *              fields of that stage (group id == build row; anything else -> DFGPU_ERR_UNSUPPORTED, use dfgpu_agg);
+ *  aggregate : AggregateExec over the surviving rows; group_cols must be the probe key of one INNER (or LEFT / LEFT_ANTI)
+ *              stage plus payload fields of that stage (group id == build row; anything else -> DFGPU_ERR_UNSUPPORTED, use dfgpu_agg);
  *              mode = DFGPU_AGG_SINGLE* or DFGPU_AGG_PARTIAL (state columns as dfgpu_agg emits them);
  *              the accumulators are words of the lookup's records (n_acc_words): 1 row counter, then per aggregate
  *                COUNT(x), and SUM / MIN / MAX over a 64-bit type: 1;  AVG over Float64: 2;
@@ -480,7 +487,18 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
  *              modes only (DFGPU_ERR_ARITH at finish when a group's value overflows, as in the dense sink).  A Decimal128 MIN /
  *              MAX needs a record of an even number of words: with payload it always is; a lookup without payload needs an odd
  *              n_acc_words (else DFGPU_ERR_UNSUPPORTED).  The pairs take even words after the row counter, behind at most one
- *              padding word, which may serve as a non-null counter; without pairs the words are taken in aggregate order;
+ *              padding word, which may serve as a non-null counter; without pairs the words are taken in aggregate order.
+ *              A LEFT / LEFT_ANTI stage must be the last stage and the one grouped on (else DFGPU_ERR_UNSUPPORTED); its key column
+ *              then means the BUILD key, emitted from the record (never NULL).  Output in slot order (unspecified) either way:
+ *                LEFT: one row per build row; a row no probe row reached is the NULL-padded row: COUNT(*) 1, COUNT(x) 0, SUM / MIN /
+ *                  MAX / AVG NULL (and their Partial states: AVG [count 0, sum NULL]), so these columns are nullable.  Every
+ *                  argument reads at least one input (probe) column and no payload field of the LEFT stage, and each of its nodes
+ *                  propagates NULL (column, literal, arithmetic, comparison, CAST, NOT, negation: no IS [NOT] NULL, IS [NOT]
+ *                  DISTINCT FROM, AND, OR), else DFGPU_ERR_UNSUPPORTED;
+ *                LEFT_ANTI: no aggregates; one row per build row no probe row reached;
+ *                and for both, a lookup whose build pushes held a NULL key ("null_keys" > 0) is DFGPU_ERR_UNSUPPORTED at the first
+ *                push (those rows are not in the lookup, but the join emits them);
+ *              every other sink over a LEFT / LEFT_ANTI stage is DFGPU_ERR_UNSUPPORTED;
  *  output    : surviving rows, columns = out_cols of the virtual schema, input order preserved. */
 int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload);
 int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, int32_t n_group,
