@@ -99,6 +99,9 @@ __device__ __forceinline__ uint64_t ld_stream_int(const void* base, int width, i
     default: { uint64_t v; asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"((const uint64_t*)base + row), "l"(pol)); return v; }
   }
 }
+__device__ __forceinline__ void st_stream_u64(unsigned long long* p, unsigned long long v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.u64 [%0], %1, %2;" :: "l"(p), "l"(v), "l"(pol) : "memory");
+}
 __device__ __forceinline__ unsigned long long ld_keep_u64(const unsigned long long* p, uint64_t pol) {
   unsigned long long v; asm volatile("ld.global.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(v) : "l"(p), "l"(pol)); return v;
 }
@@ -827,6 +830,10 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
         for (int u = 0; u < PB; ++u) g[k][u] = 0;
         if (RING && SINK == SINK_AGG && k < sp.n_gather) {
           const ENode& nd = sp.pool[sp.gather_node[k]];
+          if (PART) {   // read once, evict first: the lines around the survivors must not push the Bloom filter out of L2
+#pragma unroll
+            for (int u = 0; u < PB; ++u) if (live[u]) g[k][u] = ld_stream_int(nd.col, type_width_prim(nd.out_type), type_is_signed_int(nd.out_type) ? 1 : 0, row[u], pol_stream);
+          } else
 #pragma unroll
           for (int u = 0; u < PB; ++u) if (live[u]) g[k][u] = load_col_value(nd, row[u]);
         }
@@ -925,8 +932,8 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
           const unsigned long long v = eval_int_gathered(sp.pool + ag0.start, ag0.n, row[u], ext, sp.n_gather, g[0][u], g[1][u]);
           const unsigned long long o = obase + mypos[u];
           if (o < sp.target.cap) {
-            ((unsigned long long*)sp.out_dst[0])[o] = pkey[u];
-            ((unsigned long long*)sp.out_dst[1])[o] = v;
+            st_stream_u64((unsigned long long*)sp.out_dst[0] + o, pkey[u], pol_stream);   // the records, too, are read again only after this pass
+            st_stream_u64((unsigned long long*)sp.out_dst[1] + o, v, pol_stream);
             continue;
           }
           const LookupDev& lk = sp.stage[sp.agg_stage].lk;
