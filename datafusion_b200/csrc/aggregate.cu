@@ -176,19 +176,6 @@ __device__ __forceinline__ double load_as_f64(const void* p, int type, int64_t i
     default: return (double)load_as_i64(p, type, i);
   }
 }
-// order-preserving map double -> uint64 (IEEE total order: -NaN < -inf < ... < +inf < +NaN)
-__host__ __device__ __forceinline__ uint64_t f64_to_ordered(double d) {
-  uint64_t b;
-  memcpy(&b, &d, 8);
-  return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
-}
-__host__ __device__ __forceinline__ double ordered_to_f64(uint64_t u) {
-  uint64_t b = (u & 0x8000000000000000ull) ? (u & 0x7FFFFFFFFFFFFFFFull) : ~u;
-  double d;
-  memcpy(&d, &b, 8);
-  return d;
-}
-
 // i128 add_wrapping as two 64-bit atomics: the carry out of the low word is a function of this add alone (old + lo overflowed), so the
 // high words sum to the right value in any interleaving
 __device__ __forceinline__ void add_i128(unsigned long long* lo_word, unsigned long long* hi_word, unsigned long long lo, unsigned long long hi) {

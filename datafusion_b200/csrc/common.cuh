@@ -82,6 +82,21 @@ __host__ __device__ inline bool type_is_unsigned_int(int t) {
 __host__ __device__ inline bool type_is_float(int t) { return t == DFGPU_FLOAT32 || t == DFGPU_FLOAT64; }
 __host__ __device__ inline bool type_is_int(int t) { return type_is_signed_int(t) || type_is_unsigned_int(t); }
 
+// the order-preserving map double -> uint64 of float MIN / MAX (IEEE totalOrder on the bits: -NaN < -inf < ... < -0.0 < +0.0 < ... <
+// +inf < +NaN).  dfgpu_agg and the pipeline sinks reduce this key with unsigned min / max and map it back when they emit, so the result
+// is one of the inputs bit for bit whatever the row order
+__host__ __device__ __forceinline__ uint64_t f64_to_ordered(double d) {
+  uint64_t b;
+  memcpy(&b, &d, 8);
+  return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
+}
+__host__ __device__ __forceinline__ double ordered_to_f64(uint64_t u) {
+  uint64_t b = (u & 0x8000000000000000ull) ? (u & 0x7FFFFFFFFFFFFFFFull) : ~u;
+  double d;
+  memcpy(&d, &b, 8);
+  return d;
+}
+
 inline size_t values_bytes(int type, int64_t rows) {
   if (type == DFGPU_BOOL) return (size_t)((rows + 7) / 8);
   return (size_t)rows * (size_t)type_width(type);

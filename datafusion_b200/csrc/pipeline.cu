@@ -160,18 +160,6 @@ __device__ __forceinline__ uint64_t ext_field(uint64_t word, int shift, int widt
   return v;
 }
 
-__device__ __forceinline__ void red_f64_min(unsigned long long* p, double v, bool is_max) {
-  unsigned long long old = *(volatile unsigned long long*)p;
-  while (true) {
-    const double cur = __longlong_as_double((long long)old);
-    // f64 MIN/MAX follow the reference's total order on non-NaN data; NaN handling stays with the generic operator
-    if (is_max ? !(v > cur) : !(v < cur)) return;
-    const unsigned long long prev = atomicCAS(p, old, (unsigned long long)__double_as_longlong(v));
-    if (prev == old) return;
-    old = prev;
-  }
-}
-
 // ------------------------------------------------------------------------------------------
 // the pipeline kernel.  Every WARP runs the pipeline on its own 256-row tiles, in two phases, with no block barrier:
 //   phase A (every row, cheap, coalesced): a lane owns 8 consecutive rows and reads them with 128-bit loads (a warp request
@@ -428,9 +416,10 @@ __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefe
 constexpr int kDenseMaxSlots = 256, kDenseMaxKeys = 8, kDenseMaxAggs = 8, kDenseMaxWords = 40, kDenseMaxXTerms = 4;
 constexpr int kDenseWarpBytes = 48 * 1024;   // per-warp accumulator copies when all eight fit in this many bytes
 // how one aggregate's value combines: none (COUNT: only the non-null counter), add, min, max over u64 / i64 / f64 / i128 words
-enum DenseOp : int { DO_NONE = 0, DO_ADD_U64, DO_ADD_F64, DO_ADD_128, DO_MIN_S64, DO_MAX_S64, DO_MIN_U64, DO_MAX_U64, DO_MIN_F64, DO_MAX_F64, DO_MIN_128, DO_MAX_128 };
+enum DenseOp : int { DO_NONE = 0, DO_ADD_U64, DO_ADD_F64, DO_ADD_128, DO_MIN_S64, DO_MAX_S64, DO_MIN_U64, DO_MAX_U64, DO_MIN_128, DO_MAX_128 };
 struct DenseKey { int src /* virtual column */, pad; unsigned long long kmin, nvals /* max - min + 1: the index of NULL */, stride; };
-struct DenseAgg { int func, op, small, start, n, word /* value word(s) in a slot, -1 none */, nn_word /* non-null counter, -1 none */, pad; };
+struct DenseAgg { int func, op, small, start, n, word /* value word(s) in a slot, -1 none */, nn_word /* non-null counter, -1 none */,
+                  f64_key /* Float64 MIN / MAX: the word holds f64_to_ordered of the value */; };
 struct DenseParams {
   int n_keys, n_aggs, n_slots, n_words /* per slot, even: the 128-bit fields are 16-byte aligned; word 0 counts the rows */;
   DenseKey key[kDenseMaxKeys];
@@ -498,8 +487,6 @@ __device__ __forceinline__ bool dense_better(int op, unsigned long long lo, unsi
     case DO_MAX_S64: return (long long)lo > (long long)clo;
     case DO_MIN_U64: return lo < clo;
     case DO_MAX_U64: return lo > clo;
-    case DO_MIN_F64: return __longlong_as_double((long long)lo) < __longlong_as_double((long long)clo);
-    case DO_MAX_F64: return __longlong_as_double((long long)lo) > __longlong_as_double((long long)clo);
     case DO_MIN_128: return lt128(lo, hi, clo, chi);
     case DO_MAX_128: return lt128(clo, chi, lo, hi);
     default: return false;
@@ -526,15 +513,6 @@ __device__ __forceinline__ void dense_update(int op, unsigned long long* w, unsi
     case DO_MAX_S64: atomicMax((long long*)w, (long long)lo); break;
     case DO_MIN_U64: atomicMin(w, lo); break;
     case DO_MAX_U64: atomicMax(w, lo); break;
-    case DO_MIN_F64: case DO_MAX_F64: {
-      unsigned long long old = *(volatile unsigned long long*)w;
-      while (dense_better(op, lo, 0, old, 0)) {
-        const unsigned long long prev = atomicCAS(w, old, lo);
-        if (prev == old) break;
-        old = prev;
-      }
-      break;
-    }
     case DO_MIN_128: case DO_MAX_128: {
       // w is a generic address: shared memory in the row loop, global memory at the flush
       Rec128 cur = cas128<true>(w, Rec128{lo, hi}, Rec128{lo, hi});   // an atomic read of both words (stores only what is already there)
@@ -1031,8 +1009,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
               if (ag.small == 2) { lo = eval_int_fast(sp.pool + ag.start, ag.n, row[u], ext); ok = 1; }
               else if (DEC && ag.small == 3) { lo = pipe_eval_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, &hi); ok = err_ok[1] ? 1 : 0; }
               else { lo = pipe_eval<DEC>(sp.pool + ag.start, ag.n, ag.small, row[u], ext, err_ok); ok = err_ok[1] ? 1 : 0; }
-              // f64 MIN / MAX skip NaN as the join-keyed sink does (red_f64_min): it stays counted, the value becomes the identity
-              if (ok && (ag.op == DO_MIN_F64 || ag.op == DO_MAX_F64) && isnan(__longlong_as_double((long long)lo))) lo = dp.ident[ag.word];
+              if (ag.f64_key) lo = f64_to_ordered(__longlong_as_double((long long)lo));
             }
             if (!ok && ag.word >= 0) { lo = dp.ident[ag.word]; hi = ag.op == DO_MIN_128 || ag.op == DO_MAX_128 ? dp.ident[ag.word + 1] : 0ull; }
             dense_reduce_peers(peers, ag.op, lo, hi, ok);
@@ -1141,12 +1118,12 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
                 else red_add_u64(rec + ag.word, (unsigned long long)v);   // add_wrapping (sum.rs:316)
                 break;
               case DFGPU_AGG_MIN:
-                if (ag.cls == C_F64) red_f64_min(rec + ag.word, __longlong_as_double((long long)v), false);
+                if (ag.cls == C_F64) red_min_u64(rec + ag.word, f64_to_ordered(__longlong_as_double((long long)v)));
                 else if (ag.cls == C_U64) red_min_u64(rec + ag.word, (unsigned long long)v);
                 else red_min_s64(rec + ag.word, (long long)v);
                 break;
               case DFGPU_AGG_MAX:
-                if (ag.cls == C_F64) red_f64_min(rec + ag.word, __longlong_as_double((long long)v), true);
+                if (ag.cls == C_F64) red_max_u64(rec + ag.word, f64_to_ordered(__longlong_as_double((long long)v)));
                 else if (ag.cls == C_U64) red_max_u64(rec + ag.word, (unsigned long long)v);
                 else red_max_s64(rec + ag.word, (long long)v);
                 break;
@@ -1539,7 +1516,7 @@ struct EmitCol {
   int kind /* 0 key, 1 payload field, 2 accumulator word, 3 AVG value, 4 count as u64, 5 Decimal128 sum / min / max (two words),
               6 dense group key decoded from the slot number, 7 Decimal128 AVG value, 8 packed group field of a 128-bit tag in words 0 and 1,
               9 COUNT(*) of a LEFT join's build row: the row counter, at least 1 (the NULL-padded row of a record no probe row reached) */,
-      width, shift, word, nn_word, cnt_word, f64;
+      width, shift, word, nn_word, cnt_word, f64_key /* kind 2: the word holds f64_to_ordered of a Float64 MIN / MAX */;
   void* dst; uint32_t* valid;
   long long kmin; int kstride, kradix;   // kind 6: key = kmin + (slot / kstride) % kradix, NULL when that index is kradix - 1
   int avg_mul, avg_prec;                  // kind 7: sum * 10^avg_mul / count must fit Decimal128(avg_prec, _)
@@ -1561,7 +1538,10 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
         switch (e.kind) {
           case 0: v = r[0]; break;
           case 1: v = r[1] >> e.shift; break;
-          case 2: v = r[e.word]; ok = e.nn_word >= 0 ? r[e.nn_word] != 0ull : true; break;
+          case 2:
+            v = e.f64_key ? (uint64_t)__double_as_longlong(ordered_to_f64(r[e.word])) : r[e.word];
+            ok = e.nn_word >= 0 ? r[e.nn_word] != 0ull : true;
+            break;
           case 4: v = r[e.word]; break;
           case 9: v = max(r[e.word], 1ull); break;
           case 5:
@@ -2042,8 +2022,7 @@ static void prepare_acc(dfgpu_pipeline* p) {
     unsigned long long init, init_hi = 0;
     const bool is_min = ag.func == DFGPU_AGG_MIN;
     if (ag.cls == C_DEC) { init = is_min ? ~0ull : 0ull; init_hi = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN; }   // i128::MAX / MIN
-    else if (ag.cls == C_F64) { double d = is_min ? INFINITY : -INFINITY; memcpy(&init, &d, 8); }
-    else if (ag.cls == C_U64) init = is_min ? ~0ull : 0ull;
+    else if (ag.cls == C_U64 || ag.cls == C_F64) init = is_min ? ~0ull : 0ull;   // Float64: f64_to_ordered keys
     else init = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN;
     if (l->cap) {
       lookup_init_acc_kernel<<<grid_for((int64_t)l->cap, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, ag.word, init); DF_LAUNCH_CHECK(ctx);
@@ -2058,8 +2037,8 @@ static int dense_op(const PipeAgg& ag) {
   const bool wide = ag.cls == C_DEC, f = ag.cls == C_F64, u = ag.cls == C_U64;
   switch (ag.func) {
     case DFGPU_AGG_SUM: case DFGPU_AGG_AVG: return wide ? DO_ADD_128 : (f ? DO_ADD_F64 : DO_ADD_U64);
-    case DFGPU_AGG_MIN: return wide ? DO_MIN_128 : (f ? DO_MIN_F64 : (u ? DO_MIN_U64 : DO_MIN_S64));
-    case DFGPU_AGG_MAX: return wide ? DO_MAX_128 : (f ? DO_MAX_F64 : (u ? DO_MAX_U64 : DO_MAX_S64));
+    case DFGPU_AGG_MIN: return wide ? DO_MIN_128 : (f || u ? DO_MIN_U64 : DO_MIN_S64);   // Float64: its f64_to_ordered key
+    case DFGPU_AGG_MAX: return wide ? DO_MAX_128 : (f || u ? DO_MAX_U64 : DO_MAX_S64);
     default: return DO_NONE;
   }
 }
@@ -2100,6 +2079,7 @@ static void fill_dense(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePar
     const PipeAgg& ag = p->aggs[a];
     DenseAgg& d = dp->agg[a];
     d.func = ag.func; d.op = dense_op(ag);
+    d.f64_key = ag.cls == C_F64 && (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) ? 1 : 0;
     d.word = ag.func == DFGPU_AGG_COUNT ? -1 : ag.word;   // COUNT(x) is its non-null counter
     d.nn_word = ag.func == DFGPU_AGG_COUNT ? ag.word : ag.nn_word;
     if (ag.has_expr) {
@@ -2515,7 +2495,8 @@ static void add_agg_columns(const std::vector<PipeAgg>& aggs, int rows_word, boo
         } else { e.kind = 2; e.word = ag.word; e.nn_word = nn_word; add(sum_type, nn_word >= 0, e); }
         break;
       case DFGPU_AGG_MIN: case DFGPU_AGG_MAX:   // the argument's type; Decimal128 takes two words
-        e.kind = ag.cls == C_DEC ? 5 : 2; e.word = ag.word; e.nn_word = nn_word; add(ag.arg_type, nn_word >= 0, e);
+        e.kind = ag.cls == C_DEC ? 5 : 2; e.word = ag.word; e.nn_word = nn_word; e.f64_key = ag.cls == C_F64;
+        add(ag.arg_type, nn_word >= 0, e);
         break;
       case DFGPU_AGG_AVG:
         if (ag.cls == C_DEC) {   // Avg::return_type: Decimal128(min(38, p + 4), min(38, s + 4)) (average.rs); Single modes only
@@ -3056,8 +3037,7 @@ int dfgpu_pipeline_sink_aggregate_hash(dfgpu_pipeline* p, const int32_t* group_c
     const bool is_min = ag.func == DFGPU_AGG_MIN;
     unsigned long long& lo = p->hash_ident[ag.word];
     if (ag.cls == C_DEC) { lo = is_min ? ~0ull : 0ull; p->hash_ident[ag.word + 1] = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN; }
-    else if (ag.cls == C_F64) { const double d = is_min ? INFINITY : -INFINITY; memcpy(&lo, &d, 8); }
-    else if (ag.cls == C_U64) lo = is_min ? ~0ull : 0ull;
+    else if (ag.cls == C_U64 || ag.cls == C_F64) lo = is_min ? ~0ull : 0ull;   // Float64: f64_to_ordered keys
     else lo = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN;
   }
   p->hash_keys = std::move(keys);
@@ -3131,8 +3111,7 @@ int dfgpu_pipeline_sink_aggregate_dense(dfgpu_pipeline* p, const int32_t* group_
       unsigned long long lo = 0, hi = 0;   // MIN / MAX identities
       if (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) {
         if (ag.cls == C_DEC) { lo = is_min ? ~0ull : 0ull; hi = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN; }
-        else if (ag.cls == C_F64) { const double d = is_min ? INFINITY : -INFINITY; memcpy(&lo, &d, 8); }
-        else if (ag.cls == C_U64) lo = is_min ? ~0ull : 0ull;
+        else if (ag.cls == C_U64 || ag.cls == C_F64) lo = is_min ? ~0ull : 0ull;   // Float64: f64_to_ordered keys
         else lo = is_min ? (unsigned long long)LLONG_MAX : (unsigned long long)LLONG_MIN;
       }
       if (ag.func == DFGPU_AGG_COUNT) ag.word = take(1, 0, 0);

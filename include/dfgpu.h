@@ -368,7 +368,10 @@ typedef struct dfgpu_agg_desc {
  * and over Decimal128(p, s) -> Decimal128(min(38, p+4), min(38, s+4)) = sum * 10^(ts - s) / count truncated toward zero (DataFusion's
  * DecimalAverager::avg).  DFGPU_ERR_ARITH ("Arithmetic Overflow in AvgAccumulator") from dfgpu_agg_finish when that multiply overflows
  * i128 or the value exceeds the target precision.  AVG over Decimal128 has no defined Partial state: DFGPU_AGG_PARTIAL,
- * DFGPU_AGG_PARTIAL_REDUCE and the Final modes reject it with DFGPU_ERR_UNSUPPORTED; without GROUP BY it runs in the Single modes. */
+ * DFGPU_AGG_PARTIAL_REDUCE and the Final modes reject it with DFGPU_ERR_UNSUPPORTED; without GROUP BY it runs in the Single modes.
+ * Float MIN / MAX, here and in every pipeline aggregate sink, order by IEEE totalOrder on the value's bits: -NaN < -inf < ... < -0.0 <
+ * +0.0 < ... < +inf < +NaN, NaNs of one sign ordered by their payload bits.  The result is one of the group's input values bit for bit,
+ * it does not depend on row order, batch boundaries or thread timing, and a group without a non-NULL value is NULL. */
 int dfgpu_agg_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_cols,
                      const int32_t* group_cols, int32_t n_group,
                      const dfgpu_agg_desc* aggs, int32_t n_aggs,

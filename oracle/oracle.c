@@ -39,6 +39,8 @@
 #define SEED_REPART 0ull
 
 static inline uint64_t o_hash(uint64_t v, uint64_t seed) { return o_mix64(v ^ o_mix64(seed + 0x9E3779B97F4A7C15ull)); }
+/* a double's bits as an unsigned key that sorts in IEEE totalOrder: all bits flipped when the sign is set, else the sign bit set */
+static inline uint64_t f64_total_order(double d) { uint64_t b; memcpy(&b, &d, 8); return (b >> 63) ? ~b : (b | 0x8000000000000000ull); }
 
 static void create_hashes(int nkeys, const int64_t* const* keys, const uint8_t* const* valid, int64_t start, int64_t n,
                           uint64_t seed, int force_collisions, uint64_t* out) {
@@ -735,10 +737,10 @@ O_API int oracle_group_by(int nkeys, const int64_t* const* keys, const uint8_t* 
           case A_MIN: case A_MAX: {
             if (isnull) break;
             int first = A->seen ? !A->seen[g] : (A->counts[g] == 0);
-            if (in->is_float == 1) {
+            if (in->is_float == 1) {   /* IEEE totalOrder on the bits: -NaN < -inf < ... < -0.0 < +0.0 < ... < +inf < +NaN */
               double v = ((const double*)in->arg)[row];
-              if (first) A->fvals[g] = v;
-              else if (in->func == A_MIN ? (v < A->fvals[g]) : (v > A->fvals[g])) A->fvals[g] = v;
+              const uint64_t kv = f64_total_order(v), kc = f64_total_order(A->fvals[g]);
+              if (first || (in->func == A_MIN ? kv < kc : kv > kc)) A->fvals[g] = v;
             } else if (in->is_float == 2) {
               uint64_t v = ((const uint64_t*)in->arg)[row], cur = (uint64_t)A->ivals[g];
               if (first || (in->func == A_MIN ? v < cur : v > cur)) A->ivals[g] = (int64_t)v;

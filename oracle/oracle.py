@@ -933,6 +933,12 @@ def scalar_aggregate(aggs: Sequence[tuple], state: bool = False) -> List[Col]:
                 with np.errstate(over="ignore"):
                     out.append(one(sel.astype(dt).sum(dtype=dt) if cnt else 0, dt, cnt > 0))
         elif func in (A_MIN, A_MAX):
+            if vals.dtype.kind == "f" and cnt:   # IEEE totalOrder on the bits, as the grouped MIN / MAX
+                u = np.ascontiguousarray(sel).view(np.uint64 if vals.dtype.itemsize == 8 else np.uint32)
+                top = u.dtype.type(1 << (8 * u.dtype.itemsize - 1))
+                k = np.where(u & top, ~u, u | top)
+                out.append((sel[[np.argmin(k) if func == A_MIN else np.argmax(k)]], None))
+                continue
             out.append(one((sel.min() if func == A_MIN else sel.max()) if cnt else 0, vals.dtype, cnt > 0))
         elif func == A_AVG:
             sm = float(sel.astype(np.float64).sum()) if cnt else 0.0

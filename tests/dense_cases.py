@@ -8,6 +8,7 @@ import numpy as np
 from datafusion_b200 import capi as D
 from oracle import oracle as O
 import decimal_agg as DA
+import float_order as FO
 
 I64_MIN, I64_MAX, U64_MAX = -(1 << 63), (1 << 63) - 1, (1 << 64) - 1
 DEC38_MAX = 10 ** 38 - 1
@@ -108,6 +109,9 @@ def reference(cols, types, keep, group_cols, key_range, aggs, partial=False):
                 continue
             if not xs:
                 cells.append(None)
+            elif func in (D.AGG_MIN, D.AGG_MAX) and k == "f64":   # IEEE totalOrder on the bits
+                ordk = FO.order_key(np.asarray(xs, np.float64))
+                cells.append(xs[int(np.argmin(ordk) if func == D.AGG_MIN else np.argmax(ordk))])
             elif func == D.AGG_MIN:
                 cells.append(min(xs))
             elif func == D.AGG_MAX:
