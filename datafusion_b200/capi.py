@@ -164,7 +164,7 @@ EXPORTS = [
     "dfgpu_comm_unique_id", "dfgpu_comm_init", "dfgpu_comm_rank", "dfgpu_comm_size", "dfgpu_comm_barrier", "dfgpu_comm_allgather_i64", "dfgpu_comm_share",
     "dfgpu_comm_destroy", "dfgpu_exchange_create", "dfgpu_exchange_run", "dfgpu_exchange_columns", "dfgpu_exchange_destroy",
     "dfgpu_lookup_default_options", "dfgpu_lookup_create", "dfgpu_lookup_metric", "dfgpu_lookup_destroy", "dfgpu_lookup_clear",
-    "dfgpu_lookup_filter_buffer", "dfgpu_lookup_filter_allreduce_peer", "dfgpu_pipeline_sink_output_unordered", "dfgpu_pipeline_set_name", "dfgpu_column_minmax_device", "dfgpu_column_sum_device",
+    "dfgpu_lookup_filter_buffer", "dfgpu_lookup_filter_allreduce_peer", "dfgpu_pipeline_sink_output_unordered", "dfgpu_pipeline_set_name", "dfgpu_pipeline_set_stage_filter", "dfgpu_column_minmax_device", "dfgpu_column_sum_device",
     "dfgpu_pipeline_create", "dfgpu_pipeline_sink_build", "dfgpu_pipeline_sink_aggregate", "dfgpu_pipeline_sink_aggregate_dense",
     "dfgpu_pipeline_sink_aggregate_hash", "dfgpu_pipeline_sink_output",
     "dfgpu_pipeline_push_host", "dfgpu_pipeline_push_device", "dfgpu_pipeline_push_arrow", "dfgpu_pipeline_finish",
@@ -295,6 +295,7 @@ def load_library() -> C.CDLL:
     sig("dfgpu_pipeline_sink_aggregate_hash", C.c_int, [vp, P(i32), P(i32), i32, P(PipelineAgg), i32, i32, i64, i64])
     sig("dfgpu_pipeline_sink_output", C.c_int, [vp, P(i32), i32, i64])
     sig("dfgpu_pipeline_set_name", C.c_int, [vp, C.c_char_p])
+    sig("dfgpu_pipeline_set_stage_filter", C.c_int, [vp, i32, P(ExprNode), i32])
     sig("dfgpu_pipeline_push_host", C.c_int, [vp, P(Column), i32])
     sig("dfgpu_pipeline_push_device", C.c_int, [vp, P(Column), i32])
     sig("dfgpu_pipeline_push_arrow", C.c_int, [vp, vp, vp])
@@ -829,6 +830,12 @@ class Pipeline(_Operator):
                                                 sa, len(stages), C.byref(self.h)))
         if name:
             ctx.check(ctx.lib.dfgpu_pipeline_set_name(self.h, name.encode()))
+
+    def set_stage_filter(self, stage: int, nodes):
+        """JoinFilter of probe stage `stage`: RPN over the input columns, the payload fields of the INNER / LEFT / LEFT_ANTI stages up to
+        this one, then (SEMI / ANTI stages) this stage's own payload fields; a candidate pair matches only when it is TRUE"""
+        na = expr_nodes(nodes)
+        self.ctx.check(self.ctx.lib.dfgpu_pipeline_set_stage_filter(self.h, int(stage), na, len(nodes)))
 
     def sink_build(self, target: Lookup, key_col: int, payload_cols=()):
         self._keep.append(target)

@@ -14,8 +14,8 @@ struct ExprPlan {
   bool has_decimal = false;        // some node reads or produces a Decimal128: evaluated on the 128-bit stack (expr_dec.cuh)
   std::vector<int64_t> aux;        // per node: power-of-ten rescale exponents of decimal BINARY / CAST nodes
 };
-// type inference + validation of a post-order program against a schema
-ExprPlan plan_expr(const int32_t* schema_types, int n_cols, const dfgpu_expr_node* nodes, int n_nodes);
+// type inference + validation of a post-order program against a schema; max_nodes: the evaluator's program size (EProgram holds 48)
+ExprPlan plan_expr(const int32_t* schema_types, int n_cols, const dfgpu_expr_node* nodes, int n_nodes, int max_nodes = 48);
 
 uint64_t literal_bits(const dfgpu_expr_node& nd);
 // Per batch: which guards are active (the reference would not evaluate the RHS on every row).  Evaluates each guard's LHS over the batch

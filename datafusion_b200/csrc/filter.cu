@@ -254,8 +254,8 @@ static bool expr_type_ok(int t) {
   return t == DFGPU_BOOL || type_is_int(t) || type_is_float(t);
 }
 
-ExprPlan plan_expr(const int32_t* schema_types, int n_cols, const dfgpu_expr_node* nodes, int n_nodes) {
-  DF_CHECK(n_nodes >= 1 && n_nodes <= kMaxNodes, DFGPU_ERR_UNSUPPORTED, "expression: 1..48 nodes supported");
+ExprPlan plan_expr(const int32_t* schema_types, int n_cols, const dfgpu_expr_node* nodes, int n_nodes, int max_nodes) {
+  DF_CHECK(n_nodes >= 1 && n_nodes <= max_nodes, DFGPU_ERR_UNSUPPORTED, max_nodes == kMaxNodes ? "expression: 1..48 nodes supported" : "expression: too many nodes");
   ExprPlan p;
   p.nodes.assign(nodes, nodes + n_nodes);
   p.in_type.assign(n_nodes, 0);

@@ -396,6 +396,9 @@ __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_
 //   bit 7 (128) partitioned aggregate (with bit 6; pipeline_push decides, partitioned_parts): the aggregate stage's table exceeds L2, so
 //              phase B makes no lookup — it writes each survivor's {key, SUM argument} to the record buffer (out_dst, out_counter), and
 //              pipe_probe_agg_kernel probes them once they are radix-partitioned.  Rows past the buffer's end probe and RED right here.
+//   bit 8 (256) stage filters (FiltParams; launch_pipe picks it whenever a stage has one, on top of the sink's default bits, never with
+//              bits 6 / 7): phase B evaluates a stage's JoinFilter on the rows whose key matched there, and a row that fails counts as
+//              not matched; a filtered bitmap ANTI stage is decided in phase B instead of phase A.
 // DFGPU_PIPE_VAR selects the instantiation (aggregate sink; bits 1 and 5 also for the pack sink, bit 1 for the unordered-output sink); 0 is the
 // kernel without any of them, 11 the default.  Tried and removed: four instead of two survivors per lane and phase-B round; prefetching the
 // table record and the argument sectors already when a row passes the membership filter in phase A (the prefetches of five tiles queue up
@@ -454,6 +457,28 @@ struct HashParams {
   uint32_t* overflow; unsigned long long* overflow_count;   // deferred input rows of this launch
 };
 struct HashIdent { unsigned long long w[kHashMaxWords]; };   // initial value of each record word (tag words ~0, MIN / MAX identities)
+
+// ------------------------------------------------------------------------------------------
+// stage filters (pipe_kernel VAR bit 256, pipe_output_kernel<true>): the JoinFilter of a probe stage, a Boolean program evaluated on each
+// row whose key matched at that stage.  The programs have a node pool of their own; the block sits behind DenseParams / HashParams in the
+// parameter buffer and is copied to dynamic shared memory at smem_off (behind the sink's own block there), so PipeParams and every
+// instantiation without the bit are unchanged.
+// ------------------------------------------------------------------------------------------
+constexpr int kFiltPoolNodes = 128, kVarFilt = 256;
+struct FiltParams {
+  int smem_off;                                                  // byte offset of this block in the kernel's dynamic shared memory
+  int start[kMaxStages], n[kMaxStages] /* 0: no filter */, small[kMaxStages];
+  ENode pool[kFiltPoolNodes];
+};
+constexpr int kFiltParamsOff = kDenseParamsOff + (int)(((sizeof(DenseParams) > sizeof(HashParams) ? sizeof(DenseParams) : sizeof(HashParams)) + 15) / 16 * 16);
+// stage s's filter on one candidate pair (ext: the payload words of stages 0..s): TRUE passes, NULL and FALSE do not; errors are or-ed
+// into err_ok[0], so only candidate pairs raise
+template <bool DEC>
+__device__ __forceinline__ bool stage_filter_pass(const FiltParams& fp, int s, int64_t row, const uint64_t* ext, int* err_ok) {
+  if (fp.n[s] == 0) return true;
+  const uint64_t v = pipe_eval<DEC>(fp.pool + fp.start[s], fp.n[s], fp.small[s], row, ext, err_ok);
+  return err_ok[1] && (v & 1);
+}
 
 __device__ __forceinline__ uint64_t hash_tag_slot(uint64_t lo, uint64_t hi, uint64_t cap) { return __umul64hi(hash_combine(hash_u64(lo, kSeedAgg), hi), cap); }
 // the record of tag {lo, hi}, claimed when absent; nullptr when the row must be deferred (claim budget exhausted or probe too long)
@@ -556,7 +581,8 @@ __device__ __forceinline__ void dense_reduce_peers(unsigned peers, int op, unsig
 template <int SINK, bool DEC, int VAR = 0>
 __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PACK) || SINK == SINK_DENSE) ? 2 : 3) pipe_kernel(const PipeParams* __restrict__ gp, int64_t n, unsigned long long* __restrict__ counters /* [alive, inserted, fail, err] */) {
   constexpr int PB = kPhaseB, PBG = kPhaseBGroup, QC = kQueueCap;
-  constexpr bool RING = (VAR & 64) != 0, PART = (VAR & 128) != 0;
+  constexpr bool RING = (VAR & 64) != 0, PART = (VAR & 128) != 0, FILT = (VAR & kVarFilt) != 0;
+  static_assert(!FILT || !(RING || PART), "stage filters do not run on the ring-fed or partitioned paths");
   __shared__ PipeParams sp;
   __shared__ uint32_t q_rows[kPipeWarps][QC];
   extern __shared__ __align__(128) unsigned char dyn_smem[];   // RING: mbarriers [warp][stage], then the rings [warp][stage][ring_bytes]
@@ -575,6 +601,12 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
   if constexpr (SINK == SINK_HASH) {   // dynamic shared memory: HashParams
     const uint32_t* src = (const uint32_t*)((const char*)gp + kDenseParamsOff);
     for (int i = threadIdx.x; i < (int)(sizeof(HashParams) / 4); i += kPipeThreads) ((uint32_t*)dyn_smem)[i] = src[i];
+  }
+  const FiltParams* fpp = nullptr;   // FILT: the stage filters, in dynamic shared memory behind the sink's block
+  if constexpr (FILT) {
+    const FiltParams* g = (const FiltParams*)((const char*)gp + kFiltParamsOff);
+    fpp = (const FiltParams*)(dyn_smem + g->smem_off);
+    for (int i = threadIdx.x; i < (int)(sizeof(FiltParams) / 4); i += kPipeThreads) ((uint32_t*)fpp)[i] = ((const uint32_t*)g)[i];
   }
   __syncthreads();
   if constexpr (SINK == SINK_DENSE) {
@@ -706,6 +738,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
       for (int s = 0; s < sp.n_stages; ++s) {
         const StageDev& st = sp.stage[s];
         const bool bitmap = st.lk.mode == LK_BITMAP;
+        if constexpr (FILT) if (bitmap && st.kind == DFGPU_STAGE_ANTI && fpp->n[s] > 0) continue;   // a key match alone drops nothing: phase B
         if (!bitmap && !(st.lk.bloom && st.kind != DFGPU_STAGE_ANTI)) {   // nothing cheap to test; NULL keys of an inner / semi stage still drop here
           if (st.kind != DFGPU_STAGE_ANTI && sp.col[st.key_col].valid) mask &= valid8(sp.col[st.key_col], row0, n);
           continue;
@@ -822,6 +855,28 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
         for (int u = 0; u < PB; ++u) pay[s][u] = 0;
         if (s >= sp.n_stages) continue;
         const StageDev& st = sp.stage[s];
+        if constexpr (FILT) {
+          if (st.lk.mode == LK_BITMAP && fpp->n[s] > 0) {   // phase A kept the matches of an INNER / SEMI stage; an ANTI stage is probed here
+#pragma unroll
+            for (int u = 0; u < PB; ++u) {
+              if (!live[u]) continue;
+              bool found = true;
+              if (st.kind == DFGPU_STAGE_ANTI) {
+                const ColRef& kc = sp.col[st.key_col];
+                const uint64_t i = ld_stream_int(kc.ptr, kc.width, kc.sgn, row[u], pol_stream) - st.lk.kmin;
+                found = !(kc.valid && !bit_get(kc.valid, kc.voff + row[u])) && i < st.lk.ksize && ((__ldg(&st.lk.bits[i >> 5]) >> (i & 31)) & 1u);
+              }
+              if (found) {
+                uint64_t ext[kMaxStages];
+#pragma unroll
+                for (int k = 0; k < kMaxStages; ++k) ext[k] = k < s ? pay[k][u] : 0ull;
+                found = stage_filter_pass<DEC>(*fpp, s, row[u], ext, err_ok);
+              }
+              live[u] = st.kind == DFGPU_STAGE_ANTI ? !found : found;
+            }
+            continue;
+          }
+        }
         if (st.lk.mode == LK_BITMAP || st.kind == kStageMaybe) continue;   // decided in phase A
         const ColRef kc = sp.col[st.key_col];
         uint64_t key[PB], slot[PB], ck[PB], cp[PB];
@@ -856,7 +911,16 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
               if (st.lk.has_payload) { const uint4 v = __ldcg((const uint4*)r); ck[u] = (uint64_t)v.x | ((uint64_t)v.y << 32); cp[u] = (uint64_t)v.z | ((uint64_t)v.w << 32); }
               else ck[u] = __ldcg(r);
             }
-            if (found[u]) { pay[s][u] = cp[u]; if (SINK == SINK_AGG && s == sp.agg_stage) arec[u] = st.lk.recs + slot[u] * (uint64_t)st.lk.stride; }
+            if (found[u]) {
+              pay[s][u] = cp[u];
+              if constexpr (FILT) {   // a candidate pair the filter rejects is no match: a LEFT stage's record is not touched
+                uint64_t ext[kMaxStages];
+#pragma unroll
+                for (int k = 0; k < kMaxStages; ++k) ext[k] = k <= s ? pay[k][u] : 0ull;
+                found[u] = stage_filter_pass<DEC>(*fpp, s, row[u], ext, err_ok);
+              }
+              if (SINK == SINK_AGG && s == sp.agg_stage && (!FILT || found[u])) arec[u] = st.lk.recs + slot[u] * (uint64_t)st.lk.stride;
+            }
           }
           live[u] = live[u] && (st.kind == DFGPU_STAGE_ANTI ? !found[u] : found[u]);
         }
@@ -1262,6 +1326,9 @@ __global__ void __launch_bounds__(256) pipe_probe_agg_kernel(const ulonglong2* _
 // ------------------------------------------------------------------------------------------
 struct OutCols { int n; int src[kMaxPipeCols]; int width[kMaxPipeCols]; void* dst[kMaxPipeCols]; };
 
+// FILT: the stage filters (FiltParams at offset 0 of the dynamic shared memory), evaluated on each candidate pair with the interpreter of
+// pipe_kernel's DEC instantiations
+template <bool FILT>
 __global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipeParams* __restrict__ gp, int64_t n, OutCols oc, unsigned long long* __restrict__ tile_desc,
                                                                   unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
   __shared__ PipeParams sp;
@@ -1269,7 +1336,12 @@ __global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipePar
   __shared__ unsigned long long s_pay[kMaxStages][kPipeTile];
   __shared__ unsigned int s_tile;
   __shared__ unsigned long long s_base;
+  extern __shared__ __align__(128) unsigned char dyn_smem[];
   for (int i = threadIdx.x; i < (int)(sizeof(PipeParams) / 4); i += kPipeThreads) ((uint32_t*)&sp)[i] = ((const uint32_t*)gp)[i];
+  if constexpr (FILT) {
+    const uint32_t* src = (const uint32_t*)((const char*)gp + kFiltParamsOff);
+    for (int i = threadIdx.x; i < (int)(sizeof(FiltParams) / 4); i += kPipeThreads) ((uint32_t*)dyn_smem)[i] = src[i];
+  }
   if (threadIdx.x == 0) s_tile = atomicAdd(tile_counter, 1u);
   __syncthreads();
   const int64_t tile = s_tile;
@@ -1339,6 +1411,16 @@ __global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipePar
               if (++slot == st.lk.cap) slot = 0;
             }
           }
+        }
+      }
+      if constexpr (FILT) {
+        if (found) {
+          uint64_t ext[kMaxStages];
+#pragma unroll
+          for (int q = 0; q < kMaxStages; ++q) ext[q] = pay[q][k];
+          int eo[2] = {err, 0};
+          found = stage_filter_pass<true>(*(const FiltParams*)dyn_smem, s, row, ext, eo);
+          err = eo[0];
         }
       }
       alive[k] = st.kind == DFGPU_STAGE_ANTI ? !found : found;
@@ -1678,6 +1760,10 @@ struct dfgpu_pipeline {
   bool has_pred = false;
   ExprPlan pred;
   std::vector<dfgpu_pipeline_stage> stages;
+  // stage filters (dfgpu_pipeline_set_stage_filter): per stage the program and the payload fields its virtual columns past the inputs name
+  ExprPlan filt[kMaxStages]; bool has_filt[kMaxStages] = {false, false, false}; std::vector<ExtDef> filt_ext[kMaxStages]; int filt_nodes = 0;
+  std::unique_ptr<FiltParams> filt_host;   // staging copy of the bound programs (upload_filters)
+  bool pushed = false;
   int sink = SINK_NONE;
   // build sink
   dfgpu_lookup* target = nullptr; int bkey_col = -1; std::vector<int> bpay_cols;
@@ -1758,15 +1844,12 @@ static ColRef col_ref(const DCol& c) {
   return r;
 }
 
-// bind a planned expression into pool nodes; virtual columns >= n_cols become payload-field nodes
-static int bind_pool(const dfgpu_pipeline* p, const ExprPlan& plan, const std::vector<DCol>& cols, PipeParams* pp, int* pool_used) {
-  const int start = *pool_used;
-  const int64_t n_rows = cols.empty() ? 0 : cols[0].length;
-  const auto gmasks = resolve_guards(p->ctx, plan, cols, n_rows);   // short-circuit AND / OR: which RHS errors count on which rows (binary.rs:1182)
-  DF_CHECK(start + (int)plan.nodes.size() <= kPoolNodes, DFGPU_ERR_UNSUPPORTED, "pipeline: expressions too large (56 nodes in total)");
+// bind a planned expression into nodes at `out`; virtual columns >= n_cols become the payload fields exts[column - n_cols]
+static void bind_nodes(const ExprPlan& plan, const std::vector<DCol>& cols, const std::vector<ExtDef>& exts, const std::vector<std::pair<uint16_t, uint16_t>>& gmasks,
+                       ENode* out) {
   for (size_t i = 0; i < plan.nodes.size(); ++i) {
     const dfgpu_expr_node& nd = plan.nodes[i];
-    ENode& e = pp->pool[start + i];
+    ENode& e = out[i];
     memset(&e, 0, sizeof(e));
     e.kind = nd.kind; e.op = nd.a; e.in_type = plan.in_type[i]; e.out_type = plan.out_type[i];
     if (nd.kind == DFGPU_EXPR_COLUMN) {
@@ -1774,7 +1857,7 @@ static int bind_pool(const dfgpu_pipeline* p, const ExprPlan& plan, const std::v
         const DCol& c = cols[nd.a];
         e.col = c.values; e.valid = c.validity; e.voff = c.offset;
       } else {
-        const ExtDef& x = p->exts[nd.a - (int)cols.size()];
+        const ExtDef& x = exts[nd.a - (int)cols.size()];
         e.kind = kExprExt; e.voff = x.stage; e.lit = (uint64_t)x.shift;
       }
     } else if (nd.kind == DFGPU_EXPR_LITERAL) {
@@ -1785,8 +1868,44 @@ static int bind_pool(const dfgpu_pipeline* p, const ExprPlan& plan, const std::v
     }
     e.g_and = gmasks[i].first; e.g_or = gmasks[i].second;
   }
+}
+
+// bind a planned expression into pool nodes; virtual columns >= n_cols become payload-field nodes
+static int bind_pool(const dfgpu_pipeline* p, const ExprPlan& plan, const std::vector<DCol>& cols, PipeParams* pp, int* pool_used) {
+  const int start = *pool_used;
+  const int64_t n_rows = cols.empty() ? 0 : cols[0].length;
+  const auto gmasks = resolve_guards(p->ctx, plan, cols, n_rows);   // short-circuit AND / OR: which RHS errors count on which rows (binary.rs:1182)
+  DF_CHECK(start + (int)plan.nodes.size() <= kPoolNodes, DFGPU_ERR_UNSUPPORTED, "pipeline: expressions too large (56 nodes in total)");
+  bind_nodes(plan, cols, p->exts, gmasks, pp->pool + start);
   *pool_used = start + (int)plan.nodes.size();
   return start;
+}
+
+static bool pipeline_has_filters(const dfgpu_pipeline* p) { return p->filt_nodes > 0; }
+
+// byte offset of FiltParams in pipe_kernel's dynamic shared memory: behind the hash sink's HashParams or the dense sink's slots
+static int filt_smem_off(const dfgpu_pipeline* p);
+static int plan_depth(const ExprPlan& plan);
+
+// the stage filters for one batch, into the parameter buffer behind PipeParams and the sink's block (the pointers address `cols`)
+static void upload_filters(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
+  FiltParams& fp = *p->filt_host;
+  memset(&fp, 0, sizeof(fp));
+  fp.smem_off = filt_smem_off(p);
+  int used = 0;
+  for (int s = 0; s < kMaxStages; ++s) {
+    if (!p->has_filt[s]) continue;
+    const ExprPlan& plan = p->filt[s];
+    // no guards: set_stage_filter admits no AND / OR whose right operand can raise
+    bind_nodes(plan, cols, p->filt_ext[s], std::vector<std::pair<uint16_t, uint16_t>>(plan.nodes.size(), {0, 0}), fp.pool + used);
+    fp.start[s] = used; fp.n[s] = (int)plan.nodes.size();
+    fp.small[s] = plan.has_decimal ? 3 : (plan_depth(plan) <= 4 ? 1 : 0);
+    used += fp.n[s];
+  }
+  const size_t bytes = kFiltParamsOff + sizeof(FiltParams);
+  if (p->params_dev.bytes < bytes) p->params_dev.alloc(p->ctx, bytes);
+  // filt_host lives as long as the pipeline, and every push synchronises before the next batch rewrites it
+  DF_CUDA(cudaMemcpyAsync((char*)p->params_dev.ptr + kFiltParamsOff, &fp, sizeof(FiltParams), cudaMemcpyHostToDevice, p->ctx->stream));
 }
 
 // largest evaluation-stack depth of a post-order program (the register-resident interpreter handles <= 4)
@@ -1938,7 +2057,8 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
       }
     }
   }
-  fill_ring(pp, ring_smem(p->sink));
+  if (pipeline_has_filters(p)) upload_filters(p, cols);   // the ring-fed and partitioned paths take no stage filters
+  else fill_ring(pp, ring_smem(p->sink));
 }
 
 static void check_errors(unsigned long long err) {
@@ -1948,10 +2068,32 @@ static void check_errors(unsigned long long err) {
   if (err & kErrRingAgg) throw Error(DFGPU_ERR_INVALID, "internal: the ring-fed pipeline kernel was given an aggregate it does not evaluate");
 }
 
+static bool pipeline_has_decimal(const dfgpu_pipeline* p);
+
+// the sink's default VAR bits (launch_pipe below) plus the stage filters
+constexpr int filt_var(int sink) { return kVarFilt | (sink == SINK_AGG ? kPipeVarDefault : (sink == SINK_PACK || sink == SINK_OUTPUT_ANY ? 2 : 0)); }
+
 template <int SINK>
 static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, const char* timer_name, bool part = false) {
   dfgpu_ctx* ctx = p->ctx;
   const int64_t ntiles = (n + kPipeTile - 1) / kPipeTile;
+  // FiltParams in dynamic shared memory; Decimal128 programs anywhere take the 128-bit interpreter.  There is one filtered instantiation
+  // per sink and interpreter, so DFGPU_PIPE_VAR (which picks among the unfiltered ones) does not apply; DFGPU_PIPE_BLOCKS_PER_SM does.
+  if (pipeline_has_filters(p)) {
+    DF_CHECK(!part, DFGPU_ERR_INVALID, "internal: the partitioned aggregate takes no stage filters");
+    void (*kern)(const PipeParams*, int64_t, unsigned long long*) =
+        pipeline_has_decimal(p) ? pipe_kernel<SINK, true, kVarFilt> : pipe_kernel<SINK, false, filt_var(SINK)>;
+    DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FiltParams)));   // per device: on every launch
+    static const int blocks_env_f = getenv("DFGPU_PIPE_BLOCKS_PER_SM") ? atoi(getenv("DFGPU_PIPE_BLOCKS_PER_SM")) : 0;
+    int blocks_per_sm = blocks_env_f;
+    if (blocks_per_sm <= 0) DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, sizeof(FiltParams)));
+    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
+    const std::string tname = p->name.empty() ? std::string(timer_name) : "pipe:" + p->name;
+    KernelTimer kt(ctx, tname.c_str());
+    kern<<<grid, kPipeThreads, sizeof(FiltParams), ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, p->counters.as<unsigned long long>());
+    DF_LAUNCH_CHECK(ctx);
+    return;
+  }
   // programs that touch Decimal128 values run a second instantiation of the kernel (128-bit interpreter linked in): the integer
   // instantiation stays byte for byte what it was
   bool dec = p->has_pred && p->pred.has_decimal;
@@ -2094,7 +2236,16 @@ static void fill_dense(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePar
 static bool pipeline_has_decimal(const dfgpu_pipeline* p) {
   bool dec = p->has_pred && p->pred.has_decimal;
   for (const auto& ag : p->aggs) dec = dec || (ag.has_expr && ag.plan.has_decimal);
+  for (int s = 0; s < kMaxStages; ++s) dec = dec || (p->has_filt[s] && p->filt[s].has_decimal);
   return dec;
+}
+
+static int dense_smem(const dfgpu_pipeline* p) { return kDenseAccOff + (dense_per_warp(p) ? kPipeWarps : 1) * p->dense_slots * p->dense_words * 8; }
+
+static int filt_smem_off(const dfgpu_pipeline* p) {
+  if (p->sink == SINK_DENSE) return (dense_smem(p) + 15) / 16 * 16;
+  if (p->sink == SINK_HASH) return (int)((sizeof(HashParams) + 15) / 16 * 16);
+  return 0;
 }
 
 static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DenseParams& dp, int64_t n) {
@@ -2105,7 +2256,11 @@ static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DensePar
   DF_CUDA(cudaStreamSynchronize(ctx->stream));   // `pp` and `dp` live on the caller's stack frame
   // programs that touch Decimal128 values run the instantiation with the 128-bit interpreter
   void (*kern)(const PipeParams*, int64_t, unsigned long long*) = pipeline_has_decimal(p) ? pipe_kernel<SINK_DENSE, true> : pipe_kernel<SINK_DENSE, false>;
-  const int smem = kDenseAccOff + (dp.per_warp ? kPipeWarps : 1) * p->dense_slots * p->dense_words * 8;
+  int smem = kDenseAccOff + (dp.per_warp ? kPipeWarps : 1) * p->dense_slots * p->dense_words * 8;
+  if (pipeline_has_filters(p)) {   // the stage filters behind the slots
+    kern = pipeline_has_decimal(p) ? pipe_kernel<SINK_DENSE, true, kVarFilt> : pipe_kernel<SINK_DENSE, false, filt_var(SINK_DENSE)>;
+    smem = filt_smem_off(p) + (int)sizeof(FiltParams);
+  }
   DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));   // per device: set on every launch
   int blocks_per_sm = 0;
   DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, smem));
@@ -2125,6 +2280,7 @@ static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DensePar
 // the batch keeps the direct probe.  force_parts >= 2 (a test hook) admits tables of any size.
 static size_t partitioned_table_bytes(const dfgpu_pipeline* p, const PipeParams& pp, int force_parts) {
   if (pp.ring_stages == 0 || pipeline_has_decimal(p) || getenv("DFGPU_PIPE_VAR")) return 0;   // launch_pipe's ring kernel runs
+  if (pipeline_has_filters(p)) return 0;
   if (pp.agg_stage < 0 || p->left_kind) return 0;
   for (int s = 0; s < pp.n_stages; ++s)
     if (s != pp.agg_stage && pp.stage[s].lk.mode == LK_HASH && pp.stage[s].kind != kStageMaybe) return 0;
@@ -2176,8 +2332,14 @@ static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t 
   if (p->params_dev.bytes < pbytes) p->params_dev.alloc(ctx, pbytes);
   // programs that touch Decimal128 values run the instantiation with the 128-bit interpreter
   void (*kern)(const PipeParams*, int64_t, unsigned long long*) = pipeline_has_decimal(p) ? pipe_kernel<SINK_HASH, true> : pipe_kernel<SINK_HASH, false>;
+  int smem = (int)sizeof(HashParams);
+  if (pipeline_has_filters(p)) {   // the stage filters behind HashParams
+    kern = pipeline_has_decimal(p) ? pipe_kernel<SINK_HASH, true, kVarFilt> : pipe_kernel<SINK_HASH, false, filt_var(SINK_HASH)>;
+    smem = filt_smem_off(p) + (int)sizeof(FiltParams);
+    DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));   // per device: on every launch
+  }
   int blocks_per_sm = 0;
-  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, sizeof(HashParams)));
+  DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, smem));
   const std::string tname = p->name.empty() ? std::string("pipeline_hash") : "pipe:" + p->name;
   constexpr int64_t kMaxChunk = 1ll << 26;
   int64_t chunk = std::max<int64_t>((int64_t)p->hash_cap / 2, 1 << 20);
@@ -2209,7 +2371,7 @@ static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t 
       const int grid = (int)std::min<int64_t>((rows + kPipeTile - 1) / kPipeTile, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
       {
         KernelTimer kt(ctx, tname.c_str());
-        kern<<<grid, kPipeThreads, sizeof(HashParams), ctx->stream>>>((const PipeParams*)p->params_dev.ptr, rows, p->counters.as<unsigned long long>());
+        kern<<<grid, kPipeThreads, smem, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, rows, p->counters.as<unsigned long long>());
         DF_LAUNCH_CHECK(ctx);
       }
       unsigned long long h8[8];
@@ -2257,6 +2419,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   DF_CHECK(p->sink != SINK_NONE, DFGPU_ERR_STATE, "pipeline: choose a sink before the first push");
   DF_CHECK(cols.size() == p->in_types.size(), DFGPU_ERR_INVALID, "pipeline input column count mismatch");
   check_left_build(p);
+  p->pushed = true;
   dfgpu_ctx* ctx = p->ctx;
   set_device(ctx);
   const int64_t n = cols.empty() ? 0 : cols[0].length;
@@ -2445,7 +2608,12 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     unsigned int* counter = (unsigned int*)(totals + 2);
     {
       KernelTimer kt(ctx, "pipeline_output");
-      pipe_output_kernel<<<(int)nt, kPipeThreads, 0, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, oc, desc.as<unsigned long long>(), counter, totals, p->counters.as<unsigned long long>());
+      if (pipeline_has_filters(p)) {
+        DF_CUDA(cudaFuncSetAttribute(pipe_output_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FiltParams)));
+        pipe_output_kernel<true><<<(int)nt, kPipeThreads, sizeof(FiltParams), ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, oc, desc.as<unsigned long long>(), counter,
+                                                                                           totals, p->counters.as<unsigned long long>());
+      } else
+        pipe_output_kernel<false><<<(int)nt, kPipeThreads, 0, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, oc, desc.as<unsigned long long>(), counter, totals, p->counters.as<unsigned long long>());
       DF_LAUNCH_CHECK(ctx);
     }
     unsigned long long tot[2];
@@ -3157,6 +3325,36 @@ int dfgpu_pipeline_set_name(dfgpu_pipeline* p, const char* name) {
   if (!p || !name) return DFGPU_ERR_INVALID;
   p->name = name;
   return DFGPU_OK;
+}
+
+int dfgpu_pipeline_set_stage_filter(dfgpu_pipeline* p, int32_t stage, const dfgpu_expr_node* expr, int32_t n_nodes) {
+  DF_API_BEGIN(p ? p->ctx : nullptr)
+  DF_CHECK(p && expr && n_nodes > 0, DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(stage >= 0 && stage < (int)p->stages.size(), DFGPU_ERR_INVALID, "pipeline stage filter: stage out of range");
+  DF_CHECK(!p->pushed, DFGPU_ERR_STATE, "pipeline stage filter: set before the first push");
+  DF_CHECK(!p->has_filt[stage], DFGPU_ERR_STATE, "pipeline stage filter: the stage already has one");
+  const dfgpu_pipeline_stage& st = p->stages[stage];
+  DF_CHECK(st.kind != DFGPU_STAGE_MAYBE, DFGPU_ERR_UNSUPPORTED, "pipeline stage filter: a MAYBE stage has no candidate row to test");
+  // the filter's columns: the inputs, the payload fields of the INNER / LEFT / LEFT_ANTI stages 0..stage, then a SEMI / ANTI stage's own
+  const int nin = (int)p->in_types.size();
+  std::vector<int> types(p->in_types);
+  std::vector<ExtDef> exts;
+  for (size_t e = 0; e < p->exts.size() && p->exts[e].stage <= stage; ++e) { exts.push_back(p->exts[e]); types.push_back(p->vtypes[nin + e]); }
+  if (st.kind == DFGPU_STAGE_SEMI || st.kind == DFGPU_STAGE_ANTI)
+    for (size_t f = 0; f < st.lookup->pay_types.size(); ++f) {
+      ExtDef e; e.stage = stage; e.shift = st.lookup->pay_shift[f]; e.width = type_width(st.lookup->pay_types[f]); e.type = st.lookup->pay_types[f];
+      exts.push_back(e); types.push_back(e.type);
+    }
+  DF_CHECK(p->filt_nodes + n_nodes <= kFiltPoolNodes, DFGPU_ERR_UNSUPPORTED, "pipeline stage filter: the filters of a pipeline hold at most 128 nodes");
+  ExprPlan plan = plan_expr(types.data(), (int)types.size(), expr, n_nodes, kFiltPoolNodes);   // the filters' own pool, not EProgram
+  DF_CHECK(plan.root_type == DFGPU_BOOL, DFGPU_ERR_INVALID, "pipeline stage filter: the filter must be Boolean");
+  // the short-circuit guards are resolved per batch on the host, which cannot see payload fields
+  DF_CHECK(plan.guards.empty(), DFGPU_ERR_UNSUPPORTED,
+           "pipeline stage filter: an AND / OR whose right operand can raise (division, modulo, CAST, Decimal128 arithmetic) stays on dfgpu_hashjoin");
+  if (!p->filt_host) p->filt_host.reset(new FiltParams());
+  p->filt[stage] = std::move(plan); p->filt_ext[stage] = std::move(exts); p->has_filt[stage] = true;
+  p->filt_nodes += n_nodes;
+  DF_API_END
 }
 
 int dfgpu_pipeline_push_device(dfgpu_pipeline* p, const dfgpu_column* cols, int32_t n_cols) {

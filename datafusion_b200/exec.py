@@ -625,6 +625,7 @@ class _Scan:
         self.source, self.predicate = source, predicate
         self.stages: List[Tuple[int, str, "GpuPipelineExec"]] = []     # (stage kind, probe key column, build pipeline)
         self.visible: List[str] = [f.name for f in source.schema]       # column names the operators above may still reference
+        self.filters: dict = {}                                          # stage index -> its JoinFilter as stage-filter RPN nodes
 
     def virtual_schema(self) -> pa.Schema:
         fields = list(self.source.schema)
@@ -634,12 +635,73 @@ class _Scan:
         return pa.schema(fields)
 
 
-def _as_scan(plan: ExecutionPlan) -> Optional[_Scan]:
-    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner, one key, fusable build)]* over a source"""
+_FILTER_NODES = 128   # the node pool of a pipeline's stage filters (dfgpu_pipeline_set_stage_filter)
+
+
+def _can_raise(e: Expr, schema: pa.Schema) -> bool:
+    """CAST, integer ÷ / %, or Decimal128 arithmetic anywhere in e"""
+    if isinstance(e, CastExpr):
+        return True
+    if isinstance(e, BinaryExpr):
+        if e.op in (D.OP_DIVIDE, D.OP_MODULO) and not pa.types.is_floating(e.data_type(schema)):
+            return True
+        if e.op in (D.OP_PLUS, D.OP_MINUS, D.OP_MULTIPLY, D.OP_DIVIDE, D.OP_MODULO) and pa.types.is_decimal128(e.data_type(schema)):
+            return True
+        return _can_raise(e.left, schema) or _can_raise(e.right, schema)
+    if isinstance(e, UnaryExpr):
+        return _can_raise(e.arg, schema)
+    return False
+
+
+def _has_fallible_rhs(e: Expr, schema: pa.Schema) -> bool:
+    """an AND / OR whose right operand can raise: its short-circuit is decided per batch on the host, which cannot see payload fields"""
+    if isinstance(e, BinaryExpr):
+        if e.op in (D.OP_AND, D.OP_OR) and _can_raise(e.right, schema):
+            return True
+        return _has_fallible_rhs(e.left, schema) or _has_fallible_rhs(e.right, schema)
+    if isinstance(e, (UnaryExpr, CastExpr)):
+        return _has_fallible_rhs(e.arg, schema)
+    return False
+
+
+def _stage_filter(sc: _Scan, join: GpuHashJoinExec, kind: int, payload: List[str]) -> Optional[list]:
+    """The join's JoinFilter as the RPN program of the stage it becomes (appended next to sc.stages), or None when it cannot run there.
+    Its columns: a probe-side column -> that column of the probe chain's virtual schema, the build key -> the probe key, any other build
+    column -> the stage's payload field (`payload`, in order; a SEMI / ANTI stage's fields are seen by its filter only)."""
+    f = join.filter
+    vs = sc.virtual_schema()
+    fields = list(vs) + [join.left.schema.field(n) for n in payload]
+    bkey, pkey = join.on[0]
+    where = []
+    for side, ix in f.column_indices:
+        if side == "left":
+            name = join.left.schema.field(ix).name
+            at = vs.get_field_index(pkey) if name == bkey else (len(vs) + payload.index(name) if name in payload else -1)
+        else:
+            at = vs.get_field_index(join.right.schema.field(ix).name)   # -1 when missing or ambiguous
+        if at < 0:
+            return None
+        where.append(at)
+    inter = pa.schema([pa.field(f"f{i}", fields[at].type, fields[at].nullable) for i, at in enumerate(where)])
+    try:
+        if f.expression.data_type(inter) != pa.bool_() or _has_fallible_rhs(f.expression, inter):
+            return None
+        nodes: list = []
+        f.expression.rpn(inter, nodes)
+    except KeyError:
+        return None
+    if len(nodes) + sum(len(n) for n in sc.filters.values()) > _FILTER_NODES:
+        return None
+    return [(k, where[a], *rest) if k == D.EXPR_COLUMN else (k, a, *rest) for k, a, *rest in nodes]
+
+
+def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]:
+    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner, one key, fusable build)]* over a source.
+    join_filters: a join may carry a JoinFilter, which becomes its stage's filter (fuse_join_filters)"""
     if isinstance(plan, GpuProjectionExec):
         if not all(isinstance(e, Column) and e.name == name for e, name in plan.exprs):
             return None
-        sc = _as_scan(plan.input)
+        sc = _as_scan(plan.input, join_filters)
         if sc is not None:
             sc.visible = [name for _, name in plan.exprs]
         return sc
@@ -654,16 +716,27 @@ def _as_scan(plan: ExecutionPlan) -> Optional[_Scan]:
             sc.visible = [inner.schema.field(i).name for i in plan.projection]
         return sc
     if isinstance(plan, GpuHashJoinExec):
-        if plan.join_type not in ("RightSemi", "RightAnti", "Inner") or len(plan.on) != 1 or plan.filter is not None or plan.null_aware or plan.null_equality != "NullEqualsNothing":
+        if plan.join_type not in ("RightSemi", "RightAnti", "Inner") or len(plan.on) != 1 or (plan.filter is not None and not join_filters) or \
+                plan.null_aware or plan.null_equality != "NullEqualsNothing":
             return None
-        sc = _as_scan(plan.right)
+        sc = _as_scan(plan.right, join_filters)
         if sc is None or plan.on[0][1] not in [f.name for f in sc.source.schema]:
             return None
         kind = {"RightSemi": D.STAGE_SEMI, "RightAnti": D.STAGE_ANTI, "Inner": D.STAGE_INNER}[plan.join_type]
         payload = [f.name for f in plan.left.schema if f.name != plan.on[0][0]] if kind == D.STAGE_INNER else []
-        build = _as_build(plan.left, plan.on[0][0], payload)
+        if plan.filter is not None and kind != D.STAGE_INNER:   # a semi / anti lookup carries the build columns its filter reads
+            read = {plan.left.schema.field(ix).name for sd, ix in plan.filter.column_indices if sd == "left"}
+            payload = [f.name for f in plan.left.schema if f.name != plan.on[0][0] and f.name in read]
+        filt = None
+        if plan.filter is not None:
+            filt = _stage_filter(sc, plan, kind, payload)
+            if filt is None:
+                return None
+        build = _as_build(plan.left, plan.on[0][0], payload, join_filters)
         if build is None:
             return None
+        if filt is not None:
+            sc.filters[len(sc.stages)] = filt
         sc.stages.append((kind, plan.on[0][1], build))
         names = [f.name for f in plan.schema]
         sc.visible = names
@@ -673,8 +746,8 @@ def _as_scan(plan: ExecutionPlan) -> Optional[_Scan]:
     return _Scan(plan)
 
 
-def _as_build(plan: ExecutionPlan, key: str, payload: List[str]) -> Optional["GpuPipelineExec"]:
-    sc = _as_scan(plan)
+def _as_build(plan: ExecutionPlan, key: str, payload: List[str], join_filters: bool = False) -> Optional["GpuPipelineExec"]:
+    sc = _as_scan(plan, join_filters)
     if sc is None or len(sc.stages) >= 3:
         return None
     vs = sc.virtual_schema()
@@ -741,7 +814,16 @@ class GpuPipelineExec(ExecutionPlan):
             look = build.build_lookup(ctx)                      # the pipeline breaker: WaitBuildSide (hash_join/stream.rs:117-140)
             keep.append(look)
             stages.append((kind, ssch.get_field_index(pkey), look))
-        return D.Pipeline(ctx.gpu, [type_id(f.type) for f in ssch], nodes, stages), keep
+        pipe = D.Pipeline(ctx.gpu, [type_id(f.type) for f in ssch], nodes, stages)
+        try:
+            for s, fnodes in sorted(self.scan.filters.items()):
+                pipe.set_stage_filter(s, fnodes)
+        except BaseException:
+            pipe.close()
+            for l in keep:
+                l.close()
+            raise
+        return pipe, keep
 
     def execute(self, ctx):
         assert self.sink in ("aggregate", "dense", "hash"), "build pipelines are driven by their consumer"
@@ -871,7 +953,7 @@ def _acc_words(funcs: Sequence[str], types: Sequence[Optional[pa.DataType]], has
     return n
 
 
-def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
+def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a): AggregateExec(Single / SinglePartitioned / Partial) over [ProjectionExec] over
     HashJoinExec(Inner) whose GROUP BY is the probe key plus build-side columns becomes ONE GpuPipelineExec; its build side (filters, semi
     joins, column projections) becomes build pipelines.  The same AggregateExec over [ProjectionExec] over FilterExec over a source, with
@@ -879,9 +961,10 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     Left joins (the build side kept): the same AggregateExec over HashJoinExec(Left) grouped on the build key plus build columns
     (_fuse_left: TPC-H Q13), and a top-level HashJoinExec(LeftSemi / LeftAnti) (_fuse_left_filter: Q18, Q20, Q22) become a GpuPipelineExec
     with the join-keyed sink.  Their rows come out in slot order: the reference does not keep the build side's order either
-    (maintains_input_order is false for it).  Anything else is returned unchanged (the unfused Gpu*Exec operators run)."""
+    (maintains_input_order is false for it).  Anything else is returned unchanged (the unfused Gpu*Exec operators run).
+    join_filters: joins with a JoinFilter fuse too (fuse_join_filters)."""
     if isinstance(plan, GpuHashJoinExec) and plan.join_type in ("LeftSemi", "LeftAnti"):
-        fused = _fuse_left_filter(plan)
+        fused = _fuse_left_filter(plan, join_filters)
         return plan if fused is None else fused
     if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial"):
         return plan
@@ -894,11 +977,11 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     if isinstance(below, GpuProjectionExec):
         proj, below = below, below.input
     if isinstance(below, GpuHashJoinExec) and below.join_type == "Left":
-        fused = _fuse_left(plan, below, proj)
+        fused = _fuse_left(plan, below, proj, join_filters)
         return plan if fused is None else fused
     if not isinstance(below, GpuHashJoinExec) or below.join_type != "Inner":
         return plan
-    sc = _as_scan(below)
+    sc = _as_scan(below, join_filters)
     if sc is None or not sc.stages or sc.stages[-1][0] != D.STAGE_INNER:
         return plan
     kind, pkey, build = sc.stages[-1]
@@ -941,33 +1024,42 @@ def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
 
 
-def _left_join_scan(join: GpuHashJoinExec, kind: int) -> Optional[_Scan]:
+def _left_join_scan(join: GpuHashJoinExec, kind: int, join_filters: bool = False) -> Optional[_Scan]:
     """The probe chain of a Left / LeftSemi / LeftAnti join with the join as its last stage (kind), or None.  Conditions: one key, no
     JoinFilter, NullEqualsNothing, not null-aware; the right side is an _as_scan chain probing on one of its source columns; the left side
     is a fusable build whose key field is declared non-nullable (a NULL build key is never in the lookup, but Left / LeftAnti emit its row)
-    and has the probe key's type.  The build's payload is every other left column."""
-    if len(join.on) != 1 or join.filter is not None or join.null_aware or join.null_equality != "NullEqualsNothing":
+    and has the probe key's type.  The build's payload is every other left column.  join_filters: a JoinFilter is allowed and becomes the
+    stage's filter."""
+    if len(join.on) != 1 or (join.filter is not None and not join_filters) or join.null_aware or join.null_equality != "NullEqualsNothing":
         return None
     bkey, pkey = join.on[0]
-    sc = _as_scan(join.right)
+    sc = _as_scan(join.right, join_filters)
     ls = join.left.schema
     if sc is None or len(sc.stages) >= 3 or sc.source.schema.get_field_index(pkey) < 0 or ls.get_field_index(bkey) < 0:
         return None
     kf = ls.field(bkey)
     if kf.nullable or kf.type != sc.source.schema.field(pkey).type:
         return None
-    build = _as_build(join.left, bkey, [f.name for f in ls if f.name != bkey])
+    payload = [f.name for f in ls if f.name != bkey]
+    filt = None
+    if join.filter is not None:
+        filt = _stage_filter(sc, join, kind, payload)
+        if filt is None:
+            return None
+    build = _as_build(join.left, bkey, payload, join_filters)
     if build is None:
         return None
+    if filt is not None:
+        sc.filters[len(sc.stages)] = filt
     sc.stages.append((kind, pkey, build))
     return sc
 
 
-def _fuse_left(plan: "GpuAggregateExec", join: GpuHashJoinExec, proj: Optional[GpuProjectionExec]) -> Optional["GpuPipelineExec"]:
+def _fuse_left(plan: "GpuAggregateExec", join: GpuHashJoinExec, proj: Optional[GpuProjectionExec], join_filters: bool = False) -> Optional["GpuPipelineExec"]:
     """AggregateExec over [ProjectionExec] over HashJoinExec(Left) -> the join-keyed sink over a LEFT stage, or None.  GROUP BY the build
     key (not the probe key: NULL on a padded row) plus build columns; every aggregate COUNT(*) or an argument over right-side columns that
     reads a probe source column and propagates NULL, so that it is NULL on a build row's padded row."""
-    sc = _left_join_scan(join, D.STAGE_LEFT)
+    sc = _left_join_scan(join, D.STAGE_LEFT, join_filters)
     if sc is None:
         return None
     _, pkey, build = sc.stages[-1]
@@ -1016,10 +1108,10 @@ def _fuse_left(plan: "GpuAggregateExec", join: GpuHashJoinExec, proj: Optional[G
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
 
 
-def _fuse_left_filter(join: GpuHashJoinExec) -> Optional["GpuPipelineExec"]:
+def _fuse_left_filter(join: GpuHashJoinExec, join_filters: bool = False) -> Optional["GpuPipelineExec"]:
     """HashJoinExec(LeftSemi / LeftAnti) -> the join-keyed sink without aggregates, grouped on every left column, or None.  LeftSemi is an
     INNER stage over the unique build keys (the records a probe row reached), LeftAnti a LEFT_ANTI stage (the records none reached)."""
-    sc = _left_join_scan(join, D.STAGE_INNER if join.join_type == "LeftSemi" else D.STAGE_LEFT_ANTI)
+    sc = _left_join_scan(join, D.STAGE_INNER if join.join_type == "LeftSemi" else D.STAGE_LEFT_ANTI, join_filters)
     if sc is None:
         return None
     _, pkey, build = sc.stages[-1]
@@ -1031,14 +1123,15 @@ def _fuse_left_filter(join: GpuHashJoinExec) -> Optional["GpuPipelineExec"]:
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, mode="Single", out_schema=join.schema, project=project)
 
 
-def fuse_hash_aggregates(plan: ExecutionPlan) -> ExecutionPlan:
+def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_pipelines: its result when that rule fuses; otherwise an
     AggregateExec(Single / SinglePartitioned / Partial) with at least one GROUP BY column over [ProjectionExec] over an Inner join chain or a
     FilterExec (as _as_scan accepts them) becomes ONE GpuPipelineExec with the hash-keyed sink (dfgpu_pipeline_sink_aggregate_hash: TPC-H
     Q15's revenue0, Q3 grouped by o_custkey).  Every group key must be a plain integer-like column of the virtual schema, the packed key
     (each column at its width, one more bit per nullable column) at most 128 bits; no FILTER clause, at most 4 aggregates, and the argument
-    types the library accepts.  Anything else, a bare scan included, is returned unchanged (dfgpu_agg runs)."""
-    fused = fuse_pipelines(plan)
+    types the library accepts.  Anything else, a bare scan included, is returned unchanged (dfgpu_agg runs).  join_filters: joins with a
+    JoinFilter fuse too (fuse_join_filters)."""
+    fused = fuse_pipelines(plan, join_filters)
     if fused is not plan:
         return fused
     if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial") or not plan.group_by:
@@ -1048,7 +1141,7 @@ def fuse_hash_aggregates(plan: ExecutionPlan) -> ExecutionPlan:
         proj, below = below, below.input
     if not ((isinstance(below, GpuHashJoinExec) and below.join_type == "Inner") or isinstance(below, GpuFilterExec)):
         return plan
-    sc = _as_scan(below)
+    sc = _as_scan(below, join_filters)
     if sc is None:
         return plan
     vs = sc.virtual_schema()
@@ -1087,6 +1180,19 @@ def fuse_hash_aggregates(plan: ExecutionPlan) -> ExecutionPlan:
                 return plan
         aggs.append((a.func, e, a.alias))
     return GpuPipelineExec(sc, sink="hash", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, nullable=nullable)
+
+
+def fuse_join_filters(plan: ExecutionPlan) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_hash_aggregates: its result when that rule fuses; otherwise the same
+    shapes again with JoinFilters allowed on the Inner / RightSemi / RightAnti joins of a probe chain and on a Left / LeftSemi / LeftAnti
+    join that is the last stage.  Each filter becomes its stage's filter (dfgpu_pipeline_set_stage_filter): a probe-side column maps to
+    the probe chain's column, the build key to the probe key, other build columns to the stage's payload fields (a RightSemi /
+    RightAnti build carries exactly the columns its filter reads).  A plan is left unchanged when a payload would exceed 64 bits, the
+    filters 128 nodes, or an AND / OR has a right operand that can raise (÷, %, CAST, Decimal128 arithmetic)."""
+    fused = fuse_hash_aggregates(plan)
+    if fused is not plan:
+        return fused
+    return fuse_hash_aggregates(plan, join_filters=True)
 
 
 def collect(plan: ExecutionPlan, ctx: Optional[TaskContext] = None) -> List[pa.RecordBatch]:

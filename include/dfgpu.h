@@ -549,6 +549,25 @@ int dfgpu_pipeline_sink_output(dfgpu_pipeline* p, const int32_t* out_cols, int32
 /* the same, row order unspecified (what a RepartitionExec consumer sees anyway, repartition/mod.rs:1320-1400): runs on the two-phase
  * kernel and is several times faster than the ordered sink on selective pipelines */
 int dfgpu_pipeline_sink_output_unordered(dfgpu_pipeline* p, const int32_t* out_cols, int32_t n_out, int64_t batch_size);
+/* JoinFilter of probe stage `stage` (joins/utils.rs:1248-1320 apply_join_filter_to_indices; hash_join/stream.rs:896-906): a Boolean RPN
+ * program evaluated on each probe row whose key matched at that stage (a candidate pair).  NULL or false means the pair does not match:
+ *   INNER (Inner; LeftSemi as an INNER stage under the join-keyed sink), SEMI: the row continues when its key matches and the filter is TRUE;
+ *   ANTI: the row continues unless its key matches and the filter is TRUE;
+ *   LEFT: a record's row counter and accumulators take only the rows with filter TRUE; a build row no such row reached is the NULL-padded row;
+ *   LEFT_ANTI: emits the records that no row with filter TRUE reached;
+ *   MAYBE: DFGPU_ERR_UNSUPPORTED (a membership pre-filter has no candidate row to test).
+ * Columns of stage s's filter: the input columns, then the payload fields of the INNER / LEFT / LEFT_ANTI stages 0..s in virtual-column
+ * order, then, for a SEMI / ANTI stage only, that stage's own payload fields (seen by its filter only, not by later stages or sinks).
+ * A lookup with payload has unique keys; a filter that reads no payload field also works over key sets and bitmaps with duplicates.
+ * An error inside the filter (÷ 0, % 0, a failing CAST, Decimal128 overflow) is raised only on candidate pairs: a row without a key match,
+ * or one an earlier stage dropped, never raises.  NULL probe keys never match.
+ * Call after dfgpu_pipeline_create and before the first push; a call after the first push or a second one for the same stage is
+ * DFGPU_ERR_STATE.  DFGPU_ERR_INVALID: a result that is not Boolean, a column index out of range (a later stage's payload field
+ * included).  DFGPU_ERR_UNSUPPORTED: a MAYBE stage; an AND / OR whose right operand can raise (÷, %, CAST, Decimal128 arithmetic:
+ * the per-batch short-circuit cannot be decided for payload fields; comparisons, wrapping integer + - *, Kleene AND / OR / NOT and
+ * IS [NOT] NULL are accepted anywhere); more than 128 nodes over all filters of the pipeline.  A pipeline with a stage filter runs
+ * neither the ring-fed nor the partitioned aggregate pass ("ring_launches" and "partitioned_launches" stay 0). */
+int dfgpu_pipeline_set_stage_filter(dfgpu_pipeline* p, int32_t stage, const dfgpu_expr_node* expr, int32_t n_nodes);
 /* optional label: this pipeline's kernel is timed under the family "pipe:<name>" (dfgpu_set_kernel_timing / dfgpu_kernel_time) —
  * the per-operator metrics set of a plan node (metrics(), execution_plan.rs:713) */
 int dfgpu_pipeline_set_name(dfgpu_pipeline* p, const char* name);
