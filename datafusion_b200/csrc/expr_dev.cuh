@@ -184,6 +184,12 @@ __device__ __forceinline__ void eval_binary(const ENode& nd, uint64_t a, bool av
 __device__ __forceinline__ uint64_t cast_value(uint64_t v, int from, int to, bool valid, int* err) {
   int cf = cls_of_prim(from), ct = cls_of_prim(to);
   if (ct == C_F64) {
+    // an integer -> Float32 cast is Rust's `as f32` (arrow-cast's numeric cast): one rounding, straight from the integer.  Through a
+    // double it would round twice: Int64 2^60 + 2^36 + 1 would give 0x5d800000 instead of 0x5d800001.
+    if (to == DFGPU_FLOAT32 && cf != C_F64) {
+      const float f = cf == C_I64 ? __ll2float_rn((long long)v) : __ull2float_rn(v);
+      return (uint64_t)__double_as_longlong((double)f);
+    }
     double d = cf == C_F64 ? __longlong_as_double((long long)v) : (cf == C_U64 || cf == C_BOOL ? (double)v : (double)(long long)v);
     if (to == DFGPU_FLOAT32) d = (double)(float)d;
     return (uint64_t)__double_as_longlong(d);

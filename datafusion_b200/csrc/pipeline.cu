@@ -1376,7 +1376,14 @@ __global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipePar
       }
     } else if (sp.pred_mode == 2) {
       bool ok;
-      const uint64_t val = eval_nodes(sp.pool + sp.pred_start, sp.pred_n, row, &ok, &err);
+      uint64_t val;
+      if (sp.pred_small == 3) {   // Decimal128 nodes: the 128-bit interpreter, as in pipe_kernel's DEC instantiations
+        int eo[2] = {0, 0};
+        val = pipe_eval<true>(sp.pool + sp.pred_start, sp.pred_n, 3, row, nullptr, eo);
+        err |= eo[0]; ok = eo[1] != 0;
+      } else {
+        val = eval_nodes(sp.pool + sp.pred_start, sp.pred_n, row, &ok, &err);
+      }
       alive[k] = ok && (val & 1);
     }
   }

@@ -733,10 +733,15 @@ def _eval_flat(cols: Sequence[Col], nodes: Sequence[tuple]) -> Col:
                             if np.any(act & (rv == 0)):
                                 raise ArrowDivideByZero("Divide by zero error")
                             safe = np.where(rv == 0, 1, rv)
-                            if dtp.kind == "i":  # truncating division like Rust
-                                q = (np.abs(lv.astype(np.int64)) // np.abs(safe.astype(np.int64))) * np.sign(lv.astype(np.int64)) * np.sign(safe.astype(np.int64))
-                                r = q if a == OP_DIVIDE else lv.astype(np.int64) - q * safe.astype(np.int64)
-                                r = r.astype(dtp)
+                            if dtp.kind == "i":
+                                # Rust's truncating `/` and `%` on exact Python ints: MIN / -1 does not fit the type, and arrow's checked `div`
+                                # reports ArithmeticOverflow there; `rem` gives 0 (MIN % -1 == 0)
+                                lo = int(np.iinfo(dtp).min)
+                                if a == OP_DIVIDE and np.any(act & (lv == lo) & (rv == -1)):
+                                    raise ArrowArithmeticOverflow("Arithmetic overflow")
+                                q = [_tdiv(x, y) for x, y in zip(lv.tolist(), safe.tolist())]
+                                r = [qq if qq != -lo else 0 for qq in q] if a == OP_DIVIDE else [x - qq * y for x, y, qq in zip(lv.tolist(), safe.tolist(), q)]
+                                r = np.array(r, np.int64).astype(dtp)
                             else:
                                 r = (lv // safe) if a == OP_DIVIDE else (lv % safe)
                         elif a == OP_PLUS: r = lv + rv   # numpy integer arrays wrap
