@@ -815,7 +815,9 @@ class Lookup:
 
 
 class Pipeline(_Operator):
-    """dfgpu_pipeline: predicate -> probe stage(s) -> sink, one pass.  stages: [(kind, key_col, Lookup)]"""
+    """dfgpu_pipeline: predicate -> probe stage(s) -> sink, one pass.  stages: [(kind, key_col, Lookup)]
+    metric(): the names dfgpu.h lists at dfgpu_pipeline_metric, e.g. "partitioned_records", the {key, value} records the partitioned
+    aggregate's first pass wrote (the rows that passed the folded membership filter and fit the record buffer)"""
     _next_fn, _destroy_fn, _metric_fn = "dfgpu_pipeline_next", "dfgpu_pipeline_destroy", "dfgpu_pipeline_metric"
 
     def __init__(self, ctx, input_types, predicate=None, stages=(), name=None):

@@ -1560,6 +1560,16 @@ __global__ void __launch_bounds__(256) lookup_filter_records_kernel(LookupDev t,
     if (key != kEmptyKey) filter_set(t, key);
   }
 }
+// the membership filter folded to half its blocks: out[i] = in[2i] | in[2i+1].  bloom_pos places a key by fastrange, block =
+// umulhi(h1, blocks) = floor(h1 * blocks / 2^32), and its bit positions t do not depend on `blocks`.  For blocks = 2b,
+// umulhi(h1, 2b) >> 1 = floor(floor(h1 * b / 2^31) / 2) = floor(h1 * b / 2^32) = umulhi(h1, b): a key of exact block k lands in folded
+// block k >> 1, which holds k's bits, so probing `out` with b blocks has no false negatives for any key of the exact filter.
+__global__ void __launch_bounds__(256) bloom_fold_kernel(const ulonglong2* __restrict__ in, unsigned long long* __restrict__ out, uint64_t half) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < half; i += (uint64_t)gridDim.x * blockDim.x) {
+    const ulonglong2 v = in[i];
+    out[i] = v.x | v.y;
+  }
+}
 // accumulator identities for MIN / MAX (SUM / COUNT start at the zero the table was initialised with)
 __global__ void __launch_bounds__(256) lookup_init_acc_kernel(LookupDev t, int word, unsigned long long value) {
   for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < t.cap; s += (uint64_t)gridDim.x * blockDim.x) t.recs[s * (uint64_t)t.stride + word] = value;
@@ -1792,7 +1802,7 @@ struct dfgpu_pipeline {
   DevBuf params_dev, counters;
   std::deque<BatchPtr> outq;
   int64_t m_input_rows = 0, m_sink_rows = 0, m_output_rows = 0, m_groups = 0, m_ring_launches = 0, m_dense_block_launches = 0, m_partitioned_launches = 0,
-          m_partitioned_inserts = 0;
+          m_partitioned_inserts = 0, m_partitioned_records = 0;
   std::string name;   // optional label: the kernel-timing family becomes "pipe:<name>" (dfgpu_kernel_time)
 };
 
@@ -1829,7 +1839,8 @@ static void lookup_reserve(dfgpu_lookup* l, int64_t rows) {
   uint64_t nblocks = 0;
   const size_t table_bytes = (size_t)new_cap * l->stride * 8;
   if (l->opt.membership_filter == 1 || (l->opt.membership_filter < 0 && table_bytes > kL2TableBytes)) {
-    nblocks = std::max<uint64_t>(1024, new_cap / 8);   // 16 bits per key at load factor 0.5
+    // 16 bits per key at load factor 0.5; an even count lets the partitioned aggregate fold the filter to half size (bloom_fold_kernel)
+    nblocks = (std::max<uint64_t>(1024, new_cap / 8) + 1) & ~1ull;
     nbloom.alloc(ctx, (size_t)nblocks * 8);
     nbloom.zero();
   }
@@ -2514,7 +2525,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     // record buffer's capacity
     const int force_parts = getenv("DFGPU_PIPE_RADIX_PARTS") ? atoi(getenv("DFGPU_PIPE_RADIX_PARTS")) : 0;
     const size_t part_bytes = partitioned_table_bytes(p, pp, force_parts);
-    DevBuf rkeys, rvals, recs, meta;   // released after read_counters' synchronise
+    DevBuf rkeys, rvals, recs, meta, folded;   // released after read_counters' synchronise
     if (part_bytes) {
       // survivors are a fraction of the rows (Q3: ~5 %); the buffer holds one in eight, rows past it take the in-kernel fallback
       int64_t cap = std::min<int64_t>(n, std::max<int64_t>(n / 8, 1 << 20));
@@ -2522,6 +2533,22 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
       cap = std::max<int64_t>(cap, 1);
       rkeys.alloc(ctx, (size_t)cap * 8); rvals.alloc(ctx, (size_t)cap * 8);
       pp.out_dst[0] = rkeys.ptr; pp.out_dst[1] = rvals.ptr; pp.out_counter = p->counters.as<unsigned long long>() + 4; pp.target.cap = (uint64_t)cap;
+      // Pass 1 tests the filter once per date-qualified row, a random 8-byte load each.  At 16 bits per key the filter (Q3 SF100:
+      // 29 MB) does not stay in L2 beside the stream; folded once to 8 bits per key it does, and a false positive here costs only a
+      // record that finds nothing in an L2-resident probe.  The lookup keeps the exact filter for the direct probe, where a false
+      // positive costs a DRAM access.  Folding twice (4 bits per key, ~18 % false positives) would overflow Q3 SF100's record buffer.
+      LookupDev& lk = pp.stage[pp.agg_stage].lk;
+      if (lk.bloom) {
+        DF_CHECK(lk.bloom_blocks % 2 == 0 && !lk.coarse, DFGPU_ERR_INVALID, "internal: the partitioned aggregate folds an even-sized exact filter");
+        const uint64_t half = lk.bloom_blocks / 2;
+        folded.alloc(ctx, (size_t)half * 8);
+        {
+          KernelTimer kt(ctx, "pipe_filter_fold");
+          bloom_fold_kernel<<<grid_for((int64_t)half, 256, kNumSMs * 8), 256, 0, ctx->stream>>>((const ulonglong2*)lk.bloom, folded.as<unsigned long long>(), half);
+          DF_LAUNCH_CHECK(ctx);
+        }
+        lk.bloom = folded.as<unsigned long long>(); lk.bloom_blocks = half;
+      }
     }
     upload_params(p, pp);
     p->counters.zero();
@@ -2532,6 +2559,7 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
       DF_CUDA(cudaStreamSynchronize(ctx->stream));
       check_errors(h8[3]);
       const int64_t m = std::min<int64_t>((int64_t)h8[4], (int64_t)pp.target.cap);
+      p->m_partitioned_records += m;
       if (m > 0) {
         recs.alloc(ctx, (size_t)m * 16); meta.alloc(ctx, (size_t)(kRadixMetaWords + 1) * 8);
         meta.zero();
@@ -3417,6 +3445,7 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name) {
   if (s == "dense_block_launches") return p->m_dense_block_launches;   // dense sink launches with one accumulator copy per block (shared atomics)
   if (s == "partitioned_launches") return p->m_partitioned_launches;   // aggregate sink pushes probed from radix-partitioned records
   if (s == "partitioned_inserts") return p->m_partitioned_inserts;     // build sink pushes inserted from radix-partitioned records
+  if (s == "partitioned_records") return p->m_partitioned_records;     // {key, value} records the partitioned aggregate's pass 1 wrote
   if (s == "group_rehashes") return p->m_group_rehashes;               // hash aggregate sink: times its group table grew
   if (s == "replayed_rows") return p->m_replayed_rows;                 // hash aggregate sink: rows deferred by the claim budget and pushed again
   return -1;

@@ -580,7 +580,11 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_ro
                                                                       "group_rehashes","replayed_rows",
                                                                       "partitioned_inserts": build sink pushes whose records went into a
                                                                       table larger than 40 MB (more than L2 holds) radix-partitioned by
-                                                                      slot range, one L2-sized range at a time */
+                                                                      slot range, one L2-sized range at a time,
+                                                                      "partitioned_records": {key, value} records the partitioned
+                                                                      aggregate's first pass wrote (rows that passed the join key's
+                                                                      membership filter, folded to 8 bits per key, and fit the record
+                                                                      buffer) */
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p);
 
 /* ===================================================================================== */
