@@ -159,7 +159,7 @@ EXPORTS = [
     "dfgpu_batch_num_rows", "dfgpu_batch_num_columns", "dfgpu_batch_column", "dfgpu_batch_is_host",
     "dfgpu_batch_export_arrow", "dfgpu_batch_release", "dfgpu_hash_partition_device",
     "dfgpu_partition_plan_create", "dfgpu_partition_plan_scatter_peer", "dfgpu_partition_plan_create_chunked",
-    "dfgpu_partition_plan_scatter_peer_chunk", "dfgpu_partition_plan_destroy",
+    "dfgpu_partition_plan_scatter_peer_chunk", "dfgpu_partition_plan_scatter_peer_chunk_nullable", "dfgpu_partition_plan_destroy",
     "dfgpu_ipc_export", "dfgpu_ipc_import", "dfgpu_ipc_close",
     "dfgpu_comm_unique_id", "dfgpu_comm_init", "dfgpu_comm_rank", "dfgpu_comm_size", "dfgpu_comm_barrier", "dfgpu_comm_allgather_i64", "dfgpu_comm_share",
     "dfgpu_comm_destroy", "dfgpu_exchange_create", "dfgpu_exchange_run", "dfgpu_exchange_columns", "dfgpu_exchange_destroy",
@@ -255,6 +255,7 @@ def load_library() -> C.CDLL:
     sig("dfgpu_partition_plan_scatter_peer", C.c_int, [vp, P(vp), P(i64)])
     sig("dfgpu_partition_plan_create_chunked", C.c_int, [vp, P(Column), i32, P(i32), i32, i32, i32, P(i64), P(vp)])
     sig("dfgpu_partition_plan_scatter_peer_chunk", C.c_int, [vp, i32, P(vp), P(i64)])
+    sig("dfgpu_partition_plan_scatter_peer_chunk_nullable", C.c_int, [vp, i32, P(vp), P(vp), P(i64)])
     sig("dfgpu_partition_plan_destroy", None, [vp])
     sig("dfgpu_ipc_export", C.c_int, [vp, vp, C.c_char_p])
     sig("dfgpu_ipc_import", C.c_int, [vp, C.c_char_p, P(vp)])

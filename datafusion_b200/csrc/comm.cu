@@ -48,8 +48,9 @@ struct dfgpu_exchange {
   dfgpu_comm* comm = nullptr;
   std::vector<int> types;
   int64_t cap = 0, recv_rows = 0;
-  std::vector<DevBuf> bufs;                       // this rank's receive buffers, one per column
-  std::vector<std::vector<void*>> peer;           // [rank][col]
+  std::vector<DevBuf> bufs, vbufs;                // this rank's receive buffers and receive validity bitmaps, one per column
+  std::vector<std::vector<void*>> peer, peer_valid;   // [rank][col]
+  std::vector<bool> recv_valid;                   // per column: the last run's rows carry a validity bitmap (some sender had one)
 };
 
 namespace dfgpu {
@@ -192,20 +193,25 @@ int dfgpu_exchange_create(dfgpu_comm* c, const int32_t* col_types, int32_t n_col
   x->comm = c; x->cap = cap_rows;
   x->types.assign(col_types, col_types + n_cols);
   x->peer.assign(c->n_ranks, std::vector<void*>(n_cols, nullptr));
+  x->peer_valid = x->peer;
+  x->recv_valid.assign(n_cols, false);
   for (int i = 0; i < n_cols; ++i) {
     const int w = type_width(col_types[i]);
-    DF_CHECK(w >= 1 && w <= 8, DFGPU_ERR_UNSUPPORTED, "exchange: fixed-width columns of <= 8 bytes");
-    x->bufs.emplace_back(ctx, (size_t)cap_rows * w);
-    std::vector<void*> ptrs(c->n_ranks);
+    DF_CHECK(col_types[i] == DFGPU_BOOL || (w >= 1 && w <= 16), DFGPU_ERR_UNSUPPORTED, "exchange: Boolean or fixed-width columns of <= 16 bytes");
+    // a Boolean column's receive buffer is a bitmap; bitmaps are whole 64-bit words (the scatter writes 32-bit words)
+    x->bufs.emplace_back(ctx, col_types[i] == DFGPU_BOOL ? bitmap_alloc_bytes(cap_rows) : (size_t)cap_rows * w);
+    x->vbufs.emplace_back(ctx, bitmap_alloc_bytes(cap_rows));
+    std::vector<void*> ptrs(c->n_ranks), vptrs(c->n_ranks);
     int rc = dfgpu_comm_share(c, x->bufs.back().ptr, ptrs.data());
+    if (rc == DFGPU_OK) rc = dfgpu_comm_share(c, x->vbufs.back().ptr, vptrs.data());
     if (rc != DFGPU_OK) throw Error(rc, ctx->last_error);
-    for (int r = 0; r < c->n_ranks; ++r) x->peer[r][i] = ptrs[r];
+    for (int r = 0; r < c->n_ranks; ++r) { x->peer[r][i] = ptrs[r]; x->peer_valid[r][i] = vptrs[r]; }
   }
   *out = x.release();
   DF_API_END
 }
 
-// cols: this rank's device-resident rows (no NULLs); rows travel to rank = exchange_hash(key columns) % n_ranks and arrive grouped by
+// cols: this rank's device-resident rows; rows travel to rank = exchange_hash(key columns) % n_ranks and arrive grouped by
 // source rank, in source order.  Collective: every rank calls it.  On return the received rows are complete in this rank's buffers.
 int dfgpu_exchange_run(dfgpu_exchange* x, const dfgpu_column* cols, int32_t n_cols, const int32_t* key_cols, int32_t n_keys, int64_t* recv_rows_out) {
   DF_API_BEGIN(x ? x->comm->ctx : nullptr)
@@ -214,32 +220,44 @@ int dfgpu_exchange_run(dfgpu_exchange* x, const dfgpu_column* cols, int32_t n_co
   dfgpu_ctx* ctx = c->ctx;
   set_device(ctx);
   const int W = c->n_ranks;
-  for (int i = 0; i < n_cols; ++i) DF_CHECK(cols[i].type == x->types[i] && !(cols[i].validity && cols[i].null_count != 0), DFGPU_ERR_INVALID, "exchange: column type mismatch / nullable column");
-  int64_t counts[kCommMaxRanks] = {0};
+  for (int i = 0; i < n_cols; ++i) DF_CHECK(cols[i].type == x->types[i], DFGPU_ERR_INVALID, "exchange: column type mismatch");
+  // what every rank contributes to the all-gather: its row counts per destination, then per column whether its rows carry a validity bitmap
+  const int G = W + n_cols;
+  int64_t counts[kCommMaxRanks] = {0}, mine[kCommMaxRanks + 16] = {0};
   dfgpu_partition_plan* plan = nullptr;
   int rc = dfgpu_partition_plan_create(ctx, cols, n_cols, key_cols, n_keys, W, counts, &plan);   // histogram on the device; syncs (counts come back)
   if (rc != DFGPU_OK) throw Error(rc, ctx->last_error);
   struct PlanGuard { dfgpu_partition_plan* p; ~PlanGuard() { dfgpu_partition_plan_destroy(p); } } guard{plan};
   // the stream is idle here (the counts were read back): consumers of the previous exchange's rows have finished on this rank, and
   // the all-gather's barrier makes that true for every rank before anybody scatters into anybody's buffers
-  int64_t all[kCommMaxRanks * kCommMaxRanks];
-  rc = dfgpu_comm_allgather_i64(c, counts, W, all);   // all[src][dst]
+  for (int d = 0; d < W; ++d) mine[d] = counts[d];
+  for (int i = 0; i < n_cols; ++i) mine[W + i] = (cols[i].validity && cols[i].null_count != 0) ? 1 : 0;
+  int64_t all[kCommMaxRanks * (kCommMaxRanks + 16)];
+  rc = dfgpu_comm_allgather_i64(c, mine, G, all);   // all[src][dst], all[src][W + col]
   if (rc != DFGPU_OK) throw Error(rc, ctx->last_error);
   int64_t recv = 0, dst_row[kCommMaxRanks];
-  for (int src = 0; src < W; ++src) recv += all[src * W + c->rank];
+  for (int src = 0; src < W; ++src) recv += all[src * G + c->rank];
   for (int dst = 0; dst < W; ++dst) {
     int64_t tot = 0, before = 0;
-    for (int src = 0; src < W; ++src) { if (src < c->rank) before += all[src * W + dst]; tot += all[src * W + dst]; }
+    for (int src = 0; src < W; ++src) { if (src < c->rank) before += all[src * G + dst]; tot += all[src * G + dst]; }
     DF_CHECK(tot <= x->cap, DFGPU_ERR_OOM, "exchange: a receive buffer would overflow (raise cap_rows)");
     dst_row[dst] = before;   // lower ranks' blocks come first
   }
-  std::vector<void*> bases((size_t)W * n_cols);
-  for (int p = 0; p < W; ++p) for (int i = 0; i < n_cols; ++i) bases[(size_t)p * n_cols + i] = x->peer[p][i];
-  rc = dfgpu_partition_plan_scatter_peer(plan, bases.data(), dst_row);
+  // a column arrives with a validity bitmap when any sender has one; senders without write all-ones into their block
+  std::vector<bool> any_valid(n_cols, false);
+  for (int i = 0; i < n_cols; ++i) for (int src = 0; src < W; ++src) if (all[src * G + W + i]) any_valid[i] = true;
+  std::vector<void*> bases((size_t)W * n_cols), vbases((size_t)W * n_cols);
+  for (int p = 0; p < W; ++p)
+    for (int i = 0; i < n_cols; ++i) {
+      bases[(size_t)p * n_cols + i] = x->peer[p][i];
+      vbases[(size_t)p * n_cols + i] = any_valid[i] ? x->peer_valid[p][i] : nullptr;
+    }
+  rc = dfgpu_partition_plan_scatter_peer_chunk_nullable(plan, 0, bases.data(), vbases.data(), dst_row);
   if (rc != DFGPU_OK) throw Error(rc, ctx->last_error);
   rc = dfgpu_comm_barrier(c);   // every rank's scatter kernel has completed: all rows have landed
   if (rc != DFGPU_OK) throw Error(rc, ctx->last_error);
   x->recv_rows = recv;
+  x->recv_valid = any_valid;
   if (recv_rows_out) *recv_rows_out = recv;
   DF_API_END
 }
@@ -248,7 +266,9 @@ int dfgpu_exchange_columns(dfgpu_exchange* x, dfgpu_column* out, int32_t n_cols)
   if (!x || !out || n_cols != (int)x->types.size()) return DFGPU_ERR_INVALID;
   for (int i = 0; i < n_cols; ++i) {
     memset(&out[i], 0, sizeof(dfgpu_column));
-    out[i].type = x->types[i]; out[i].length = x->recv_rows; out[i].values = x->bufs[i].ptr; out[i].validity = nullptr; out[i].null_count = 0;
+    out[i].type = x->types[i]; out[i].length = x->recv_rows; out[i].values = x->bufs[i].ptr;
+    out[i].validity = x->recv_valid[i] ? (const uint8_t*)x->vbufs[i].ptr : nullptr;
+    out[i].null_count = x->recv_valid[i] ? -1 : 0;
   }
   return DFGPU_OK;
 }

@@ -191,42 +191,78 @@ def all_gather_columns(ctx: D.Context, cols, dist):
     return ExchangedBatch(ctx, out, types, total, None)
 
 
+def _bitmap_bytes(rows: int) -> int:
+    return (int(rows) + 63) // 64 * 8          # whole 64-bit words: the scatter writes bitmaps in 32-bit words
+
+
+def has_bitmap(arr, n_cols: int) -> List[int]:
+    """per column of a dfgpu_column array: 1 when it carries a validity bitmap that may hold a NULL (pure host logic)"""
+    return [1 if (arr[i].validity and arr[i].null_count != 0) else 0 for i in range(n_cols)]
+
+
 class PeerExchange:
     """Fused partition + exchange over NVLink peer memory (no NCCL payload transfer).
 
-    Every rank owns one persistent receive buffer per column (capacity `cap_rows`), exported once through CUDA IPC;
-    an exchange is: count rows per destination (CUDA) -> all-gather the world x world count matrix (tiny NCCL
-    collective, which also orders this exchange after everybody's previous use of the buffers) -> ONE scatter
+    Every rank owns one persistent receive buffer and one receive validity bitmap per column (capacity `cap_rows`; a
+    Boolean column's buffer is a bitmap too), exported once through CUDA IPC; an exchange is: count rows per destination
+    (CUDA) -> all-gather the world x world count matrix and every rank's per-column "has a validity bitmap" flags (tiny
+    NCCL collective, which also orders this exchange after everybody's previous use of the buffers) -> ONE scatter
     kernel that writes each row directly into its owner's buffer -> a one-element all-reduce as the completion
-    barrier.  Rows arrive grouped by source rank, in source order (same layout as the all-to-all path)."""
+    barrier.  Rows arrive grouped by source rank, in source order (same layout as the all-to-all path).  A column arrives
+    with a validity bitmap when any sender had one (the other senders' rows are marked valid)."""
 
     def __init__(self, ctx: D.Context, dist, col_types: Sequence[int], cap_rows: int):
         import torch
         self.ctx, self.dist, self.types, self.cap = ctx, dist, list(col_types), int(cap_rows)
         self.world, self.rank = dist.get_world_size(), dist.get_rank()
         self.dev = torch.device("cuda", ctx.device)
-        self.bufs = [D.DeviceBuffer(ctx, self.cap * D.WIDTH[t]) for t in self.types]
+        self.bufs = [D.DeviceBuffer(ctx, _bitmap_bytes(self.cap) if t == D.BOOL else self.cap * D.WIDTH[t]) for t in self.types]
+        self.vbufs = [D.DeviceBuffer(ctx, _bitmap_bytes(self.cap)) for _ in self.types]
         import ctypes as C
-        mine = torch.zeros(len(self.types) * 64, dtype=torch.uint8)
-        for i, b in enumerate(self.bufs):
+        shared = self.bufs + self.vbufs
+        mine = torch.zeros(len(shared) * 64, dtype=torch.uint8)
+        for i, b in enumerate(shared):
             h = C.create_string_buffer(64)
             ctx.check(ctx.lib.dfgpu_ipc_export(ctx.h, C.c_void_p(b.ptr), h))
             mine[i * 64:(i + 1) * 64] = torch.frombuffer(bytearray(h.raw), dtype=torch.uint8)
         allh = [torch.zeros_like(mine).to(self.dev) for _ in range(self.world)]
         dist.all_gather(allh, mine.to(self.dev))
-        self.peer_ptrs = []   # [rank][col]
+        nc = len(self.types)
+        self.peer_ptrs, self.peer_valid = [], []   # [rank][col]
         for r in range(self.world):
             ptrs = []
             hb = bytes(allh[r].cpu().numpy().tobytes())
-            for i in range(len(self.types)):
+            for i in range(len(shared)):
                 if r == self.rank:
-                    ptrs.append(self.bufs[i].ptr)
+                    ptrs.append(shared[i].ptr)
                 else:
                     out = C.c_void_p()
                     ctx.check(ctx.lib.dfgpu_ipc_import(ctx.h, hb[i * 64:(i + 1) * 64], C.byref(out)))
                     ptrs.append(out.value)
-            self.peer_ptrs.append(ptrs)
+            self.peer_ptrs.append(ptrs[:nc])
+            self.peer_valid.append(ptrs[nc:])
         self._flag = torch.zeros(1, dtype=torch.int32, device=self.dev)
+
+    def scatter(self, plan, chunk: int, dst_row, recv_valid):
+        """scatter one chunk of a partition plan into the receive buffers; recv_valid[c]: column c keeps a receive bitmap"""
+        import ctypes as C
+        ctx, world, nc = self.ctx, self.world, len(self.types)
+        bases = (C.c_void_p * (world * nc))(*[self.peer_ptrs[p][c] for p in range(world) for c in range(nc)])
+        vbases = (C.c_void_p * (world * nc))(*[self.peer_valid[p][c] if recv_valid[c] else None for p in range(world) for c in range(nc)])
+        rows = (C.c_int64 * world)(*[int(x) for x in dst_row])
+        ctx.check(ctx.lib.dfgpu_partition_plan_scatter_peer_chunk_nullable(plan, int(chunk), bases, vbases, rows))
+
+    def columns(self, start: int, rows: int, recv_valid) -> List[D.Column]:
+        """device views of receive rows [start, start + rows)"""
+        cols = []
+        for i, ty in enumerate(self.types):
+            c = D.Column()
+            c.type, c.flags, c.length, c.offset = ty, 0, int(rows), int(start)
+            c.values = self.bufs[i].ptr
+            c.validity = self.vbufs[i].ptr if recv_valid[i] else None
+            c.null_count = -1 if recv_valid[i] else 0
+            cols.append(c)
+        return cols
 
     def exchange(self, cols, key_cols: Sequence[int]) -> "ExchangedPeerBatch":
         import ctypes as C
@@ -237,16 +273,15 @@ class PeerExchange:
         plan = C.c_void_p()
         ctx.check(ctx.lib.dfgpu_partition_plan_create(ctx.h, arr, nc, D._i32arr(list(key_cols)), len(key_cols), world, counts, C.byref(plan)))
         try:
-            mine = torch.tensor(list(counts), dtype=torch.int64, device=self.dev)
-            allc = torch.empty(world * world, dtype=torch.int64, device=self.dev)
-            self.dist.all_gather_into_tensor(allc, mine)          # [src][dst]; also the "buffers are free again" barrier
-            m = allc.view(world, world).cpu().numpy()
+            mine = torch.tensor(list(counts) + has_bitmap(arr, nc), dtype=torch.int64, device=self.dev)
+            allc = torch.empty(world * (world + nc), dtype=torch.int64, device=self.dev)
+            self.dist.all_gather_into_tensor(allc, mine)          # [src][dst | col]; also the "buffers are free again" barrier
+            g = allc.view(world, world + nc).cpu().numpy()
+            m, recv_valid = g[:, :world], g[:, world:].any(axis=0).tolist()
             recv_rows = int(m[:, self.rank].sum())
             if m.sum(axis=0).max() > self.cap:
                 raise RuntimeError(f"PeerExchange: a receive buffer would overflow ({int(m.sum(axis=0).max())} rows > capacity {self.cap})")
-            dst_row = (C.c_int64 * world)(*[int(m[:self.rank, p].sum()) for p in range(world)])   # my block starts after lower ranks' blocks
-            bases = (C.c_void_p * (world * nc))(*[self.peer_ptrs[p][c] for p in range(world) for c in range(nc)])
-            ctx.check(ctx.lib.dfgpu_partition_plan_scatter_peer(plan, bases, dst_row))
+            self.scatter(plan, 0, [int(m[:self.rank, p].sum()) for p in range(world)], recv_valid)   # my block starts after lower ranks' blocks
             shared_stream = (ctx.lib.dfgpu_ctx_stream(ctx.h) or 0) == torch.cuda.current_stream().cuda_stream
             if not shared_stream:
                 ctx.sync()
@@ -255,21 +290,15 @@ class PeerExchange:
                 torch.cuda.current_stream().synchronize()
         finally:
             ctx.lib.dfgpu_partition_plan_destroy(plan)
-        return ExchangedPeerBatch(self, recv_rows)
+        return ExchangedPeerBatch(self, recv_rows, recv_valid)
 
 
 class ExchangedPeerBatch:
-    def __init__(self, px: PeerExchange, rows: int):
-        self.px, self.rows = px, rows
+    def __init__(self, px: PeerExchange, rows: int, recv_valid):
+        self.px, self.rows, self.recv_valid = px, rows, list(recv_valid)
 
     def columns(self) -> List[D.Column]:
-        cols = []
-        for b, ty in zip(self.px.bufs, self.px.types):
-            c = D.Column()
-            c.type, c.flags, c.length, c.offset, c.null_count = ty, 0, self.rows, 0, 0
-            c.values, c.validity = b.ptr, None
-            cols.append(c)
-        return cols
+        return self.px.columns(0, self.rows, self.recv_valid)
 
 
 def peer_chunk_layout(m, rank: int):
@@ -355,44 +384,35 @@ class PartitionedHashJoin:
         ctx.check(ctx.lib.dfgpu_partition_plan_create_chunked(ctx.h, arr, len(cols), D._i32arr(list(key_cols)), len(key_cols), self.world, n_chunks, counts, C.byref(plan)))
         return plan, np.array(list(counts), dtype=np.int64).reshape(n_chunks, self.world), arr
 
-    def _scatter(self, plan, px, chunk, dst_row):
-        import ctypes as C
-        world, nc = self.world, len(px.types)
-        bases = (C.c_void_p * (world * nc))(*[px.peer_ptrs[p][c] for p in range(world) for c in range(nc)])
-        rows = (C.c_int64 * world)(*[int(x) for x in dst_row])
-        self.ctx_x.check(self.ctx_x.lib.dfgpu_partition_plan_scatter_peer_chunk(plan, chunk, bases, rows))
-
-    @staticmethod
-    def _slice(px, start, rows):
-        cols = []
-        for b, ty in zip(px.bufs, px.types):
-            c = D.Column()
-            c.type, c.flags, c.length, c.offset, c.null_count = ty, 0, int(rows), 0, 0
-            c.values, c.validity = b.ptr + int(start) * D.WIDTH[ty], None
-            cols.append(c)
-        return cols
+    def _gather_counts(self, cnt, flags):
+        """all-gather every rank's [chunks][world] counts and per-column bitmap flags: (m[src][chunk][dst], recv_valid[col])"""
+        torch, world = self.torch, self.world
+        chunks = cnt.shape[0]
+        mine = torch.from_numpy(np.concatenate([cnt.reshape(-1), np.asarray(flags, dtype=np.int64)])).to(self.dev)
+        allc = torch.empty(world * mine.numel(), dtype=torch.int64, device=self.dev)
+        self.dist.all_gather_into_tensor(allc, mine)          # also: every rank has finished reading the previous step's buffers
+        g = allc.view(world, -1).cpu().numpy()
+        return g[:, :chunks * world].reshape(world, chunks, world), g[:, chunks * world:].any(axis=0).tolist()
 
     # -- streaming form: build once, then any number of probe batches (each call is collective) ----------------
     def build(self, build_cols):
         """exchange the build side and build this rank's table (collect_left_input of the partitioned join)"""
-        torch, world = self.torch, self.world
+        torch = self.torch
         assert getattr(self, "_join", None) is None, "PartitionedHashJoin: build() called twice without finish()"
         plan = None
         try:
             with torch.cuda.stream(self.xs):
-                plan, cnt, _ = self._plan(build_cols, self.on_build, 1)
-                allc = torch.empty(world * world, dtype=torch.int64, device=self.dev)
-                self.dist.all_gather_into_tensor(allc, torch.from_numpy(cnt.reshape(-1)).to(self.dev))
-                m = allc.view(world, 1, world).cpu().numpy()
+                plan, cnt, arr = self._plan(build_cols, self.on_build, 1)
+                m, valid = self._gather_counts(cnt, has_bitmap(arr, len(self.build_types)))
                 row, start, rows, mx = peer_chunk_layout(m, self.rank)
                 if mx > self.px_b.cap:
                     raise RuntimeError(f"PartitionedHashJoin: build receive buffer would overflow ({mx} rows > capacity {self.px_b.cap})")
-                self._scatter(plan, self.px_b, 0, row[0])
+                self.px_b.scatter(plan, 0, row[0], valid)
                 self.dist.all_reduce(self._flag)
                 ev = torch.cuda.Event(); ev.record(self.xs)
             self._join = D.HashJoinHandle(self.ctx, self.build_types, self.probe_types, self.on_build, self.on_probe, self.out_side, self.out_index, **self.join_kwargs)
             self.js.wait_event(ev)
-            self._join.push_build_device(self._slice(self.px_b, start[0], rows[0]))
+            self._join.push_build_device(self.px_b.columns(start[0], rows[0], valid))
             self._join.finish_build()
             self.xs.synchronize()
         finally:
@@ -402,27 +422,25 @@ class PartitionedHashJoin:
     def probe(self, probe_cols, n_chunks: int = None, keep_output: bool = True):
         """exchange one probe batch (in n_chunks pieces, scatter of piece c+1 overlapping the probe of piece c) and probe
         it; returns the device output batches.  Host-synchronous: the batch is fully consumed when the call returns."""
-        torch, world = self.torch, self.world
+        torch = self.torch
         C = int(n_chunks or self.n_chunks)
         j = self._join
         plan, outs = None, []
         try:
             with torch.cuda.stream(self.xs):
-                plan, cnt, _ = self._plan(probe_cols, self.on_probe, C)
-                allc = torch.empty(world * C * world, dtype=torch.int64, device=self.dev)
-                self.dist.all_gather_into_tensor(allc, torch.from_numpy(cnt.reshape(-1)).to(self.dev))   # also: the receive buffers are free again
-                m = allc.view(world, C, world).cpu().numpy()
+                plan, cnt, arr = self._plan(probe_cols, self.on_probe, C)
+                m, valid = self._gather_counts(cnt, has_bitmap(arr, len(self.probe_types)))   # also: the receive buffers are free again
                 row, start, rows, mx = peer_chunk_layout(m, self.rank)
                 if mx > self.px_p.cap:
                     raise RuntimeError(f"PartitionedHashJoin: probe receive buffer would overflow ({mx} rows > capacity {self.px_p.cap})")
                 evs = []
                 for c in range(C):
-                    self._scatter(plan, self.px_p, c, row[c])
+                    self.px_p.scatter(plan, c, row[c], valid)
                     self.dist.all_reduce(self._flag)
                     e = torch.cuda.Event(); e.record(self.xs); evs.append(e)
             for c in range(C):
                 self.js.wait_event(evs[c])
-                j.push_probe_device(self._slice(self.px_p, start[c], rows[c]))
+                j.push_probe_device(self.px_p.columns(start[c], rows[c], valid))
                 got = j.drain(host=False)
                 if keep_output:
                     outs += got
@@ -453,37 +471,36 @@ class PartitionedHashJoin:
     def run(self, build_cols, probe_cols, keep_output: bool = True):
         """build_cols / probe_cols: this rank's device-resident input columns (complete before the call).  One fused
         step: both sides' counts travel in ONE collective.  Returns (output_rows, [device batches])."""
-        torch, world, C = self.torch, self.world, self.n_chunks
+        torch, C = self.torch, self.n_chunks
         plans = []
         try:
             with torch.cuda.stream(self.xs):
                 plan_b, cnt_b, keep_b = self._plan(build_cols, self.on_build, 1); plans.append(plan_b)
                 plan_p, cnt_p, keep_p = self._plan(probe_cols, self.on_probe, C); plans.append(plan_p)
-                mine = torch.from_numpy(np.concatenate([cnt_b, cnt_p]).reshape(-1)).to(self.dev)
-                allc = torch.empty(world * (1 + C) * world, dtype=torch.int64, device=self.dev)
-                self.dist.all_gather_into_tensor(allc, mine)       # also: every rank has finished reading the previous step's buffers
-                m = allc.view(world, 1 + C, world).cpu().numpy()
+                nb = len(self.build_types)
+                m, valid = self._gather_counts(np.concatenate([cnt_b, cnt_p]), has_bitmap(keep_b, nb) + has_bitmap(keep_p, len(self.probe_types)))
+                valid_b, valid_p = valid[:nb], valid[nb:]
                 row_b, start_b, rows_b, max_b = peer_chunk_layout(m[:, :1, :], self.rank)
                 row_p, start_p, rows_p, max_p = peer_chunk_layout(m[:, 1:, :], self.rank)
                 if max_b > self.px_b.cap or max_p > self.px_p.cap:
                     raise RuntimeError(f"PartitionedHashJoin: a receive buffer would overflow (build {max_b}/{self.px_b.cap}, probe {max_p}/{self.px_p.cap} rows)")
-                self._scatter(plan_b, self.px_b, 0, row_b[0])
+                self.px_b.scatter(plan_b, 0, row_b[0], valid_b)
                 self.dist.all_reduce(self._flag)                    # completion barrier, ordered on the exchange stream
                 ev_b = torch.cuda.Event(); ev_b.record(self.xs)
                 ev_p = []
                 for c in range(C):
-                    self._scatter(plan_p, self.px_p, c, row_p[c])
+                    self.px_p.scatter(plan_p, c, row_p[c], valid_p)
                     self.dist.all_reduce(self._flag)
                     e = torch.cuda.Event(); e.record(self.xs); ev_p.append(e)
             j = D.HashJoinHandle(self.ctx, self.build_types, self.probe_types, self.on_build, self.on_probe, self.out_side, self.out_index, **self.join_kwargs)
             outs = []
             try:
                 self.js.wait_event(ev_b)
-                j.push_build_device(self._slice(self.px_b, start_b[0], rows_b[0]))
+                j.push_build_device(self.px_b.columns(start_b[0], rows_b[0], valid_b))
                 j.finish_build()
                 for c in range(C):
                     self.js.wait_event(ev_p[c])
-                    j.push_probe_device(self._slice(self.px_p, start_p[c], rows_p[c]))
+                    j.push_probe_device(self.px_p.columns(start_p[c], rows_p[c], valid_p))
                     if keep_output:
                         outs += j.drain(host=False)
                     else:

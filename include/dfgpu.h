@@ -606,7 +606,9 @@ void dfgpu_batch_release(dfgpu_batch* b);
 
 /* Scatter the rows of `cols` (device) into n_parts contiguous regions by
  * partition = exchange_hash(key columns) % n_parts.  Output columns are library-owned device
- * buffers of the same types; part_offsets_host[n_parts+1] receives the region boundaries. */
+ * buffers of the same types, with a validity bitmap wherever the input column had one;
+ * part_offsets_host[n_parts+1] receives the region boundaries.  Keys: 1..4 fixed-width columns
+ * of <= 128 bits each (Decimal128 included); a NULL key leaves the running hash untouched. */
 int dfgpu_hash_partition_device(dfgpu_ctx* ctx, const dfgpu_column* cols, int32_t n_cols,
                                 const int32_t* key_cols, int32_t n_keys, int32_t n_parts,
                                 dfgpu_batch** out, int64_t* part_offsets_host);
@@ -615,7 +617,10 @@ int dfgpu_hash_partition_device(dfgpu_ctx* ctx, const dfgpu_column* cols, int32_
  * buffer of the GPU that owns its partition — no staging copy, no NCCL payload transfer.  Phase 1 counts rows per
  * destination (the caller all-gathers the counts to learn where its block starts in every receiver), phase 2
  * scatters.  dst_bases[p * n_cols + c] points at column c of rank p's receive buffer (mapped with dfgpu_ipc_import;
- * the local pointer for p == own rank); dst_row_offset[p] is the first row this rank owns in that buffer. */
+ * the local pointer for p == own rank); dst_row_offset[p] is the first row this rank owns in that buffer.
+ * Columns: <= 16, fixed-width or Boolean, nullable or not; keys as for dfgpu_hash_partition_device.  A plan with a
+ * nullable (validity bitmap) or Boolean column is scattered with dfgpu_partition_plan_scatter_peer_chunk_nullable
+ * only: the two calls below refuse it with DFGPU_ERR_INVALID rather than drop its bits. */
 typedef struct dfgpu_partition_plan dfgpu_partition_plan;
 int dfgpu_partition_plan_create(dfgpu_ctx* ctx, const dfgpu_column* cols, int32_t n_cols, const int32_t* key_cols, int32_t n_keys,
                                 int32_t n_parts, int64_t* counts_host, dfgpu_partition_plan** out);
@@ -627,6 +632,15 @@ int dfgpu_partition_plan_scatter_peer(dfgpu_partition_plan* plan, void* const* d
 int dfgpu_partition_plan_create_chunked(dfgpu_ctx* ctx, const dfgpu_column* cols, int32_t n_cols, const int32_t* key_cols, int32_t n_keys,
                                         int32_t n_parts, int32_t n_chunks, int64_t* counts_host, dfgpu_partition_plan** out);
 int dfgpu_partition_plan_scatter_peer_chunk(dfgpu_partition_plan* plan, int32_t chunk, void* const* dst_bases, const int64_t* dst_row_offset);
+/* The same with bit-packed data.  dst_validity[p * n_cols + c] is rank p's receive bitmap for column c, or NULL when column c
+ * keeps no bitmap at the receivers (then for every p; a column whose input has NULLs needs one).  dst_validity itself may be
+ * NULL: no column keeps a bitmap.  A source column without a bitmap writes all-ones into its block of a receive bitmap, so
+ * senders may disagree on nullability.  A Boolean column's dst_bases entry is its receive bitmap, addressed in bits like the
+ * validity (row r = bit r).  Bitmap pointers must be 4-byte aligned and readable and writable in whole 32-bit words.  Only
+ * the bits of this rank's block change, with atomic updates (system scope in peer memory) of the words it shares with a
+ * neighbouring block: receive bitmaps need no zeroing, and several ranks may scatter into one bitmap at the same time. */
+int dfgpu_partition_plan_scatter_peer_chunk_nullable(dfgpu_partition_plan* plan, int32_t chunk, void* const* dst_bases, void* const* dst_validity,
+                                                     const int64_t* dst_row_offset);
 void dfgpu_partition_plan_destroy(dfgpu_partition_plan* plan);
 /* CUDA IPC: export a device allocation made with dfgpu_malloc (64-byte handle) / map a peer's allocation */
 int dfgpu_ipc_export(dfgpu_ctx* ctx, void* dev_ptr, uint8_t* handle_out);
@@ -677,11 +691,15 @@ int dfgpu_comm_allgather_i64(dfgpu_comm* c, const int64_t* mine, int32_t n, int6
 int dfgpu_comm_share(dfgpu_comm* c, void* dev_ptr, void** peer_ptrs_out);
 void dfgpu_comm_destroy(dfgpu_comm* c);
 /* RepartitionExec Hash(key columns) across the ranks (repartition/mod.rs:1097-1145): persistent receive buffers of cap_rows rows per
- * column, shared once; one run = histogram -> count all-gather -> fused partition + peer-memory scatter -> barrier.  Rows arrive grouped
- * by source rank, in source order.  All three calls are collective; columns must be free of NULLs. */
+ * column and a receive validity bitmap of cap_rows bits per column, shared once; one run = histogram -> count all-gather (which also
+ * tells every rank which columns some sender holds with a validity bitmap) -> fused partition + peer-memory scatter -> barrier.  Rows
+ * arrive grouped by source rank, in source order.  Column types: fixed-width up to 16 bytes (Decimal128(p, s) included) or Boolean,
+ * nullable or not.  All three calls are collective. */
 int dfgpu_exchange_create(dfgpu_comm* c, const int32_t* col_types, int32_t n_cols, int64_t cap_rows, dfgpu_exchange** out);
 int dfgpu_exchange_run(dfgpu_exchange* x, const dfgpu_column* cols, int32_t n_cols, const int32_t* key_cols, int32_t n_keys, int64_t* recv_rows_out);
-int dfgpu_exchange_columns(dfgpu_exchange* x, dfgpu_column* out, int32_t n_cols);   /* device views of the received rows (valid until the next run) */
+/* device views of the received rows (valid until the next run); a column some sender held with a validity bitmap comes with the
+ * receive bitmap and null_count -1, the others with validity NULL */
+int dfgpu_exchange_columns(dfgpu_exchange* x, dfgpu_column* out, int32_t n_cols);
 void dfgpu_exchange_destroy(dfgpu_exchange* x);
 
 #ifdef __cplusplus
