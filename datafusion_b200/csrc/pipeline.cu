@@ -399,6 +399,8 @@ __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_
 //   bit 8 (256) stage filters (FiltParams; launch_pipe picks it whenever a stage has one, on top of the sink's default bits, never with
 //              bits 6 / 7): phase B evaluates a stage's JoinFilter on the rows whose key matched there, and a row that fails counts as
 //              not matched; a filtered bitmap ANTI stage is decided in phase B instead of phase A.
+//   bit 9 (512) output columns with validity bitmaps or 16 bytes wide, unordered output sink only (OutValid; pipeline_push picks it when a
+//              column of the push needs it, on top of the sink's default or filtered bits).
 // DFGPU_PIPE_VAR selects the instantiation (aggregate sink; bits 1 and 5 also for the pack sink, bit 1 for the unordered-output sink); 0 is the
 // kernel without any of them, 11 the default.  Tried and removed: four instead of two survivors per lane and phase-B round; prefetching the
 // table record and the argument sectors already when a row passes the membership filter in phase A (the prefetches of five tiles queue up
@@ -471,6 +473,26 @@ struct FiltParams {
   ENode pool[kFiltPoolNodes];
 };
 constexpr int kFiltParamsOff = kDenseParamsOff + (int)(((sizeof(DenseParams) > sizeof(HashParams) ? sizeof(DenseParams) : sizeof(HashParams)) + 15) / 16 * 16);
+
+// ------------------------------------------------------------------------------------------
+// output columns with validity bitmaps or 16 bytes wide (pipe_kernel VAR bit 512 on the unordered output sink, pipe_output_cols_kernel on
+// the ordered one): the output bitmaps, zeroed before the launch, sit in the sink's block behind PipeParams (where DenseParams / HashParams
+// sit for their sinks), so PipeParams, OutCols and every instantiation without them are unchanged.  An output column has a bitmap exactly
+// when its input column has one in this push; payload fields never do.
+// ------------------------------------------------------------------------------------------
+constexpr int kVarOutCols = 512;
+struct OutValid { uint32_t* valid[kMaxPipeCols]; /* nullptr: the column leaves without a bitmap */ };
+static_assert(kDenseParamsOff + (int)sizeof(OutValid) <= kFiltParamsOff, "OutValid fits the sink's block");
+// one 16-byte value (Decimal128): Arrow promises only 8-byte alignment of a sliced input buffer
+__device__ __forceinline__ void copy16(const ColRef& c, int64_t row, void* dst, uint64_t pol) {
+  uint4 v;
+  if (c.vec) v = ld_stream_v4((const char*)c.ptr + row * 16, pol);
+  else {
+    const uint64_t lo = ld_stream_int(c.ptr, 8, 0, 2 * row, pol), hi = ld_stream_int(c.ptr, 8, 0, 2 * row + 1, pol);
+    v = make_uint4((uint32_t)lo, (uint32_t)(lo >> 32), (uint32_t)hi, (uint32_t)(hi >> 32));
+  }
+  *(uint4*)dst = v;
+}
 // stage s's filter on one candidate pair (ext: the payload words of stages 0..s): TRUE passes, NULL and FALSE do not; errors are or-ed
 // into err_ok[0], so only candidate pairs raise
 template <bool DEC>
@@ -581,8 +603,9 @@ __device__ __forceinline__ void dense_reduce_peers(unsigned peers, int op, unsig
 template <int SINK, bool DEC, int VAR = 0>
 __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PACK) || SINK == SINK_DENSE) ? 2 : 3) pipe_kernel(const PipeParams* __restrict__ gp, int64_t n, unsigned long long* __restrict__ counters /* [alive, inserted, fail, err] */) {
   constexpr int PB = kPhaseB, PBG = kPhaseBGroup, QC = kQueueCap;
-  constexpr bool RING = (VAR & 64) != 0, PART = (VAR & 128) != 0, FILT = (VAR & kVarFilt) != 0;
+  constexpr bool RING = (VAR & 64) != 0, PART = (VAR & 128) != 0, FILT = (VAR & kVarFilt) != 0, OUTV = (VAR & kVarOutCols) != 0;
   static_assert(!FILT || !(RING || PART), "stage filters do not run on the ring-fed or partitioned paths");
+  static_assert(!OUTV || SINK == SINK_OUTPUT_ANY, "output bitmaps and 16-byte columns belong to the unordered output sink");
   __shared__ PipeParams sp;
   __shared__ uint32_t q_rows[kPipeWarps][QC];
   extern __shared__ __align__(128) unsigned char dyn_smem[];   // RING: mbarriers [warp][stage], then the rings [warp][stage][ring_bytes]
@@ -939,6 +962,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
           alive_cnt++;
           for (int c = 0; c < sp.n_out; ++c) {
             const int src = sp.out_src[c], w = sp.out_width[c];
+            if (OUTV && w == 16) { copy16(sp.col[src], row[u], (char*)sp.out_dst[c] + (obase + mypos[u]) * 16, pol_stream); continue; }   // inputs only
             uint64_t v;
             if (src < sp.n_cols) v = ld_stream_int(sp.col[src].ptr, w, 0, row[u], pol_stream);
             else { const ExtDef e = sp.ext[src - sp.n_cols]; uint64_t wd = 0;
@@ -952,6 +976,29 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
               case 4: ((uint32_t*)sp.out_dst[c])[o] = (uint32_t)v; break;
               default: ((uint64_t*)sp.out_dst[c])[o] = v; break;
             }
+          }
+        }
+        if constexpr (OUTV) {   // the live lanes of item u hold the lane-ordered range [obase + at, obase + at + popc(m)): at most two words
+          const OutValid* ov = (const OutValid*)((const char*)gp + kDenseParamsOff);
+          unsigned int at = 0;
+#pragma unroll
+          for (int u = 0; u < PB; ++u) {
+            const unsigned m = __ballot_sync(0xffffffffu, live[u]);
+            const unsigned rank = __popc(m & ((1u << lane) - 1u));
+            const unsigned long long start = obase + at;
+#pragma unroll 1
+            for (int c = 0; m && c < sp.n_out; ++c) {
+              uint32_t* dv = ov->valid[c];
+              if (!dv) continue;
+              const ColRef& col = sp.col[sp.out_src[c]];
+              const unsigned bits = __reduce_or_sync(0xffffffffu, live[u] && bit_get(col.valid, col.voff + row[u]) ? 1u << rank : 0u);
+              const int sh = (int)(start & 31);
+              if (lane == 0 && bits) {
+                atomicOr(dv + (start >> 5), bits << sh);
+                if (sh && (bits >> (32 - sh))) atomicOr(dv + (start >> 5) + 1, bits >> (32 - sh));
+              }
+            }
+            at += __popc(m);
           }
         }
       }
@@ -1327,10 +1374,10 @@ __global__ void __launch_bounds__(256) pipe_probe_agg_kernel(const ulonglong2* _
 struct OutCols { int n; int src[kMaxPipeCols]; int width[kMaxPipeCols]; void* dst[kMaxPipeCols]; };
 
 // FILT: the stage filters (FiltParams at offset 0 of the dynamic shared memory), evaluated on each candidate pair with the interpreter of
-// pipe_kernel's DEC instantiations
-template <bool FILT>
-__global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipeParams* __restrict__ gp, int64_t n, OutCols oc, unsigned long long* __restrict__ tile_desc,
-                                                                  unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
+// pipe_kernel's DEC instantiations.  COLS: output columns with bitmaps or 16 bytes wide (OutValid behind PipeParams; pipe_output_cols_kernel)
+template <bool FILT, bool COLS>
+__device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ gp, int64_t n, const OutCols& oc, unsigned long long* __restrict__ tile_desc,
+                                                 unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
   __shared__ PipeParams sp;
   __shared__ uint32_t s_p[kPipeTile];
   __shared__ unsigned long long s_pay[kMaxStages][kPipeTile];
@@ -1459,6 +1506,7 @@ __global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipePar
   for (int c = 0; c < oc.n; ++c) {
     const int src = oc.src[c], w = oc.width[c];
     for (uint32_t j = threadIdx.x; j < tot; j += kPipeThreads) {
+      if (COLS && w == 16) { copy16(sp.col[src], prow0 + s_p[j], (char*)oc.dst[c] + (obase + j) * 16, policy_evict_first()); continue; }   // inputs only
       uint64_t v;
       if (src < sp.n_cols) v = ld_stream_int(sp.col[src].ptr, w, 0, prow0 + s_p[j], policy_evict_first());
       else { const ExtDef e = sp.ext[src - sp.n_cols]; v = ext_field(s_pay[e.stage][j], e.shift, e.width, DFGPU_UINT64); }
@@ -1470,7 +1518,51 @@ __global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipePar
       }
     }
   }
+  if constexpr (COLS) {
+    // the tile's output bits [obase, obase + tot), staged as whole words in shared memory: a warp's 32 survivors are one ballot, or-ed
+    // into at most two staged words.  The first and the last word may be shared with the neighbouring tiles: atomicOr into the zeroed
+    // bitmap; the words in between belong to this tile alone: plain stores.
+    __shared__ uint32_t s_vw[kPipeTile / 32 + 2];
+    const OutValid* ov = (const OutValid*)((const char*)gp + kDenseParamsOff);
+    const int sh = (int)(obase & 31), lane = threadIdx.x & 31;
+    const int nw = tot ? (int)((sh + tot + 31) >> 5) : 0;
+    for (int c = 0; c < oc.n; ++c) {
+      uint32_t* dv = ov->valid[c];
+      if (!dv || nw == 0) continue;
+      const ColRef& col = sp.col[oc.src[c]];
+      for (int i = threadIdx.x; i < nw; i += kPipeThreads) s_vw[i] = 0;
+      __syncthreads();
+      for (uint32_t j0 = 0; j0 < tot; j0 += kPipeThreads) {
+        const uint32_t j = j0 + threadIdx.x;
+        const unsigned bits = __ballot_sync(0xffffffffu, j < tot && bit_get(col.valid, col.voff + prow0 + s_p[j]));
+        const uint32_t first = (uint32_t)sh + j0 + (threadIdx.x & ~31u);   // staged bit of this warp's lane 0
+        if (lane == 0 && bits) {
+          atomicOr(&s_vw[first >> 5], bits << (first & 31));
+          if ((first & 31) && (bits >> (32 - (first & 31)))) atomicOr(&s_vw[(first >> 5) + 1], bits >> (32 - (first & 31)));
+        }
+      }
+      __syncthreads();
+      uint32_t* g = dv + (obase >> 5);
+      for (int i = threadIdx.x; i < nw; i += kPipeThreads) {
+        if (i == 0 || i == nw - 1) { if (s_vw[i]) atomicOr(g + i, s_vw[i]); }
+        else g[i] = s_vw[i];
+      }
+      __syncthreads();   // s_vw is staged again for the next column
+    }
+  }
   if (err) atomicOr(&counters[3], (unsigned long long)err);
+}
+
+template <bool FILT>
+__global__ void __launch_bounds__(kPipeThreads) pipe_output_kernel(const PipeParams* __restrict__ gp, int64_t n, OutCols oc, unsigned long long* __restrict__ tile_desc,
+                                                                  unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
+  pipe_output_tile<FILT, false>(gp, n, oc, tile_desc, tile_counter, totals, counters);
+}
+// the same for output columns with validity bitmaps or 16 bytes wide
+template <bool FILT>
+__global__ void __launch_bounds__(kPipeThreads) pipe_output_cols_kernel(const PipeParams* __restrict__ gp, int64_t n, OutCols oc, unsigned long long* __restrict__ tile_desc,
+                                                                       unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
+  pipe_output_tile<FILT, true>(gp, n, oc, tile_desc, tile_counter, totals, counters);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -2092,7 +2184,7 @@ static bool pipeline_has_decimal(const dfgpu_pipeline* p);
 constexpr int filt_var(int sink) { return kVarFilt | (sink == SINK_AGG ? kPipeVarDefault : (sink == SINK_PACK || sink == SINK_OUTPUT_ANY ? 2 : 0)); }
 
 template <int SINK>
-static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, const char* timer_name, bool part = false) {
+static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, const char* timer_name, bool part = false, bool out_cols = false) {
   dfgpu_ctx* ctx = p->ctx;
   const int64_t ntiles = (n + kPipeTile - 1) / kPipeTile;
   // FiltParams in dynamic shared memory; Decimal128 programs anywhere take the 128-bit interpreter.  There is one filtered instantiation
@@ -2101,6 +2193,8 @@ static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, cons
     DF_CHECK(!part, DFGPU_ERR_INVALID, "internal: the partitioned aggregate takes no stage filters");
     void (*kern)(const PipeParams*, int64_t, unsigned long long*) =
         pipeline_has_decimal(p) ? pipe_kernel<SINK, true, kVarFilt> : pipe_kernel<SINK, false, filt_var(SINK)>;
+    if constexpr (SINK == SINK_OUTPUT_ANY)   // output bitmaps or 16-byte columns (OutValid)
+      if (out_cols) kern = pipeline_has_decimal(p) ? pipe_kernel<SINK, true, kVarFilt | kVarOutCols> : pipe_kernel<SINK, false, filt_var(SINK) | kVarOutCols>;
     DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FiltParams)));   // per device: on every launch
     static const int blocks_env_f = getenv("DFGPU_PIPE_BLOCKS_PER_SM") ? atoi(getenv("DFGPU_PIPE_BLOCKS_PER_SM")) : 0;
     int blocks_per_sm = blocks_env_f;
@@ -2136,6 +2230,16 @@ static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, cons
     return;
   }
   DF_CHECK(!part, DFGPU_ERR_INVALID, "internal: the partitioned aggregate needs the ring-fed pipeline kernel");
+  if constexpr (SINK == SINK_OUTPUT_ANY) if (out_cols) {   // output bitmaps or 16-byte columns: the default bits of this sink plus OutValid
+    void (*kern)(const PipeParams*, int64_t, unsigned long long*) = dec ? pipe_kernel<SINK, true, kVarOutCols> : pipe_kernel<SINK, false, 2 | kVarOutCols>;
+    int blocks_per_sm = 0;
+    DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, 0));
+    const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
+    KernelTimer kt(ctx, tname.c_str());
+    kern<<<grid, kPipeThreads, 0, ctx->stream>>>(gp, n, cnt);
+    DF_LAUNCH_CHECK(ctx);
+    return;
+  }
   static const int blocks_env = getenv("DFGPU_PIPE_BLOCKS_PER_SM") ? atoi(getenv("DFGPU_PIPE_BLOCKS_PER_SM")) : 0;
   int blocks_per_sm = blocks_env;
   if (blocks_per_sm <= 0) {   // persistent blocks: exactly one resident wave (a second wave would start after the first finished)
@@ -2170,6 +2274,32 @@ static void upload_params(dfgpu_pipeline* p, const PipeParams& pp) {
   if (!p->params_dev.ptr) p->params_dev.alloc(p->ctx, sizeof(PipeParams));
   DF_CUDA(cudaMemcpyAsync(p->params_dev.ptr, &pp, sizeof(PipeParams), cudaMemcpyHostToDevice, p->ctx->stream));
   DF_CUDA(cudaStreamSynchronize(p->ctx->stream));   // `pp` lives on the caller's stack frame
+}
+
+// the output sink's columns for one push of n rows: a column has a (zeroed) bitmap exactly when its input column has one in this push
+static std::vector<DCol> alloc_output(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t n, OutValid* ov) {
+  memset(ov, 0, sizeof(*ov));
+  std::vector<DCol> part;
+  for (size_t c = 0; c < p->out_cols.size(); ++c) {
+    const int src = p->out_cols[c];
+    const bool nullable = src < (int)cols.size() && cols[src].validity;
+    DCol d = alloc_col(p->ctx, p->vtypes[src], n, nullable);
+    if (nullable) { d.own_validity->zero(); ov->valid[c] = d.own_validity->as<uint32_t>(); }
+    part.push_back(std::move(d));
+  }
+  return part;
+}
+// the output kernels with bitmaps and 16-byte columns (pipe_kernel VAR bit 512, pipe_output_cols_kernel) run only when a column needs them
+static bool output_needs_cols(const dfgpu_pipeline* p, const OutValid* ov) {
+  for (size_t c = 0; c < p->out_cols.size(); ++c)
+    if (ov->valid[c] || type_width(p->vtypes[p->out_cols[c]]) == 16) return true;
+  return false;
+}
+// OutValid into the sink's block behind PipeParams (after fill_params: the stage filters' upload sizes the buffer past this block)
+static void upload_out_valid(dfgpu_pipeline* p, const OutValid& ov) {
+  const size_t bytes = kDenseParamsOff + sizeof(OutValid);
+  if (p->params_dev.bytes < bytes) p->params_dev.alloc(p->ctx, bytes);
+  DF_CUDA(cudaMemcpyAsync((char*)p->params_dev.ptr + kDenseParamsOff, &ov, sizeof(OutValid), cudaMemcpyHostToDevice, p->ctx->stream));
 }
 
 static void prepare_acc(dfgpu_pipeline* p) {
@@ -2595,19 +2725,19 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   } else if (!p->out_ordered) {   // SINK_OUTPUT, row order unspecified: the two-phase kernel, one global reservation per 128 survivors
     DF_CHECK(n < 0xFFFFFFFFll, DFGPU_ERR_UNSUPPORTED, "pipeline: a batch must have < 2^32-1 rows");
     fill_params(p, cols, &pp);
-    std::vector<DCol> part;
+    OutValid ov;
+    std::vector<DCol> part = alloc_output(p, cols, n, &ov);
     pp.n_out = (int)p->out_cols.size();
     for (int c = 0; c < pp.n_out; ++c) {
       const int src = p->out_cols[c];
-      if (src < (int)cols.size()) DF_CHECK(!cols[src].validity, DFGPU_ERR_UNSUPPORTED, "pipeline output: nullable columns stay on the unfused operators");
-      DCol d = alloc_col(ctx, p->vtypes[src], n, false);
-      pp.out_src[c] = src; pp.out_width[c] = type_width(p->vtypes[src]); pp.out_dst[c] = d.own_values->ptr;
-      part.push_back(std::move(d));
+      pp.out_src[c] = src; pp.out_width[c] = type_width(p->vtypes[src]); pp.out_dst[c] = part[c].own_values->ptr;
     }
+    const bool out_cols = output_needs_cols(p, &ov);
+    if (out_cols) upload_out_valid(p, ov);
     p->counters.zero();
     pp.out_counter = p->counters.as<unsigned long long>() + 4;
     upload_params(p, pp);
-    launch_pipe<SINK_OUTPUT_ANY>(p, pp, n, "pipeline_output");
+    launch_pipe<SINK_OUTPUT_ANY>(p, pp, n, "pipeline_output", false, out_cols);
     unsigned long long h8[8];
     DF_CUDA(cudaMemcpyAsync(h8, p->counters.ptr, 64, cudaMemcpyDeviceToHost, ctx->stream));
     DF_CUDA(cudaStreamSynchronize(ctx->stream));
@@ -2623,18 +2753,18 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     DF_CHECK(n < 0xFFFFFFFFll, DFGPU_ERR_UNSUPPORTED, "pipeline: a batch must have < 2^32-1 rows");
     for (auto& st : p->stages) DF_CHECK(st.kind != DFGPU_STAGE_MAYBE, DFGPU_ERR_UNSUPPORTED, "pipeline: MAYBE stages feed an exchange — use the unordered output sink");
     fill_params(p, cols, &pp);
+    OutValid ov;
+    std::vector<DCol> part = alloc_output(p, cols, n, &ov);
+    const bool out_cols = output_needs_cols(p, &ov);
+    if (out_cols) upload_out_valid(p, ov);
     upload_params(p, pp);
     p->counters.zero();
     OutCols oc;
     memset(&oc, 0, sizeof(oc));
     oc.n = (int)p->out_cols.size();
-    std::vector<DCol> part;
     for (int c = 0; c < oc.n; ++c) {
       const int src = p->out_cols[c];
-      if (src < (int)cols.size()) DF_CHECK(!cols[src].validity, DFGPU_ERR_UNSUPPORTED, "pipeline output: nullable columns stay on the unfused operators");
-      DCol d = alloc_col(ctx, p->vtypes[src], n, false);
-      oc.src[c] = src; oc.width[c] = type_width(p->vtypes[src]); oc.dst[c] = d.own_values->ptr;
-      part.push_back(std::move(d));
+      oc.src[c] = src; oc.width[c] = type_width(p->vtypes[src]); oc.dst[c] = part[c].own_values->ptr;
     }
     const int64_t nt = (n + kPipeTile - 1) / kPipeTile;
     DevBuf desc(ctx, (size_t)nt * 8 + 32);
@@ -2643,7 +2773,14 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     unsigned int* counter = (unsigned int*)(totals + 2);
     {
       KernelTimer kt(ctx, "pipeline_output");
-      if (pipeline_has_filters(p)) {
+      if (out_cols) {   // the instantiations above stay as they were for columns without bitmaps, <= 8 bytes wide
+        const bool filt = pipeline_has_filters(p);
+        void (*kern)(const PipeParams*, int64_t, OutCols, unsigned long long*, unsigned int*, unsigned long long*, unsigned long long*) =
+            filt ? pipe_output_cols_kernel<true> : pipe_output_cols_kernel<false>;
+        if (filt) DF_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FiltParams)));
+        kern<<<(int)nt, kPipeThreads, filt ? sizeof(FiltParams) : 0, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, oc, desc.as<unsigned long long>(), counter, totals,
+                                                                                   p->counters.as<unsigned long long>());
+      } else if (pipeline_has_filters(p)) {
         DF_CUDA(cudaFuncSetAttribute(pipe_output_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(FiltParams)));
         pipe_output_kernel<true><<<(int)nt, kPipeThreads, sizeof(FiltParams), ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, oc, desc.as<unsigned long long>(), counter,
                                                                                            totals, p->counters.as<unsigned long long>());
@@ -3343,7 +3480,6 @@ int dfgpu_pipeline_sink_output(dfgpu_pipeline* p, const int32_t* out_cols, int32
   check_no_left_stage(p);
   for (int c = 0; c < n_out; ++c) {
     DF_CHECK(out_cols[c] >= 0 && out_cols[c] < (int)p->vtypes.size(), DFGPU_ERR_INVALID, "pipeline output: column out of range");
-    DF_CHECK(type_width(p->vtypes[out_cols[c]]) <= 8, DFGPU_ERR_UNSUPPORTED, "pipeline output: 16-byte columns leave through dfgpu_filter / dfgpu_hashjoin");
     p->out_cols.push_back(out_cols[c]);
   }
   p->batch_size = batch_size; p->sink = SINK_OUTPUT;

@@ -764,11 +764,14 @@ class GpuPipelineExec(ExecutionPlan):
 
     def __init__(self, scan: _Scan, sink: str, key: Optional[str] = None, payload: Sequence[str] = (), group_by: Sequence[str] = (),
                  aggs: Sequence[Tuple[str, Optional[Expr], str]] = (), mode: str = "Single", out_schema: Optional[pa.Schema] = None,
-                 key_range: Sequence[Tuple[int, int]] = (), nullable: Sequence[bool] = (), project: Optional[Sequence[int]] = None):
+                 key_range: Sequence[Tuple[int, int]] = (), nullable: Sequence[bool] = (), project: Optional[Sequence[int]] = None,
+                 out_cols: Sequence[int] = (), fallback: Optional[ExecutionPlan] = None):
         self.scan, self.sink, self.key, self.payload, self.group_by, self.aggs, self.mode = scan, sink, key, list(payload), list(group_by), list(aggs), mode
         self.key_range = list(key_range)   # dense sink: the declared (min, max) of every group column
         self.nullable = list(nullable)     # hash sink: the declared nullability of every group column
         self.project = None if project is None else list(project)   # the emitted columns that form the output (a LeftSemi / LeftAnti join's projection)
+        self.out_cols = list(out_cols)     # output sink: the virtual columns of the scan that form the output, in order
+        self.fallback = fallback           # output sink: the unfused plan, run when a build side cannot be fused (_execute_output)
         self.schema = out_schema if out_schema is not None else pa.schema([])
         self.n_acc_words = 0
         self._metrics = {}
@@ -790,13 +793,20 @@ class GpuPipelineExec(ExecutionPlan):
             if lo:
                 key_range = (min(lo), max(hi))
         look = D.Lookup(ctx.gpu, type_id(ktype), [type_id(vs.field(n).type) for n in self.payload], key_range=key_range, n_acc_words=self.n_acc_words)
-        pipe, keep = self._make_pipeline(ctx)
+        try:
+            pipe, keep = self._make_pipeline(ctx)
+        except BaseException:
+            look.close()
+            raise
         try:
             pipe.sink_build(look, vs.get_field_index(self.key), [vs.get_field_index(n) for n in self.payload])
             for rb in batches:
                 pipe.push_arrow(rb)
             pipe.finish()
             self._metrics = {"input_rows": pipe.metric("input_rows"), "build_rows": pipe.metric("sink_rows"), "lookup_mode": look.metric("mode")}
+        except BaseException:
+            look.close()
+            raise
         finally:
             pipe.close()
             for l in keep:
@@ -810,10 +820,15 @@ class GpuPipelineExec(ExecutionPlan):
             nodes = []
             self.scan.predicate.rpn(ssch, nodes)
         stages, keep = [], []
-        for kind, pkey, build in self.scan.stages:
-            look = build.build_lookup(ctx)                      # the pipeline breaker: WaitBuildSide (hash_join/stream.rs:117-140)
-            keep.append(look)
-            stages.append((kind, ssch.get_field_index(pkey), look))
+        try:
+            for kind, pkey, build in self.scan.stages:
+                look = build.build_lookup(ctx)                  # the pipeline breaker: WaitBuildSide (hash_join/stream.rs:117-140)
+                keep.append(look)
+                stages.append((kind, ssch.get_field_index(pkey), look))
+        except BaseException:
+            for l in keep:
+                l.close()
+            raise
         pipe = D.Pipeline(ctx.gpu, [type_id(f.type) for f in ssch], nodes, stages)
         try:
             for s, fnodes in sorted(self.scan.filters.items()):
@@ -826,7 +841,10 @@ class GpuPipelineExec(ExecutionPlan):
         return pipe, keep
 
     def execute(self, ctx):
-        assert self.sink in ("aggregate", "dense", "hash"), "build pipelines are driven by their consumer"
+        assert self.sink in ("aggregate", "dense", "hash", "output"), "build pipelines are driven by their consumer"
+        if self.sink == "output":
+            yield from self._execute_output(ctx)
+            return
         vs = self.scan.virtual_schema()
         pipe, keep = self._make_pipeline(ctx)
         try:
@@ -857,6 +875,45 @@ class GpuPipelineExec(ExecutionPlan):
             pipe.close()
             for l in keep:
                 l.close()
+
+
+    def _execute_output(self, ctx):
+        """the ordered output sink (dfgpu_pipeline_sink_output): the surviving rows in input order, sliced by batch_size.  The sink
+        emits nothing before finish, so every refusal comes first: when the library refuses the fused plan (DFGPU_ERR_UNSUPPORTED, e.g.
+        duplicate keys in an Inner stage's build, a NULL in a payload column, a Boolean input column) the unfused plan runs instead and
+        the metric "fallback" holds the reason.  Other errors (arithmetic, state) propagate."""
+        try:
+            pipe, keep = self._make_pipeline(ctx)
+        except D.DfgpuError as e:
+            yield from self._fall_back(ctx, e)
+            return
+        try:
+            try:
+                pipe.sink_output(self.out_cols, batch_size=ctx.config.batch_size)
+                for rb in self.scan.source.execute(ctx):
+                    pipe.push_arrow(rb)
+                pipe.finish()
+            except D.DfgpuError as e:
+                refused = e
+            else:
+                refused = None
+                yield from _drain(pipe, self.schema)
+                self._metrics = {k: pipe.metric(k) for k in ("input_rows", "sink_rows", "output_rows")}
+        finally:
+            pipe.close()
+            for l in keep:
+                l.close()
+        if refused is not None:
+            yield from self._fall_back(ctx, refused)
+
+    def _fall_back(self, ctx, e: "D.DfgpuError"):
+        if self.fallback is None or e.code != _ERR_UNSUPPORTED:
+            raise e
+        yield from self.fallback.execute(ctx)
+        self._metrics = {"fallback": str(e)}
+
+
+_ERR_UNSUPPORTED = -3   # DFGPU_ERR_UNSUPPORTED (include/dfgpu.h)
 
 
 def _source_bounds(source: ExecutionPlan, name: str) -> Optional[Tuple[int, int]]:
@@ -1193,6 +1250,67 @@ def fuse_join_filters(plan: ExecutionPlan) -> ExecutionPlan:
     if fused is not plan:
         return fused
     return fuse_hash_aggregates(plan, join_filters=True)
+
+
+def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_join_filters: its result when that rule fuses; otherwise a top-level
+    [ProjectionExec(columns only)] over a HashJoinExec(Inner / RightSemi / RightAnti) chain, as _as_scan accepts it with JoinFilters and
+    with at least one stage, becomes ONE GpuPipelineExec over the ordered output sink (dfgpu_pipeline_sink_output) that emits the plan's
+    schema: a probe-side column comes from the input, the build key of an Inner stage from its probe key (only when the two have the
+    same type), any other build column from the stage's payload field.  The fused lookups need unique build keys: an Inner stage without
+    payload gets a row-counter word, so its build refuses duplicate keys like one with payload.  Whether the keys are unique is known
+    only once the build side has run, so the fused node keeps the plan as its fallback: a build the library refuses (duplicate keys,
+    NULL payloads) runs the unfused joins instead, before any row is emitted.  The fused Inner join emits its rows in probe order, the
+    reference's order for unique build keys.  Anything else (a bare FilterExec, Left / Right / Full joins, several keys,
+    null-aware joins, computed projections) is returned unchanged."""
+    fused = fuse_join_filters(plan)
+    if fused is not plan:
+        return fused
+    join = plan.input if isinstance(plan, GpuProjectionExec) else plan
+    if not isinstance(join, GpuHashJoinExec) or join.join_type not in ("Inner", "RightSemi", "RightAnti"):
+        return plan
+    sc = _as_scan(join, join_filters=True)
+    if sc is None or not sc.stages:
+        return plan
+    vs = sc.virtual_schema()
+    kind, pkey, build = sc.stages[-1]
+    n_below = len(vs) - (len(build.payload) if kind == D.STAGE_INNER else 0)   # the virtual columns the top join's probe side sees
+    keys = {b.key: (p, b) for k, p, b in sc.stages if k == D.STAGE_INNER}       # an Inner stage's build key -> its probe key
+
+    def probe_col(name: str) -> int:
+        at = [i for i in range(n_below) if vs.field(i).name == name]
+        if len(at) == 1:
+            return at[0]
+        if not at and name in keys:                                             # a lower Inner stage's build key
+            p, b = keys[name]
+            i = probe_col(p) if p != name else -1
+            return i if i >= 0 and b.scan_field(name).type == vs.field(i).type else -1
+        return -1
+
+    pick = list(range(len(join.column_indices)))                                # the join's columns that form the output
+    if isinstance(plan, GpuProjectionExec):
+        names = [f.name for f in join.schema]
+        if not all(isinstance(e, Column) and names.count(e.name) == 1 for e, _ in plan.exprs):
+            return plan
+        pick = [names.index(e.name) for e, _ in plan.exprs]
+    cols = []
+    for side, ix in (join.column_indices[i] for i in pick):
+        if side == 1:
+            at = probe_col(join.right.schema.field(ix).name)
+        else:
+            name = join.left.schema.field(ix).name
+            if name == join.on[0][0]:
+                at = probe_col(pkey)
+                at = at if at >= 0 and join.left.schema.field(ix).type == vs.field(at).type else -1
+            else:
+                at = n_below + build.payload.index(name) if name in build.payload else -1
+        if at < 0:
+            return plan
+        cols.append(at)
+    for k, _, b in sc.stages:
+        if k == D.STAGE_INNER and not b.payload:
+            b.n_acc_words = max(b.n_acc_words, 1)
+    return GpuPipelineExec(sc, sink="output", out_schema=plan.schema, out_cols=cols, fallback=plan)
 
 
 def collect(plan: ExecutionPlan, ctx: Optional[TaskContext] = None) -> List[pa.RecordBatch]:

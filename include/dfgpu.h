@@ -545,9 +545,16 @@ int dfgpu_pipeline_sink_aggregate_dense(dfgpu_pipeline* p, const int32_t* group_
 int dfgpu_pipeline_sink_aggregate_hash(dfgpu_pipeline* p, const int32_t* group_cols, const int32_t* group_nullable, int32_t n_group,
                                        const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size,
                                        int64_t capacity_hint);
+/* output: the surviving rows, columns = out_cols (1..16) of the virtual schema, input order preserved, sliced by batch_size (0 = one
+ * batch).  Any input column may leave: widths 1, 2, 4, 8 and 16 bytes (Decimal128(p, s) included), with or without a validity bitmap
+ * at any Arrow bit offset; payload fields leave too (they are never nullable).  An output column has a bitmap exactly when its input
+ * column had one in that push (a column pushed with null_count 0 has none); once several pushes are merged, a column has one when any
+ * push gave it one.  Returned bitmap columns report null_count = -1 (unknown), as dfgpu_exchange_columns does.  Boolean input
+ * columns are refused by the push (DFGPU_ERR_UNSUPPORTED), so they cannot be output. */
 int dfgpu_pipeline_sink_output(dfgpu_pipeline* p, const int32_t* out_cols, int32_t n_out, int64_t batch_size);
 /* the same, row order unspecified (what a RepartitionExec consumer sees anyway, repartition/mod.rs:1320-1400): runs on the two-phase
- * kernel and is several times faster than the ordered sink on selective pipelines */
+ * kernel and is several times faster than the ordered sink on selective pipelines; it takes the same columns, bitmaps and
+ * Decimal128 values as the ordered sink */
 int dfgpu_pipeline_sink_output_unordered(dfgpu_pipeline* p, const int32_t* out_cols, int32_t n_out, int64_t batch_size);
 /* JoinFilter of probe stage `stage` (joins/utils.rs:1248-1320 apply_join_filter_to_indices; hash_join/stream.rs:896-906): a Boolean RPN
  * program evaluated on each probe row whose key matched at that stage (a candidate pair).  NULL or false means the pair does not match:
