@@ -169,6 +169,7 @@ EXPORTS = [
     "dfgpu_pipeline_sink_aggregate_hash", "dfgpu_pipeline_sink_output",
     "dfgpu_pipeline_push_host", "dfgpu_pipeline_push_device", "dfgpu_pipeline_push_arrow", "dfgpu_pipeline_finish",
     "dfgpu_pipeline_next", "dfgpu_pipeline_metric", "dfgpu_pipeline_destroy",
+    "dfgpu_lookup_create_composite", "dfgpu_pipeline_set_stage_keys", "dfgpu_pipeline_sink_build_composite",
     "dfgpu_dictionary_create", "dfgpu_dictionary_unify", "dfgpu_dictionary_code", "dfgpu_dictionary_size", "dfgpu_dictionary_value",
     "dfgpu_dictionary_remap", "dfgpu_dictionary_destroy",
 ]
@@ -281,6 +282,7 @@ def load_library() -> C.CDLL:
     sig("dfgpu_dictionary_destroy", None, [vp])
     sig("dfgpu_lookup_default_options", None, [P(LookupOptions)])
     sig("dfgpu_lookup_create", C.c_int, [vp, i32, P(i32), i32, P(LookupOptions), P(vp)])
+    sig("dfgpu_lookup_create_composite", C.c_int, [vp, P(i32), P(i64), P(i64), i32, P(i32), i32, P(LookupOptions), P(vp)])
     sig("dfgpu_lookup_metric", i64, [vp, C.c_char_p])
     sig("dfgpu_lookup_destroy", None, [vp])
     sig("dfgpu_lookup_clear", C.c_int, [vp])
@@ -291,6 +293,8 @@ def load_library() -> C.CDLL:
     sig("dfgpu_column_sum_device", C.c_int, [vp, P(Column), P(u64), P(i64)])
     sig("dfgpu_pipeline_create", C.c_int, [vp, P(i32), i32, P(ExprNode), i32, P(PipelineStage), i32, P(vp)])
     sig("dfgpu_pipeline_sink_build", C.c_int, [vp, vp, i32, P(i32), i32])
+    sig("dfgpu_pipeline_sink_build_composite", C.c_int, [vp, vp, P(i32), i32, P(i32), i32])
+    sig("dfgpu_pipeline_set_stage_keys", C.c_int, [vp, i32, P(i32), i32])
     sig("dfgpu_pipeline_sink_aggregate", C.c_int, [vp, P(i32), i32, P(PipelineAgg), i32, i32, i64])
     sig("dfgpu_pipeline_sink_aggregate_dense", C.c_int, [vp, P(i32), P(i64), P(i64), i32, P(PipelineAgg), i32, i32, i64])
     sig("dfgpu_pipeline_sink_aggregate_hash", C.c_int, [vp, P(i32), P(i32), i32, P(PipelineAgg), i32, i32, i64, i64])
@@ -773,10 +777,12 @@ def column_sum_device(ctx: Context, col) -> int:
 
 
 class Lookup:
-    """dfgpu_lookup: the build side of a fused join (unique keys, <= 64 bits of payload, optional accumulator words)"""
+    """dfgpu_lookup: the build side of a fused join (unique keys, <= 64 bits of payload, optional accumulator words).
+    A composite key (dfgpu_lookup_create_composite): key_types = the 2..4 component types and key_ranges = their declared (min, max),
+    instead of key_type / key_range"""
 
-    def __init__(self, ctx: Context, key_type: int, payload_types=(), expected_rows: int = 0, key_range=None, n_acc_words: int = 0,
-                 membership_filter: int = -1, filter_only: bool = False):
+    def __init__(self, ctx: Context, key_type: Optional[int] = None, payload_types=(), expected_rows: int = 0, key_range=None, n_acc_words: int = 0,
+                 membership_filter: int = -1, filter_only: bool = False, key_types=None, key_ranges=None):
         self.ctx = ctx
         self.h = C.c_void_p()
         opt = LookupOptions()
@@ -785,7 +791,17 @@ class Lookup:
         opt.filter_only = 1 if filter_only else 0
         if key_range is not None:
             opt.has_key_range, opt.key_min, opt.key_max = 1, int(key_range[0]), int(key_range[1])
-        ctx.check(ctx.lib.dfgpu_lookup_create(ctx.h, key_type, _i32arr(list(payload_types)), len(payload_types), C.byref(opt), C.byref(self.h)))
+        pay = _i32arr(list(payload_types))
+        if key_types is not None:
+            if key_type is not None or key_ranges is None or len(key_ranges) != len(key_types):
+                raise ValueError("Lookup: a composite key takes key_types and one (min, max) per component in key_ranges, and no key_type")
+            n = len(key_types)
+            kmin = (C.c_int64 * n)(*[int(lo) for lo, _ in key_ranges])
+            kmax = (C.c_int64 * n)(*[int(hi) for _, hi in key_ranges])
+            ctx.check(ctx.lib.dfgpu_lookup_create_composite(ctx.h, _i32arr(list(key_types)), kmin, kmax, n, pay, len(payload_types), C.byref(opt),
+                                                            C.byref(self.h)))
+        else:
+            ctx.check(ctx.lib.dfgpu_lookup_create(ctx.h, key_type, pay, len(payload_types), C.byref(opt), C.byref(self.h)))
 
     def metric(self, name: str) -> int:
         return self.ctx.lib.dfgpu_lookup_metric(self.h, name.encode())
@@ -816,7 +832,8 @@ class Lookup:
 
 
 class Pipeline(_Operator):
-    """dfgpu_pipeline: predicate -> probe stage(s) -> sink, one pass.  stages: [(kind, key_col, Lookup)]
+    """dfgpu_pipeline: predicate -> probe stage(s) -> sink, one pass.  stages: [(kind, key_col, Lookup)]; key_col may be a list of input
+    columns, the components of a composite-key lookup (set_stage_keys)
     metric(): the names dfgpu.h lists at dfgpu_pipeline_metric, e.g. "partitioned_records", the {key, value} records the partitioned
     aggregate's first pass wrote (the rows that passed the folded membership filter and fit the record buffer)"""
     _next_fn, _destroy_fn, _metric_fn = "dfgpu_pipeline_next", "dfgpu_pipeline_destroy", "dfgpu_pipeline_metric"
@@ -828,11 +845,18 @@ class Pipeline(_Operator):
         na = expr_nodes(predicate) if predicate else None
         sa = (PipelineStage * max(len(stages), 1))()
         for i, (kind, key_col, lk) in enumerate(stages):
-            sa[i].kind, sa[i].key_col, sa[i].lookup = kind, key_col, lk.h
+            sa[i].kind, sa[i].key_col, sa[i].lookup = kind, key_col[0] if isinstance(key_col, (list, tuple)) else key_col, lk.h
         ctx.check(ctx.lib.dfgpu_pipeline_create(ctx.h, _i32arr(input_types), len(input_types), na, len(predicate) if predicate else 0,
                                                 sa, len(stages), C.byref(self.h)))
         if name:
             ctx.check(ctx.lib.dfgpu_pipeline_set_name(self.h, name.encode()))
+        for i, (_, key_col, _) in enumerate(stages):
+            if isinstance(key_col, (list, tuple)):
+                self.set_stage_keys(i, key_col)
+
+    def set_stage_keys(self, stage: int, key_cols):
+        """composite key of probe stage `stage`: the input columns of the lookup's components, in order"""
+        self.ctx.check(self.ctx.lib.dfgpu_pipeline_set_stage_keys(self.h, int(stage), _i32arr(list(key_cols)), len(key_cols)))
 
     def set_stage_filter(self, stage: int, nodes):
         """JoinFilter of probe stage `stage`: RPN over the input columns, the payload fields of the INNER / LEFT / LEFT_ANTI stages up to
@@ -840,9 +864,15 @@ class Pipeline(_Operator):
         na = expr_nodes(nodes)
         self.ctx.check(self.ctx.lib.dfgpu_pipeline_set_stage_filter(self.h, int(stage), na, len(nodes)))
 
-    def sink_build(self, target: Lookup, key_col: int, payload_cols=()):
+    def sink_build(self, target: Lookup, key_col: Optional[int] = None, payload_cols=(), key_cols=None):
+        """key_col: the key's input column; key_cols instead: the input columns of a composite-key lookup's components"""
         self._keep.append(target)
-        self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_build(self.h, target.h, key_col, _i32arr(list(payload_cols)), len(payload_cols)))
+        pay = _i32arr(list(payload_cols))
+        if key_cols is not None:
+            self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_build_composite(self.h, target.h, _i32arr(list(key_cols)), len(key_cols), pay,
+                                                                            len(payload_cols)))
+        else:
+            self.ctx.check(self.ctx.lib.dfgpu_pipeline_sink_build(self.h, target.h, key_col, pay, len(payload_cols)))
 
     def _agg_array(self, aggs):
         arr = (PipelineAgg * max(len(aggs), 1))()

@@ -396,6 +396,17 @@ int radix_partition(dfgpu_ctx* ctx, const unsigned long long* keys, const unsign
 // The same for n rows that are already 16-byte {key, val} records (recs 16-byte aligned): each 2048-row tile arrives by one bulk copy.
 int radix_partition_records(dfgpu_ctx* ctx, const void* recs, int64_t n, size_t table_bytes, int force_parts, void* out, unsigned long long* meta);
 
+// Composite join keys (composite_key.cu): the tuple of 2..4 integer-like components packs into sum_g (v_g - kmin_g) * stride_g, a
+// bijection of the declared domain onto [0, domain).  A probe-side key (out_valid == nullptr) whose row has a NULL or out-of-domain
+// component becomes `domain`, which no lookup holds.  A build-side key gets a validity bit (out_valid, bit offset 0): 0 for a NULL
+// component (counted in flags[1]) and for an out-of-domain one (flags[0] set to 1, never inserted).  Values and bitmaps are read at any
+// alignment and Arrow bit offset; out is 16-byte aligned.
+constexpr int kMaxKeyParts = 4, kMaxPackedKeys = 4;
+struct KeyPart { const void* ptr; const uint8_t* valid; int64_t voff; int width, sgn; unsigned long long kmin, range, stride; };
+struct PackedKey { int n_parts, pad; KeyPart part[kMaxKeyParts]; unsigned long long* out; uint8_t* out_valid; unsigned long long domain; };
+struct PackKeysParams { int n_keys, pad; PackedKey key[kMaxPackedKeys]; unsigned long long* flags /* [out-of-domain, NULL build keys] */; };
+void pack_keys(dfgpu_ctx* ctx, const PackKeysParams& kp, int64_t n);
+
 // ------------------------------------------------------------------------------------------
 // device bit helpers (Arrow validity bitmaps are LSB-numbered)
 // ------------------------------------------------------------------------------------------

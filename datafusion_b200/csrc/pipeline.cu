@@ -1706,12 +1706,14 @@ __global__ void __launch_bounds__(256) lookup_groups_kernel(LookupDev t, int row
 struct EmitCol {
   int kind /* 0 key, 1 payload field, 2 accumulator word, 3 AVG value, 4 count as u64, 5 Decimal128 sum / min / max (two words),
               6 dense group key decoded from the slot number, 7 Decimal128 AVG value, 8 packed group field of a 128-bit tag in words 0 and 1,
-              9 COUNT(*) of a LEFT join's build row: the row counter, at least 1 (the NULL-padded row of a record no probe row reached) */,
+              9 COUNT(*) of a LEFT join's build row: the row counter, at least 1 (the NULL-padded row of a record no probe row reached),
+              10 component of a composite key decoded from the packed key in word 0 */,
       width, shift, word, nn_word, cnt_word, f64_key /* kind 2: the word holds f64_to_ordered of a Float64 MIN / MAX */;
   void* dst; uint32_t* valid;
   long long kmin; int kstride, kradix;   // kind 6: key = kmin + (slot / kstride) % kradix, NULL when that index is kradix - 1
   int avg_mul, avg_prec;                  // kind 7: sum * 10^avg_mul / count must fit Decimal128(avg_prec, _)
   int tag_null;                           // kind 8: the field starts at bit `shift`; NULL when bit tag_null (>= 0) is set
+  unsigned long long cstride, cradix;     // kind 10: component = kmin + (key / cstride) % cradix
 };
 struct EmitCols { int n; EmitCol c[kMaxPipeCols]; unsigned long long* err /* kind 7: set to 1 on overflow */; };
 __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uint32_t* __restrict__ slots, int64_t n, int rows_word, EmitCols ec) {
@@ -1735,6 +1737,7 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
             break;
           case 4: v = r[e.word]; break;
           case 9: v = max(r[e.word], 1ull); break;
+          case 10: v = (uint64_t)e.kmin + (r[0] / e.cstride) % e.cradix; break;
           case 5:
             ok = e.nn_word >= 0 ? r[e.nn_word] != 0ull : true;
             ((unsigned long long*)e.dst)[2 * i] = ok ? r[e.word] : 0ull;
@@ -1858,6 +1861,8 @@ struct dfgpu_lookup {
   int64_t rows = 0, rehashes = 0;
   int64_t null_keys = 0;   // build rows pushed with a NULL key (counted before the predicate): never inserted, so a LEFT / LEFT_ANTI stage cannot emit them
   bool acc_claimed = false, filter_only = false;
+  // composite key (dfgpu_lookup_create_composite): the key is the packed tuple of these components, in [0, domain)
+  std::vector<int> comp_types; std::vector<int64_t> comp_min; std::vector<uint64_t> comp_range, comp_stride; uint64_t domain = 0;
 };
 
 struct PipeAgg { int func; ExprPlan plan; bool has_expr = false; int word = -1, nn_word = -1, cnt_word = -1, cls = C_I64, arg_type = 0; };
@@ -1876,6 +1881,11 @@ struct dfgpu_pipeline {
   int sink = SINK_NONE;
   // build sink
   dfgpu_lookup* target = nullptr; int bkey_col = -1; std::vector<int> bpay_cols;
+  // composite keys: the component input columns of each stage (dfgpu_pipeline_set_stage_keys) and of the build sink
+  // (dfgpu_pipeline_sink_build_composite); `packed` holds the current batch's packed keys in that order (stages, then the build sink),
+  // in PipeParams' column array behind the input columns; key_flags: [out-of-domain build key seen, NULL build keys], read at finish
+  std::vector<int> stage_keys[kMaxStages]; std::vector<int> bkey_cols;
+  std::vector<DCol> packed; DevBuf key_flags;
   // aggregate sink
   std::vector<int> group_cols; std::vector<PipeAgg> aggs; int agg_mode = DFGPU_AGG_SINGLE, agg_stage = -1, rows_word = -1; bool acc_ready = false;
   int left_kind = 0;   // DFGPU_STAGE_LEFT / DFGPU_STAGE_LEFT_ANTI when the last stage is one (it is then agg_stage), else 0
@@ -2102,12 +2112,22 @@ static bool conjunction_terms(const dfgpu_pipeline* p, int max_terms, std::vecto
   return fast && depth == 1 && !terms->empty();
 }
 
+// the column of PipeParams' array that stage s (s == kMaxStages: the build sink) reads its key from: a composite key's packed column
+// behind the input columns (pack_batch_keys' order), else the key column itself
+static int key_slot(const dfgpu_pipeline* p, int s) {
+  int k = (int)p->in_types.size();
+  for (int t = 0; t < (int)p->stages.size() && t < s; ++t) k += p->stage_keys[t].empty() ? 0 : 1;
+  if (s == kMaxStages) return p->bkey_cols.empty() ? p->bkey_col : k;
+  return p->stage_keys[s].empty() ? p->stages[s].key_col : k;
+}
+
 static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipeParams* pp) {
   memset(pp, 0, sizeof(*pp));
   pp->n_cols = (int)cols.size();
   static const int hints_env = getenv("DFGPU_PIPE_HINTS") ? atoi(getenv("DFGPU_PIPE_HINTS")) : 3;
   pp->hints = hints_env;
   for (size_t c = 0; c < cols.size(); ++c) pp->col[c] = col_ref(cols[c]);
+  for (size_t k = 0; k < p->packed.size(); ++k) pp->col[cols.size() + k] = col_ref(p->packed[k]);   // hidden: n_cols stays the inputs'
   int pool_used = 0;
   pp->pred_mode = 0;
   if (p->has_pred) {
@@ -2129,14 +2149,14 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
   for (size_t s = 0; s < p->stages.size(); ++s) {
     // a LEFT / LEFT_ANTI stage probes as an INNER one: the build rows no probe row reached are found in the records at finish
     const int kind = p->stages[s].kind;
-    pp->stage[s].kind = kind == DFGPU_STAGE_LEFT || kind == DFGPU_STAGE_LEFT_ANTI ? DFGPU_STAGE_INNER : kind; pp->stage[s].key_col = p->stages[s].key_col; pp->stage[s].lk = lookup_dev(p->stages[s].lookup);
+    pp->stage[s].kind = kind == DFGPU_STAGE_LEFT || kind == DFGPU_STAGE_LEFT_ANTI ? DFGPU_STAGE_INNER : kind; pp->stage[s].key_col = key_slot(p, (int)s); pp->stage[s].lk = lookup_dev(p->stages[s].lookup);
   }
   pp->n_ext = (int)p->exts.size();
   for (size_t e = 0; e < p->exts.size(); ++e) pp->ext[e] = p->exts[e];
   pp->agg_stage = -1;
   if (p->sink == SINK_BUILD) {
     pp->target = lookup_dev(p->target);
-    pp->bkey_col = p->bkey_col;
+    pp->bkey_col = key_slot(p, kMaxStages);
     pp->target_unique = (p->target->has_payload || p->target->opt.n_acc_words > 0) ? 1 : 0;
     pp->n_bpay = (int)p->bpay_cols.size();
     for (size_t c = 0; c < p->bpay_cols.size(); ++c) {
@@ -2495,12 +2515,15 @@ static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t 
   unsigned long long groups = 0;
   DF_CUDA(cudaMemcpyAsync(&groups, p->hash_ngroups.ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
   DF_CUDA(cudaStreamSynchronize(ctx->stream));
+  const std::vector<DCol> packed = p->packed;   // the batch's packed keys, sliced and replayed with the input columns
   for (int64_t done = 0; done < n; done += chunk, chunk = std::min(chunk * 4, kMaxChunk)) {
     const int64_t m = std::min(chunk, n - done);
     if (groups * 2 > p->hash_cap) hash_grow(p, p->hash_cap * 4);
     if (overflow.bytes < (size_t)m * 4) overflow.alloc(ctx, (size_t)m * 4);
     std::vector<DCol> batch;
     for (const DCol& c : cols) batch.push_back(m == n ? c : slice_column(c, done, m));
+    p->packed.clear();
+    for (const DCol& c : packed) p->packed.push_back(m == n ? c : slice_column(c, done, m));
     int64_t rows = m;
     while (true) {
       PipeParams pp;
@@ -2535,6 +2558,7 @@ static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t 
       std::vector<DCol> replay;
       for (const DCol& c : batch) replay.push_back(take_column(ctx, c, overflow.as<uint32_t>(), deferred, false));
       batch = std::move(replay);
+      for (DCol& c : p->packed) c = take_column(ctx, c, overflow.as<uint32_t>(), deferred, false);
       rows = deferred;
       p->m_replayed_rows += deferred;
     }
@@ -2562,10 +2586,45 @@ static int64_t count_null_keys(dfgpu_ctx* ctx, const DCol& c) {
   return c.length - (int64_t)h[2];
 }
 
+// One launch packs every composite key of the batch (composite_key.cu) into p->packed, timed as "pipe_keys:<name>"
+static void pack_batch_keys(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t n) {
+  p->packed.clear();
+  PackKeysParams kp;
+  memset(&kp, 0, sizeof(kp));
+  auto add = [&](const dfgpu_lookup* l, const std::vector<int>& key_cols, bool build) {
+    PackedKey& k = kp.key[kp.n_keys++];
+    k.n_parts = (int)key_cols.size();
+    for (size_t g = 0; g < key_cols.size(); ++g) {
+      const DCol& c = cols[key_cols[g]];
+      KeyPart& kc = k.part[g];
+      kc.ptr = c.values; kc.valid = c.validity; kc.voff = c.offset; kc.width = type_width(c.type); kc.sgn = type_is_signed_int(c.type) ? 1 : 0;
+      kc.kmin = (unsigned long long)l->comp_min[g]; kc.range = l->comp_range[g]; kc.stride = l->comp_stride[g];
+    }
+    DCol d = alloc_col(p->ctx, DFGPU_INT64, n, build);
+    if (build) d.null_count = -1;
+    k.out = d.own_values->as<unsigned long long>(); k.out_valid = build ? d.own_validity->as<uint8_t>() : nullptr; k.domain = l->domain;
+    p->packed.push_back(std::move(d));
+  };
+  for (size_t s = 0; s < p->stages.size(); ++s)
+    if (!p->stage_keys[s].empty()) add(p->stages[s].lookup, p->stage_keys[s], false);
+  if (!p->bkey_cols.empty()) {
+    add(p->target, p->bkey_cols, true);
+    if (!p->key_flags.ptr) { p->key_flags.alloc(p->ctx, 16); p->key_flags.zero(); }
+    kp.flags = p->key_flags.as<unsigned long long>();
+  }
+  if (kp.n_keys == 0) return;
+  const std::string tname = p->name.empty() ? std::string("pipe_keys") : "pipe_keys:" + p->name;
+  KernelTimer kt(p->ctx, tname.c_str());
+  pack_keys(p->ctx, kp, n);
+}
+
 static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   DF_CHECK(!p->finished, DFGPU_ERR_STATE, "push after finish");
   DF_CHECK(p->sink != SINK_NONE, DFGPU_ERR_STATE, "pipeline: choose a sink before the first push");
   DF_CHECK(cols.size() == p->in_types.size(), DFGPU_ERR_INVALID, "pipeline input column count mismatch");
+  for (size_t s = 0; s < p->stages.size(); ++s)
+    DF_CHECK(p->stages[s].lookup->comp_types.empty() || !p->stage_keys[s].empty(), DFGPU_ERR_STATE,
+             "pipeline: a stage over a composite-key lookup needs dfgpu_pipeline_set_stage_keys before the first push");
   check_left_build(p);
   p->pushed = true;
   dfgpu_ctx* ctx = p->ctx;
@@ -2580,11 +2639,12 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   p->m_input_rows += n;
   if (n == 0) return;
   if (!p->counters.ptr) p->counters.alloc(ctx, 64);
+  pack_batch_keys(p, cols, n);
   PipeParams pp;
   unsigned long long h[4];
   if (p->sink == SINK_BUILD) {
     dfgpu_lookup* t = p->target;
-    t->null_keys += count_null_keys(ctx, cols[p->bkey_col]);
+    if (p->bkey_cols.empty()) t->null_keys += count_null_keys(ctx, cols[p->bkey_col]);   // a composite key's: pack_keys counts them
     if (t->mode == LK_HASH && !t->filter_only && (uint64_t)(t->rows + n) * 2 > t->cap) {
       // the batch may not fit at load factor 0.5 and nobody knows how many rows survive: ONE pass evaluates the pipeline and leaves
       // the survivors as packed {key, payload} records; the table is sized for exactly that many and the records are inserted by a
@@ -2872,6 +2932,13 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     return;
   }
   if (p->sink == SINK_DENSE) { dense_finish(p); return; }
+  if (p->sink == SINK_BUILD && p->key_flags.ptr) {   // a composite build key: what the packing passes saw, read once
+    unsigned long long f[2];
+    DF_CUDA(cudaMemcpyAsync(f, p->key_flags.ptr, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    DF_CUDA(cudaStreamSynchronize(ctx->stream));
+    p->target->null_keys += (int64_t)f[1];
+    if (f[0]) throw Error(DFGPU_ERR_INVALID, "lookup build: a composite key has a component outside its declared domain");
+  }
   if (p->sink != SINK_AGG && p->sink != SINK_HASH) return;
   check_left_build(p);
   LookupDev t;
@@ -2903,6 +2970,7 @@ static void pipeline_finish(dfgpu_pipeline* p) {
   if (dec_avg) { err.alloc(ctx, 8); err.zero(); ec.err = err.as<unsigned long long>(); }
   std::vector<DCol> out;
   const int key_col = p->sink == SINK_AGG ? p->stages[p->agg_stage].key_col : -1;
+  const std::vector<int> no_keys, &comp_cols = p->sink == SINK_AGG ? p->stage_keys[p->agg_stage] : no_keys;
   auto add = [&](int type, bool nullable, EmitCol e) {
     DF_CHECK(ec.n < kMaxPipeCols, DFGPU_ERR_UNSUPPORTED, "pipeline: too many output columns");
     DCol d = alloc_col(ctx, type, groups, nullable);
@@ -2920,7 +2988,13 @@ static void pipeline_finish(dfgpu_pipeline* p) {
   for (int g : p->group_cols) {
     if (p->sink == SINK_HASH) break;
     EmitCol e; memset(&e, 0, sizeof(e));
-    if (g == key_col) { e.kind = 0; add(p->in_types[g], false, e); }
+    const auto comp = std::find(comp_cols.begin(), comp_cols.end(), g);
+    if (comp != comp_cols.end()) {   // a component of the composite key, decoded from the packed key
+      const dfgpu_lookup* l = p->stages[p->agg_stage].lookup;
+      const size_t c = comp - comp_cols.begin();
+      e.kind = 10; e.kmin = l->comp_min[c]; e.cstride = l->comp_stride[c]; e.cradix = l->comp_range[c];
+      add(p->in_types[g], false, e);
+    } else if (g == key_col) { e.kind = 0; add(p->in_types[g], false, e); }
     else { const ExtDef& x = p->exts[g - (int)p->in_types.size()]; e.kind = 1; e.shift = x.shift; add(x.type, false, e); }
   }
   add_agg_columns(p->aggs, p->rows_word, partial, p->left_kind == DFGPU_STAGE_LEFT, add);
@@ -3135,6 +3209,40 @@ int dfgpu_lookup_create(dfgpu_ctx* ctx, int32_t key_type, const int32_t* payload
   *out = l.release();
   DF_API_END
 }
+int dfgpu_lookup_create_composite(dfgpu_ctx* ctx, const int32_t* key_types, const int64_t* key_min, const int64_t* key_max, int32_t n_keys,
+                                  const int32_t* payload_types, int32_t n_payload, const dfgpu_lookup_options* opts, dfgpu_lookup** out) {
+  DF_API_BEGIN(ctx)
+  DF_CHECK(ctx && out && key_types && key_min && key_max, DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(n_keys >= 2 && n_keys <= kMaxKeyParts, DFGPU_ERR_INVALID, "lookup: a composite key has 2..4 components");
+  dfgpu_lookup_options o;
+  if (opts) o = *opts; else dfgpu_lookup_default_options(&o);
+  DF_CHECK(!o.has_key_range, DFGPU_ERR_INVALID, "lookup: a composite key's range is its declared domains (has_key_range must be 0)");
+  // r_g = max_g - min_g + 1, stride_0 = 1, stride_{g+1} = stride_g r_g; D = prod r_g <= 2^63 - 1 (so no packed key is kEmptyKey)
+  std::vector<uint64_t> range(n_keys), stride(n_keys);
+  uint64_t domain = 1;
+  for (int g = 0; g < n_keys; ++g) {
+    DF_CHECK(key_type_ok(key_types[g]), DFGPU_ERR_UNSUPPORTED, "lookup: composite key components must be integer-like columns of <= 64 bits");
+    DF_CHECK(key_min[g] <= key_max[g], DFGPU_ERR_INVALID, "lookup: composite key domain with min > max");
+    DF_CHECK(!type_is_unsigned_int(key_types[g]) || key_min[g] >= 0, DFGPU_ERR_INVALID, "lookup: an unsigned component's domain starts at 0 or above");
+    const uint64_t span = (uint64_t)key_max[g] - (uint64_t)key_min[g];
+    DF_CHECK(span < (uint64_t)INT64_MAX, DFGPU_ERR_UNSUPPORTED, "lookup: the composite key's domain exceeds 2^63 - 1 values");
+    range[g] = span + 1;
+    stride[g] = domain;
+    DF_CHECK(domain <= (uint64_t)INT64_MAX / range[g], DFGPU_ERR_UNSUPPORTED, "lookup: the composite key's domain exceeds 2^63 - 1 values");
+    domain *= range[g];
+  }
+  // the packed key is an Int64 in [0, D - 1]: the bitmap / hash / Bloom rules of dfgpu_lookup_create apply to that range (a filter-only
+  // lookup is a Bloom filter whatever its range)
+  if (!o.filter_only) { o.has_key_range = 1; o.key_min = 0; o.key_max = (int64_t)(domain - 1); }
+  dfgpu_lookup* l = nullptr;
+  const int rc = dfgpu_lookup_create(ctx, DFGPU_INT64, payload_types, n_payload, &o, &l);
+  if (rc != DFGPU_OK) return rc;
+  l->opt.has_key_range = 0;
+  l->comp_types.assign(key_types, key_types + n_keys); l->comp_min.assign(key_min, key_min + n_keys);
+  l->comp_range = range; l->comp_stride = stride; l->domain = domain;
+  *out = l;
+  DF_API_END
+}
 int64_t dfgpu_lookup_metric(dfgpu_lookup* l, const char* name) {
   if (!l || !name) return -1;
   std::string s(name);
@@ -3146,6 +3254,7 @@ int64_t dfgpu_lookup_metric(dfgpu_lookup* l, const char* name) {
   if (s == "rehashes") return l->rehashes;
   if (s == "stride_bytes") return l->stride * 8;
   if (s == "null_keys") return l->null_keys;
+  if (s == "key_domain") return l->comp_types.empty() ? -1 : (int64_t)l->domain;
   return -1;
 }
 int dfgpu_lookup_clear(dfgpu_lookup* l) {
@@ -3258,8 +3367,11 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
     DF_CHECK(!st.lookup->filter_only || st.kind == DFGPU_STAGE_MAYBE, DFGPU_ERR_INVALID, "pipeline: a filter-only lookup can only back a MAYBE stage");
     DF_CHECK(st.key_col >= 0 && st.key_col < n_cols, DFGPU_ERR_INVALID, "pipeline: stage key column out of range");
     const int kt = input_types[st.key_col], lt = st.lookup->key_type;
-    DF_CHECK(key_type_ok(kt) && type_width(kt) == type_width(lt) && type_is_signed_int(kt) == type_is_signed_int(lt), DFGPU_ERR_INVALID,
-             "pipeline: probe key type differs from the lookup's key type");
+    if (!st.lookup->comp_types.empty())   // a composite key: key_col is its first component (dfgpu_pipeline_set_stage_keys names them all)
+      DF_CHECK(kt == st.lookup->comp_types[0], DFGPU_ERR_INVALID, "pipeline: probe key type differs from the lookup's first key component");
+    else
+      DF_CHECK(key_type_ok(kt) && type_width(kt) == type_width(lt) && type_is_signed_int(kt) == type_is_signed_int(lt), DFGPU_ERR_INVALID,
+               "pipeline: probe key type differs from the lookup's key type");
     DF_CHECK(st.lookup->ctx->device == ctx->device, DFGPU_ERR_INVALID, "pipeline: lookup lives on another device");
     p->stages.push_back(st);
     if (st.kind == DFGPU_STAGE_INNER || st.kind == DFGPU_STAGE_LEFT || st.kind == DFGPU_STAGE_LEFT_ANTI)
@@ -3274,15 +3386,22 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
   DF_API_END
 }
 
-int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload) {
-  DF_API_BEGIN(p ? p->ctx : nullptr)
-  DF_CHECK(p && target, DFGPU_ERR_INVALID, "null argument");
-  DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
-  check_no_left_stage(p);
-  DF_CHECK(key_col >= 0 && key_col < (int)p->in_types.size(), DFGPU_ERR_INVALID, "pipeline build sink: the key must be an input column");
-  const int kt = p->in_types[key_col];
-  DF_CHECK(type_width(kt) == type_width(target->key_type) && type_is_signed_int(kt) == type_is_signed_int(target->key_type), DFGPU_ERR_INVALID,
-           "pipeline build sink: key type differs from the lookup's key type");
+// the input columns key_cols[0 .. n_keys) as the components of a composite-key lookup, in order and of the same types (a stage's or the
+// build sink's); the hidden packed columns and the inputs share PipeParams' 16 column slots
+static void check_composite_keys(const dfgpu_pipeline* p, const dfgpu_lookup* l, const int32_t* key_cols, int32_t n_keys, int extra_packed) {
+  DF_CHECK(!l->comp_types.empty(), DFGPU_ERR_INVALID, "pipeline: composite key columns for a lookup with a one-column key");
+  DF_CHECK(key_cols && n_keys == (int)l->comp_types.size(), DFGPU_ERR_INVALID, "pipeline: the key column count differs from the lookup's components");
+  for (int g = 0; g < n_keys; ++g) {
+    DF_CHECK(key_cols[g] >= 0 && key_cols[g] < (int)p->in_types.size(), DFGPU_ERR_INVALID, "pipeline: a composite key component must be an input column");
+    DF_CHECK(p->in_types[key_cols[g]] == l->comp_types[g], DFGPU_ERR_INVALID, "pipeline: a key column's type differs from the lookup's component type");
+  }
+  int packed = extra_packed + (p->bkey_cols.empty() ? 0 : 1);
+  for (int s = 0; s < kMaxStages; ++s) packed += p->stage_keys[s].empty() ? 0 : 1;
+  DF_CHECK((int)p->in_types.size() + packed <= kMaxPipeCols, DFGPU_ERR_UNSUPPORTED,
+           "pipeline: the input columns and the packed composite keys exceed 16 columns");
+}
+
+static void set_build_sink(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload) {
   DF_CHECK(n_payload == (int)target->pay_types.size(), DFGPU_ERR_INVALID, "pipeline build sink: payload column count differs from the lookup's");
   for (int c = 0; c < n_payload; ++c) {
     DF_CHECK(payload_cols[c] >= 0 && payload_cols[c] < (int)p->vtypes.size(), DFGPU_ERR_INVALID, "pipeline build sink: payload column out of range");
@@ -3291,6 +3410,43 @@ int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t k
   }
   for (auto& st : p->stages) DF_CHECK(st.lookup != target, DFGPU_ERR_INVALID, "pipeline: cannot build the lookup it probes");
   p->target = target; p->bkey_col = key_col; p->sink = SINK_BUILD;
+}
+
+int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload) {
+  DF_API_BEGIN(p ? p->ctx : nullptr)
+  DF_CHECK(p && target, DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  check_no_left_stage(p);
+  DF_CHECK(target->comp_types.empty(), DFGPU_ERR_INVALID, "pipeline build sink: a composite-key lookup is built by dfgpu_pipeline_sink_build_composite");
+  DF_CHECK(key_col >= 0 && key_col < (int)p->in_types.size(), DFGPU_ERR_INVALID, "pipeline build sink: the key must be an input column");
+  const int kt = p->in_types[key_col];
+  DF_CHECK(type_width(kt) == type_width(target->key_type) && type_is_signed_int(kt) == type_is_signed_int(target->key_type), DFGPU_ERR_INVALID,
+           "pipeline build sink: key type differs from the lookup's key type");
+  set_build_sink(p, target, key_col, payload_cols, n_payload);
+  DF_API_END
+}
+
+int dfgpu_pipeline_sink_build_composite(dfgpu_pipeline* p, dfgpu_lookup* target, const int32_t* key_cols, int32_t n_keys, const int32_t* payload_cols,
+                                        int32_t n_payload) {
+  DF_API_BEGIN(p ? p->ctx : nullptr)
+  DF_CHECK(p && target, DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
+  check_no_left_stage(p);
+  check_composite_keys(p, target, key_cols, n_keys, 1);
+  set_build_sink(p, target, key_cols[0], payload_cols, n_payload);
+  p->bkey_cols.assign(key_cols, key_cols + n_keys);
+  DF_API_END
+}
+
+int dfgpu_pipeline_set_stage_keys(dfgpu_pipeline* p, int32_t stage, const int32_t* key_cols, int32_t n_keys) {
+  DF_API_BEGIN(p ? p->ctx : nullptr)
+  DF_CHECK(p, DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(stage >= 0 && stage < (int)p->stages.size(), DFGPU_ERR_INVALID, "pipeline stage keys: stage out of range");
+  DF_CHECK(!p->pushed && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline stage keys: set before the first push");
+  DF_CHECK(p->stage_keys[stage].empty(), DFGPU_ERR_STATE, "pipeline stage keys: the stage already has them");
+  check_composite_keys(p, p->stages[stage].lookup, key_cols, n_keys, 1);
+  DF_CHECK(key_cols[0] == p->stages[stage].key_col, DFGPU_ERR_INVALID, "pipeline stage keys: the stage's key_col must be the first component");
+  p->stage_keys[stage].assign(key_cols, key_cols + n_keys);
   DF_API_END
 }
 
@@ -3308,20 +3464,29 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
     DF_CHECK(s == n_stages - 1, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: a LEFT / LEFT_ANTI stage must be the last stage");
     left = s;
   }
-  // functional dependence: every group column is the probe key of ONE inner stage or a payload field of that stage
+  for (int s = 0; s < n_stages; ++s)   // the group columns name a composite key's components
+    DF_CHECK(p->stages[s].lookup->comp_types.empty() || !p->stage_keys[s].empty(), DFGPU_ERR_STATE,
+             "pipeline aggregate: set a composite-key stage's keys (dfgpu_pipeline_set_stage_keys) before this sink");
+  // functional dependence: every group column is the probe key (every component of a composite one) of ONE inner stage or a payload
+  // field of that stage
   const int nin = (int)p->in_types.size();
   int stage = -1;
   for (int s = 0; s < n_stages && stage < 0; ++s) {
     if (left >= 0 ? s != left : p->stages[s].kind != DFGPU_STAGE_INNER) continue;
-    bool has_key = false, ok = true;
+    // the key: the probe key column, or every component of a composite key
+    const std::vector<int> keys = p->stage_keys[s].empty() ? std::vector<int>{p->stages[s].key_col} : p->stage_keys[s];
+    size_t has_keys = 0;
+    bool ok = true;
     for (int g = 0; g < n_group; ++g) {
       const int c = group_cols[g];
       DF_CHECK(c >= 0 && c < (int)p->vtypes.size(), DFGPU_ERR_INVALID, "pipeline aggregate: group column out of range");
-      if (c == p->stages[s].key_col) has_key = true;
+      if (std::find(keys.begin(), keys.end(), c) != keys.end()) has_keys++;
       else if (c >= nin && p->exts[c - nin].stage == (int)s) {}
       else ok = false;
     }
-    if (ok && has_key) stage = (int)s;
+    bool all_keys = true;
+    for (int k : keys) all_keys = all_keys && std::find(group_cols, group_cols + n_group, k) != group_cols + n_group;
+    if (ok && has_keys > 0 && all_keys) stage = (int)s;
   }
   DF_CHECK(stage >= 0, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: group keys are not determined by one join key — use the unfused dfgpu_agg");
   dfgpu_lookup* l = p->stages[stage].lookup;

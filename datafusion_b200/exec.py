@@ -623,7 +623,7 @@ class _Scan:
 
     def __init__(self, source: ExecutionPlan, predicate: Optional[Expr] = None):
         self.source, self.predicate = source, predicate
-        self.stages: List[Tuple[int, str, "GpuPipelineExec"]] = []     # (stage kind, probe key column, build pipeline)
+        self.stages: List[Tuple[int, object, "GpuPipelineExec"]] = []  # (stage kind, probe key column — a list of them for a composite key, build pipeline)
         self.visible: List[str] = [f.name for f in source.schema]       # column names the operators above may still reference
         self.filters: dict = {}                                          # stage index -> its JoinFilter as stage-filter RPN nodes
 
@@ -664,19 +664,55 @@ def _has_fallible_rhs(e: Expr, schema: pa.Schema) -> bool:
     return False
 
 
+_MAX_PIPE_COLS = 16   # input columns plus packed composite keys of one pipeline (dfgpu_pipeline_set_stage_keys)
+
+
+def _key_pairs(pkey, build: "GpuPipelineExec") -> List[Tuple[str, str]]:
+    """(build key, probe key) of every key column of a stage: one pair, or one per component of a composite key"""
+    if isinstance(pkey, list):
+        return list(zip(build.key, pkey))
+    return [(build.key, pkey)]
+
+
+def _integer_like(t: pa.DataType) -> bool:
+    return pa.types.is_integer(t) or pa.types.is_date32(t) or pa.types.is_date64(t) or pa.types.is_timestamp(t)
+
+
+def _join_keys(join: GpuHashJoinExec, sc: _Scan):
+    """(build keys, probe keys) of a join fused as one stage of the probe chain sc: the two names for one key (as they always were), two
+    lists for a composite key of 2..4 pairs, or None.  A composite key needs pairs of the same integer-like Arrow type whose probe keys
+    are source columns of the chain; whether the build keys pack (source columns with known bounds, domain <= 2^63 - 1) is _as_build's
+    decision."""
+    src = [f.name for f in sc.source.schema]
+    if len(join.on) == 1:
+        return join.on[0]
+    if not 2 <= len(join.on) <= 4:
+        return None
+    for b, pk in join.on:
+        if pk not in src or join.left.schema.get_field_index(b) < 0:
+            return None
+        bt, pt = join.left.schema.field(b).type, sc.source.schema.field(pk).type
+        if bt != pt or not _integer_like(bt):
+            return None
+    if len(src) + sum(isinstance(k, list) for _, k, _ in sc.stages) + 1 > _MAX_PIPE_COLS:
+        return None
+    return [b for b, _ in join.on], [pk for _, pk in join.on]
+
+
 def _stage_filter(sc: _Scan, join: GpuHashJoinExec, kind: int, payload: List[str]) -> Optional[list]:
     """The join's JoinFilter as the RPN program of the stage it becomes (appended next to sc.stages), or None when it cannot run there.
     Its columns: a probe-side column -> that column of the probe chain's virtual schema, the build key -> the probe key, any other build
-    column -> the stage's payload field (`payload`, in order; a SEMI / ANTI stage's fields are seen by its filter only)."""
+    column -> the stage's payload field (`payload`, in order; a SEMI / ANTI stage's fields are seen by its filter only).  Each column of
+    a composite key maps to its paired probe key."""
     f = join.filter
     vs = sc.virtual_schema()
     fields = list(vs) + [join.left.schema.field(n) for n in payload]
-    bkey, pkey = join.on[0]
+    paired = dict(join.on)
     where = []
     for side, ix in f.column_indices:
         if side == "left":
             name = join.left.schema.field(ix).name
-            at = vs.get_field_index(pkey) if name == bkey else (len(vs) + payload.index(name) if name in payload else -1)
+            at = vs.get_field_index(paired[name]) if name in paired else (len(vs) + payload.index(name) if name in payload else -1)
         else:
             at = vs.get_field_index(join.right.schema.field(ix).name)   # -1 when missing or ambiguous
         if at < 0:
@@ -696,8 +732,9 @@ def _stage_filter(sc: _Scan, join: GpuHashJoinExec, kind: int, payload: List[str
 
 
 def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]:
-    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner, one key, fusable build)]* over a source.
-    join_filters: a join may carry a JoinFilter, which becomes its stage's filter (fuse_join_filters)"""
+    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner, one key or a composite key
+    (_join_keys), fusable build)]* over a source.  join_filters: a join may carry a JoinFilter, which becomes its stage's filter
+    (fuse_join_filters)"""
     if isinstance(plan, GpuProjectionExec):
         if not all(isinstance(e, Column) and e.name == name for e, name in plan.exprs):
             return None
@@ -716,28 +753,31 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]
             sc.visible = [inner.schema.field(i).name for i in plan.projection]
         return sc
     if isinstance(plan, GpuHashJoinExec):
-        if plan.join_type not in ("RightSemi", "RightAnti", "Inner") or len(plan.on) != 1 or (plan.filter is not None and not join_filters) or \
+        if plan.join_type not in ("RightSemi", "RightAnti", "Inner") or (plan.filter is not None and not join_filters) or \
                 plan.null_aware or plan.null_equality != "NullEqualsNothing":
             return None
         sc = _as_scan(plan.right, join_filters)
-        if sc is None or plan.on[0][1] not in [f.name for f in sc.source.schema]:
+        keys = None if sc is None else _join_keys(plan, sc)
+        if keys is None or (isinstance(keys[1], str) and keys[1] not in [f.name for f in sc.source.schema]):
             return None
+        bkey, pkey = keys
+        bkeys = bkey if isinstance(bkey, list) else [bkey]
         kind = {"RightSemi": D.STAGE_SEMI, "RightAnti": D.STAGE_ANTI, "Inner": D.STAGE_INNER}[plan.join_type]
-        payload = [f.name for f in plan.left.schema if f.name != plan.on[0][0]] if kind == D.STAGE_INNER else []
+        payload = [f.name for f in plan.left.schema if f.name not in bkeys] if kind == D.STAGE_INNER else []
         if plan.filter is not None and kind != D.STAGE_INNER:   # a semi / anti lookup carries the build columns its filter reads
             read = {plan.left.schema.field(ix).name for sd, ix in plan.filter.column_indices if sd == "left"}
-            payload = [f.name for f in plan.left.schema if f.name != plan.on[0][0] and f.name in read]
+            payload = [f.name for f in plan.left.schema if f.name not in bkeys and f.name in read]
         filt = None
         if plan.filter is not None:
             filt = _stage_filter(sc, plan, kind, payload)
             if filt is None:
                 return None
-        build = _as_build(plan.left, plan.on[0][0], payload, join_filters)
+        build = _as_build(plan.left, bkey, payload, join_filters)
         if build is None:
             return None
         if filt is not None:
             sc.filters[len(sc.stages)] = filt
-        sc.stages.append((kind, plan.on[0][1], build))
+        sc.stages.append((kind, pkey, build))
         names = [f.name for f in plan.schema]
         sc.visible = names
         return sc
@@ -746,17 +786,35 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]
     return _Scan(plan)
 
 
-def _as_build(plan: ExecutionPlan, key: str, payload: List[str], join_filters: bool = False) -> Optional["GpuPipelineExec"]:
+def _as_build(plan: ExecutionPlan, key, payload: List[str], join_filters: bool = False) -> Optional["GpuPipelineExec"]:
+    """the build pipeline of a fused join on `key` (a list of columns for a composite key: source columns with known bounds
+    (_source_bounds) whose domain, the product of max - min + 1, is at most 2^63 - 1, so that the tuple packs into one 64-bit key)"""
     sc = _as_scan(plan, join_filters)
     if sc is None or len(sc.stages) >= 3:
         return None
     vs = sc.virtual_schema()
-    if vs.get_field_index(key) < 0 or vs.get_field_index(key) >= len(sc.source.schema) or any(vs.get_field_index(n) < 0 for n in payload):
+    keys = key if isinstance(key, list) else [key]
+    if any(vs.get_field_index(k) < 0 or vs.get_field_index(k) >= len(sc.source.schema) for k in keys) or any(vs.get_field_index(n) < 0 for n in payload):
         return None
     bits = sum(D.WIDTH[type_id(vs.field(n).type)] * 8 for n in payload)
     if bits > 64:
         return None
-    return GpuPipelineExec(sc, sink="build", key=key, payload=payload)
+    ranges = []
+    if isinstance(key, list):
+        if len(sc.source.schema) + sum(isinstance(k, list) for _, k, _ in sc.stages) + 1 > _MAX_PIPE_COLS:
+            return None
+        dom = 1
+        for k in keys:
+            b = _source_bounds(sc.source, k)
+            if b is None:
+                return None
+            dom *= b[1] - b[0] + 1
+            ranges.append(b)
+        if dom > (1 << 63) - 1:
+            return None
+    build = GpuPipelineExec(sc, sink="build", key=key, payload=payload)
+    build.key_ranges = ranges
+    return build
 
 
 class GpuPipelineExec(ExecutionPlan):
@@ -774,6 +832,7 @@ class GpuPipelineExec(ExecutionPlan):
         self.fallback = fallback           # output sink: the unfused plan, run when a build side cannot be fused (_execute_output)
         self.schema = out_schema if out_schema is not None else pa.schema([])
         self.n_acc_words = 0
+        self.key_ranges: List[Tuple[int, int]] = []   # build sink of a composite key: the declared (min, max) of every component
         self._metrics = {}
 
     def children(self): return [self.scan.source] + [b for _, _, b in self.scan.stages]
@@ -784,6 +843,10 @@ class GpuPipelineExec(ExecutionPlan):
     def build_lookup(self, ctx: TaskContext) -> D.Lookup:
         vs = self.scan.virtual_schema()
         batches = list(self.scan.source.execute(ctx))
+        if isinstance(self.key, list):
+            look = D.Lookup(ctx.gpu, key_types=[type_id(vs.field(k).type) for k in self.key], key_ranges=self.key_ranges,
+                            payload_types=[type_id(vs.field(n).type) for n in self.payload], n_acc_words=self.n_acc_words)
+            return self._run_build(ctx, look, batches, dict(key_cols=[vs.get_field_index(k) for k in self.key]))
         key_range = None
         ktype = vs.field(self.key).type
         if not self.payload and self.n_acc_words == 0 and pa.types.is_integer(ktype) and batches:   # statistics: the bounds collect_left_input tracks
@@ -793,13 +856,17 @@ class GpuPipelineExec(ExecutionPlan):
             if lo:
                 key_range = (min(lo), max(hi))
         look = D.Lookup(ctx.gpu, type_id(ktype), [type_id(vs.field(n).type) for n in self.payload], key_range=key_range, n_acc_words=self.n_acc_words)
+        return self._run_build(ctx, look, batches, dict(key_col=vs.get_field_index(self.key)))
+
+    def _run_build(self, ctx: TaskContext, look: D.Lookup, batches, key: dict) -> D.Lookup:
+        vs = self.scan.virtual_schema()
         try:
             pipe, keep = self._make_pipeline(ctx)
         except BaseException:
             look.close()
             raise
         try:
-            pipe.sink_build(look, vs.get_field_index(self.key), [vs.get_field_index(n) for n in self.payload])
+            pipe.sink_build(look, payload_cols=[vs.get_field_index(n) for n in self.payload], **key)
             for rb in batches:
                 pipe.push_arrow(rb)
             pipe.finish()
@@ -824,7 +891,7 @@ class GpuPipelineExec(ExecutionPlan):
             for kind, pkey, build in self.scan.stages:
                 look = build.build_lookup(ctx)                  # the pipeline breaker: WaitBuildSide (hash_join/stream.rs:117-140)
                 keep.append(look)
-                stages.append((kind, ssch.get_field_index(pkey), look))
+                stages.append((kind, [ssch.get_field_index(k) for k in pkey] if isinstance(pkey, list) else ssch.get_field_index(pkey), look))
         except BaseException:
             for l in keep:
                 l.close()
@@ -1044,17 +1111,19 @@ def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False) -> Execution
     kind, pkey, build = sc.stages[-1]
     vs = sc.virtual_schema()
     exprs = {name: e for e, name in proj.exprs} if proj is not None else {f.name: Column(f.name) for f in below.schema}
-    # group keys: the probe key (or the equal build key) and payload fields of the LAST inner stage
+    # group keys: the probe key (or the equal build key; every component of a composite key) and payload fields of the LAST inner stage
+    paired = dict(_key_pairs(pkey, build))
+    pkeys = list(paired.values())
     group = []
     for g in plan.group_by:
         e = exprs.get(g)
         if not isinstance(e, Column):
             return plan
-        n = pkey if e.name == build.key else e.name
-        if n != pkey and n not in build.payload:
+        n = paired.get(e.name, e.name)
+        if n not in pkeys and n not in build.payload:
             return plan
         group.append(n)
-    if pkey not in group:
+    if any(k not in group for k in pkeys):
         return plan
     aggs = []
     for a in plan.aggr_expr:
@@ -1082,22 +1151,27 @@ def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False) -> Execution
 
 
 def _left_join_scan(join: GpuHashJoinExec, kind: int, join_filters: bool = False) -> Optional[_Scan]:
-    """The probe chain of a Left / LeftSemi / LeftAnti join with the join as its last stage (kind), or None.  Conditions: one key, no
-    JoinFilter, NullEqualsNothing, not null-aware; the right side is an _as_scan chain probing on one of its source columns; the left side
-    is a fusable build whose key field is declared non-nullable (a NULL build key is never in the lookup, but Left / LeftAnti emit its row)
-    and has the probe key's type.  The build's payload is every other left column.  join_filters: a JoinFilter is allowed and becomes the
-    stage's filter."""
-    if len(join.on) != 1 or (join.filter is not None and not join_filters) or join.null_aware or join.null_equality != "NullEqualsNothing":
+    """The probe chain of a Left / LeftSemi / LeftAnti join with the join as its last stage (kind), or None.  Conditions: one key or a
+    composite key (_join_keys), no JoinFilter, NullEqualsNothing, not null-aware; the right side is an _as_scan chain probing on its
+    source columns; the left side is a fusable build whose key fields are declared non-nullable (a NULL build key is never in the lookup,
+    but Left / LeftAnti emit its row) and have the probe keys' types.  The build's payload is every other left column.  join_filters: a
+    JoinFilter is allowed and becomes the stage's filter."""
+    if (join.filter is not None and not join_filters) or join.null_aware or join.null_equality != "NullEqualsNothing":
         return None
-    bkey, pkey = join.on[0]
     sc = _as_scan(join.right, join_filters)
+    keys = None if sc is None or len(sc.stages) >= 3 else _join_keys(join, sc)
+    if keys is None:
+        return None
+    bkey, pkey = keys
     ls = join.left.schema
-    if sc is None or len(sc.stages) >= 3 or sc.source.schema.get_field_index(pkey) < 0 or ls.get_field_index(bkey) < 0:
-        return None
-    kf = ls.field(bkey)
-    if kf.nullable or kf.type != sc.source.schema.field(pkey).type:
-        return None
-    payload = [f.name for f in ls if f.name != bkey]
+    for b, pk in (zip(bkey, pkey) if isinstance(bkey, list) else [(bkey, pkey)]):
+        if sc.source.schema.get_field_index(pk) < 0 or ls.get_field_index(b) < 0:
+            return None
+        kf = ls.field(b)
+        if kf.nullable or kf.type != sc.source.schema.field(pk).type:
+            return None
+    bkeys = bkey if isinstance(bkey, list) else [bkey]
+    payload = [f.name for f in ls if f.name not in bkeys]
     filt = None
     if join.filter is not None:
         filt = _stage_filter(sc, join, kind, payload)
@@ -1122,13 +1196,14 @@ def _fuse_left(plan: "GpuAggregateExec", join: GpuHashJoinExec, proj: Optional[G
     _, pkey, build = sc.stages[-1]
     vs = sc.virtual_schema()
     exprs = {name: e for e, name in proj.exprs} if proj is not None else {f.name: Column(f.name) for f in join.schema}
+    paired = dict(_key_pairs(pkey, build))
     group = []
     for g in plan.group_by:
         e = exprs.get(g)
-        if not isinstance(e, Column) or (e.name != build.key and e.name not in build.payload):
+        if not isinstance(e, Column) or (e.name not in paired and e.name not in build.payload):
             return None
-        group.append(pkey if e.name == build.key else e.name)
-    if pkey not in group:
+        group.append(paired.get(e.name, e.name))
+    if any(k not in group for k in paired.values()):
         return None
     n_src, left_payload = len(sc.source.schema), range(len(vs) - len(build.payload), len(vs))
     aggs, types = [], []
@@ -1172,7 +1247,8 @@ def _fuse_left_filter(join: GpuHashJoinExec, join_filters: bool = False) -> Opti
     if sc is None:
         return None
     _, pkey, build = sc.stages[-1]
-    group = [pkey if f.name == build.key else f.name for f in join.left.schema]
+    paired = dict(_key_pairs(pkey, build))
+    group = [paired.get(f.name, f.name) for f in join.left.schema]
     build.n_acc_words = _acc_words([], [], bool(build.payload))
     project = [i for _, i in join.column_indices]          # the join's projection: left columns only
     if project == list(range(len(group))):
@@ -1199,7 +1275,9 @@ def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False) -> Exe
     if not ((isinstance(below, GpuHashJoinExec) and below.join_type == "Inner") or isinstance(below, GpuFilterExec)):
         return plan
     sc = _as_scan(below, join_filters)
-    if sc is None:
+    # a composite-key stage under the hash-keyed sink (TPC-H Q9's lineitem x partsupp profit by supplier) measured slower than the
+    # unfused dfgpu_hashjoin -> dfgpu_agg (README): that shape stays unfused
+    if sc is None or any(isinstance(k, list) for _, k, _ in sc.stages):
         return plan
     vs = sc.virtual_schema()
     exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
@@ -1275,7 +1353,7 @@ def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     vs = sc.virtual_schema()
     kind, pkey, build = sc.stages[-1]
     n_below = len(vs) - (len(build.payload) if kind == D.STAGE_INNER else 0)   # the virtual columns the top join's probe side sees
-    keys = {b.key: (p, b) for k, p, b in sc.stages if k == D.STAGE_INNER}       # an Inner stage's build key -> its probe key
+    keys = {bk: (pk, b) for k, p, b in sc.stages if k == D.STAGE_INNER for bk, pk in _key_pairs(p, b)}   # an Inner stage's build key -> its probe key
 
     def probe_col(name: str) -> int:
         at = [i for i in range(n_below) if vs.field(i).name == name]
@@ -1299,8 +1377,9 @@ def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
             at = probe_col(join.right.schema.field(ix).name)
         else:
             name = join.left.schema.field(ix).name
-            if name == join.on[0][0]:
-                at = probe_col(pkey)
+            paired = dict(_key_pairs(pkey, build))
+            if name in paired:
+                at = probe_col(paired[name])
                 at = at if at >= 0 and join.left.schema.field(ix).type == vs.field(at).type else -1
             else:
                 at = n_below + build.payload.index(name) if name in build.payload else -1

@@ -429,6 +429,25 @@ void dfgpu_lookup_default_options(dfgpu_lookup_options* o);
  * ArrayMap idea, exec.rs:111-191, at one bit per key). */
 int dfgpu_lookup_create(dfgpu_ctx* ctx, int32_t key_type, const int32_t* payload_types, int32_t n_payload,
                         const dfgpu_lookup_options* opts, dfgpu_lookup** out);
+/* Composite keys: a join on n_keys = 2..4 key columns (TPC-H Q9's (ps_partkey, ps_suppkey)) whose values have declared domains
+ * [key_min[g], key_max[g]] (column statistics: the per-column bounds collect_left_input tracks, exec.rs:2585-2619).
+ *  Components: integer-like types (Int8..Int64, UInt8..UInt64, Date32, Date64, Timestamp, dictionary codes as Int32); key_min[g] <=
+ *    key_max[g] (an unsigned component's key_min >= 0), else DFGPU_ERR_INVALID.
+ *  Packing: r_g = key_max[g] - key_min[g] + 1, D = prod_g r_g; the packed key is sum_g (v_g - key_min[g]) * stride_g with stride_0 = 1,
+ *    stride_{g+1} = stride_g * r_g, a bijection of the in-domain tuples onto [0, D - 1].  D > 2^63 - 1 is DFGPU_ERR_UNSUPPORTED (such
+ *    joins stay on dfgpu_hashjoin's wide-key path).  The lookup is a lookup of that Int64 key: the bitmap / hash / Bloom rules of
+ *    dfgpu_lookup_create apply to the range [0, D - 1] (a key set with a small D becomes a bitmap); "unique keys" means unique tuples.
+ *    opts->has_key_range must be 0 (DFGPU_ERR_INVALID).  dfgpu_lookup_metric(l, "key_domain") returns D (-1 for a one-column key).
+ *  Probe side (dfgpu_pipeline_set_stage_keys): a row with a NULL component, or a component outside its domain, packs to the sentinel D,
+ *    which no lookup holds: it matches nothing in INNER / SEMI / LEFT / LEFT_ANTI / MAYBE stages and is kept by ANTI stages, as a NULL
+ *    key is (NullEqualsNothing, utils.rs:2146-2155).
+ *  Build side (dfgpu_pipeline_sink_build_composite): a row with a NULL component has a NULL key: not inserted, counted in "null_keys".
+ *    A row with a non-NULL component outside its domain is not inserted either, and the build pipeline's dfgpu_pipeline_finish returns
+ *    DFGPU_ERR_INVALID (like the dense sink's key outside its declared range).  Both are judged on every pushed row, before the predicate.
+ *  Each push packs its keys in one extra pass (timed as "pipe_keys:<name>", next to "pipe:<name>"): 8 bytes per row and key are written
+ *    and read again by the pipeline kernel. */
+int dfgpu_lookup_create_composite(dfgpu_ctx* ctx, const int32_t* key_types, const int64_t* key_min, const int64_t* key_max, int32_t n_keys,
+                                  const int32_t* payload_types, int32_t n_payload, const dfgpu_lookup_options* opts, dfgpu_lookup** out);
 /* forget every record / key / filter bit, keep the allocations (a persistent build side refilled per query) */
 int dfgpu_lookup_clear(dfgpu_lookup* l);
 /* the membership filter as raw 64-bit blocks (device pointer + size): exported with dfgpu_ipc_export for the peer all-reduce below */
@@ -504,6 +523,12 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
  *              every other sink over a LEFT / LEFT_ANTI stage is DFGPU_ERR_UNSUPPORTED;
  *  output    : surviving rows, columns = out_cols of the virtual schema, input order preserved. */
 int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload);
+/* the build sink of a composite-key lookup (dfgpu_lookup_create_composite): key = the packed tuple of the INPUT columns key_cols[0..n_keys),
+ * of the lookup's component types in order (else DFGPU_ERR_INVALID); payload as for dfgpu_pipeline_sink_build.  The packed keys are
+ * hidden columns behind the inputs: input columns plus packed keys (this one and one per composite stage) must not exceed 16
+ * (DFGPU_ERR_UNSUPPORTED). */
+int dfgpu_pipeline_sink_build_composite(dfgpu_pipeline* p, dfgpu_lookup* target, const int32_t* key_cols, int32_t n_keys,
+                                        const int32_t* payload_cols, int32_t n_payload);
 int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, int32_t n_group,
                                   const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size);
 /* dense aggregate: AggregateExec over the surviving rows whose 0..8 group columns (virtual columns: input columns or payload
@@ -575,6 +600,15 @@ int dfgpu_pipeline_sink_output_unordered(dfgpu_pipeline* p, const int32_t* out_c
  * IS [NOT] NULL are accepted anywhere); more than 128 nodes over all filters of the pipeline.  A pipeline with a stage filter runs
  * neither the ring-fed nor the partitioned aggregate pass ("ring_launches" and "partitioned_launches" stay 0). */
 int dfgpu_pipeline_set_stage_filter(dfgpu_pipeline* p, int32_t stage, const dfgpu_expr_node* expr, int32_t n_nodes);
+/* Composite key of probe stage `stage`, whose lookup came from dfgpu_lookup_create_composite: the stage probes with the packed tuple of
+ * the INPUT columns key_cols[0..n_keys) (components taken from payload fields of earlier stages are not supported).  Their types must be
+ * the lookup's component types in order, and the stage's key_col must be key_cols[0] (DFGPU_ERR_INVALID); input columns plus packed keys
+ * must not exceed 16 (DFGPU_ERR_UNSUPPORTED).  Call after dfgpu_pipeline_create, before the join-keyed aggregate sink and before the
+ * first push (DFGPU_ERR_STATE otherwise, and for a second call on the stage); a push through a composite-key stage without its keys is
+ * DFGPU_ERR_STATE.  The join-keyed aggregate sink then groups on ALL the components (plus payload fields of the stage): they are
+ * decoded from the record's packed key, (key / stride_g) % r_g + key_min[g], at the component's type; for LEFT / LEFT_ANTI they are the
+ * build key's components, never NULL.  The dense, hash and output sinks take the components as ordinary input columns. */
+int dfgpu_pipeline_set_stage_keys(dfgpu_pipeline* p, int32_t stage, const int32_t* key_cols, int32_t n_keys);
 /* optional label: this pipeline's kernel is timed under the family "pipe:<name>" (dfgpu_set_kernel_timing / dfgpu_kernel_time) —
  * the per-operator metrics set of a plan node (metrics(), execution_plan.rs:713) */
 int dfgpu_pipeline_set_name(dfgpu_pipeline* p, const char* name);
