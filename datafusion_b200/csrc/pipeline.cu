@@ -1784,6 +1784,65 @@ __global__ void __launch_bounds__(256) lookup_emit_kernel(LookupDev t, const uin
   }
 }
 
+// lookup_groups_kernel (sel 0) -> compact -> lookup_emit_kernel in one pass over the table, for emissions whose every column is a word of
+// the record (kinds 0, 1, 4, and 2 without a non-null counter or a Float64 key) without a validity bitmap: each 1024-slot tile finds its
+// records with a non-zero rows_word, ranks them in slot order (ballots, then decoupled look-back across tiles taken in order), and writes
+// their columns at those ranks, so the groups come out in the order of the three-kernel path.  The table is read once, with no bitmap,
+// index array or host round trip in between.  total[0]: the group count; the columns hold max_out rows, and rows past them are not written.
+__global__ void __launch_bounds__(256) lookup_scan_emit_kernel(LookupDev t, int rows_word, EmitCols ec, unsigned int* __restrict__ tile_counter,
+                                                               unsigned long long* __restrict__ tile_desc, unsigned long long* __restrict__ total, uint64_t max_out) {
+  constexpr int ITEMS = 4, TILE = 256 * ITEMS;
+  __shared__ unsigned int s_tile;
+  __shared__ uint32_t s_rank[ITEMS * 8];   // exclusive rank of (item k, warp w) at [k * 8 + w]
+  __shared__ unsigned long long s_base;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint64_t ntiles = (t.cap + TILE - 1) / TILE;
+  while (true) {
+    __syncthreads();
+    if (threadIdx.x == 0) s_tile = atomicAdd(tile_counter, 1u);   // tiles in slot order: look-back waits on earlier tiles only
+    __syncthreads();
+    const uint64_t tile = s_tile;
+    if (tile >= ntiles) break;
+    unsigned bal[ITEMS];
+    bool occ[ITEMS];
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const uint64_t slot = tile * TILE + k * 256 + threadIdx.x;
+      occ[k] = slot < t.cap && t.recs[slot * (uint64_t)t.stride + rows_word] != 0ull;
+      bal[k] = __ballot_sync(0xffffffffu, occ[k]);
+      if (lane == 0) s_rank[k * 8 + warp] = __popc(bal[k]);
+    }
+    __syncthreads();
+    if (warp == 0) {
+      const uint32_t c = s_rank[lane];
+      uint32_t inc = c;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, inc, d); if (lane >= d) inc += v; }
+      s_rank[lane] = inc - c;
+      const uint32_t tot = __shfl_sync(0xffffffffu, inc, 31);
+      const unsigned long long ex = tile_lookback((int64_t)tile, tot, tile_desc);
+      if (lane == 0) { s_base = ex; if (tile == ntiles - 1) total[0] = ex + tot; }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < ITEMS; ++k) {
+      const uint64_t i = s_base + s_rank[k * 8 + warp] + __popc(bal[k] & ((1u << lane) - 1u));
+      if (!occ[k] || i >= max_out) continue;
+      const unsigned long long* r = t.recs + (tile * TILE + k * 256 + threadIdx.x) * (uint64_t)t.stride;
+      for (int c = 0; c < ec.n; ++c) {
+        const EmitCol& e = ec.c[c];
+        const uint64_t v = e.kind == 0 ? r[0] : (e.kind == 1 ? r[1] >> e.shift : r[e.word]);
+        switch (e.width) {
+          case 1: ((uint8_t*)e.dst)[i] = (uint8_t)v; break;
+          case 2: ((uint16_t*)e.dst)[i] = (uint16_t)v; break;
+          case 4: ((uint32_t*)e.dst)[i] = (uint32_t)v; break;
+          default: ((uint64_t*)e.dst)[i] = v; break;
+        }
+      }
+    }
+  }
+}
+
 // OR-all-reduce of n_ranks membership filters of identical geometry over peer memory (NVLink): this rank merges slice
 // `rank` of every filter (reads of the peers' slices travel over NVLink) and writes the merged slice into every rank's
 // filter.  Slice r of rank q's buffer is read only by rank r, and written by rank r only after it has read it.
@@ -2951,14 +3010,24 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     memset(&t, 0, sizeof(t));
     t.recs = p->hash_recs.as<unsigned long long>(); t.cap = p->hash_cap + 1; t.stride = p->hash_stride;
   }
-  const uint64_t nw = (t.cap + 31) / 32;
-  DevBuf words(ctx, (size_t)nw * 4 + 8), idx;
   const int sel = p->left_kind == DFGPU_STAGE_LEFT ? 2 : (p->left_kind == DFGPU_STAGE_LEFT_ANTI ? 1 : 0);
-  lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, p->rows_word, sel, words.as<uint32_t>());
-  DF_LAUNCH_CHECK(ctx);
-  const int64_t groups = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)t.cap, 1, &idx);
-  p->m_groups = groups;
-  if (groups == 0) return;
+  // the join-keyed sink's groups are at most the lookup's records: columns of that length let lookup_scan_emit_kernel find and emit the
+  // groups in one pass, when every column is one it emits
+  const bool try_scan = p->sink == SINK_AGG && sel == 0;
+  int64_t groups = try_scan ? p->stages[p->agg_stage].lookup->rows : 0;
+  DevBuf idx;
+  auto scan_groups = [&]() {
+    const uint64_t nw = (t.cap + 31) / 32;
+    DevBuf words(ctx, (size_t)nw * 4 + 8);
+    lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, p->rows_word, sel, words.as<uint32_t>());
+    DF_LAUNCH_CHECK(ctx);
+    groups = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)t.cap, 1, &idx);
+  };
+  if (!try_scan) {
+    scan_groups();
+    p->m_groups = groups;
+    if (groups == 0) return;
+  }
   // output schema: group columns, then one (Single) or the state (Partial) columns per aggregate
   const bool partial = p->agg_mode == DFGPU_AGG_PARTIAL;
   EmitCols ec;
@@ -2979,27 +3048,60 @@ static void pipeline_finish(dfgpu_pipeline* p) {
     ec.c[ec.n++] = e;
     out.push_back(std::move(d));
   };
-  for (size_t k = 0; k < p->hash_keys.size(); ++k) {   // hash sink: the fields of the packed tag
-    const HashKey& hk = p->hash_keys[k];
-    EmitCol e; memset(&e, 0, sizeof(e));
-    e.kind = 8; e.shift = hk.shift; e.tag_null = hk.null_bit;
-    add(p->vtypes[hk.src], hk.null_bit >= 0, e);
+  auto add_columns = [&]() {
+    for (size_t k = 0; k < p->hash_keys.size(); ++k) {   // hash sink: the fields of the packed tag
+      const HashKey& hk = p->hash_keys[k];
+      EmitCol e; memset(&e, 0, sizeof(e));
+      e.kind = 8; e.shift = hk.shift; e.tag_null = hk.null_bit;
+      add(p->vtypes[hk.src], hk.null_bit >= 0, e);
+    }
+    for (int g : p->group_cols) {
+      if (p->sink == SINK_HASH) break;
+      EmitCol e; memset(&e, 0, sizeof(e));
+      const auto comp = std::find(comp_cols.begin(), comp_cols.end(), g);
+      if (comp != comp_cols.end()) {   // a component of the composite key, decoded from the packed key
+        const dfgpu_lookup* l = p->stages[p->agg_stage].lookup;
+        const size_t c = comp - comp_cols.begin();
+        e.kind = 10; e.kmin = l->comp_min[c]; e.cstride = l->comp_stride[c]; e.cradix = l->comp_range[c];
+        add(p->in_types[g], false, e);
+      } else if (g == key_col) { e.kind = 0; add(p->in_types[g], false, e); }
+      else { const ExtDef& x = p->exts[g - (int)p->in_types.size()]; e.kind = 1; e.shift = x.shift; add(x.type, false, e); }
+    }
+    add_agg_columns(p->aggs, p->rows_word, partial, p->left_kind == DFGPU_STAGE_LEFT, add);
+  };
+  add_columns();
+  bool scan = try_scan && !dec_avg;
+  for (int c = 0; c < ec.n && scan; ++c) {
+    const EmitCol& e = ec.c[c];
+    scan = !e.valid && (e.kind == 0 || e.kind == 1 || e.kind == 4 || (e.kind == 2 && e.nn_word < 0 && !e.f64_key));
   }
-  for (int g : p->group_cols) {
-    if (p->sink == SINK_HASH) break;
-    EmitCol e; memset(&e, 0, sizeof(e));
-    const auto comp = std::find(comp_cols.begin(), comp_cols.end(), g);
-    if (comp != comp_cols.end()) {   // a component of the composite key, decoded from the packed key
-      const dfgpu_lookup* l = p->stages[p->agg_stage].lookup;
-      const size_t c = comp - comp_cols.begin();
-      e.kind = 10; e.kmin = l->comp_min[c]; e.cstride = l->comp_stride[c]; e.cradix = l->comp_range[c];
-      add(p->in_types[g], false, e);
-    } else if (g == key_col) { e.kind = 0; add(p->in_types[g], false, e); }
-    else { const ExtDef& x = p->exts[g - (int)p->in_types.size()]; e.kind = 1; e.shift = x.shift; add(x.type, false, e); }
+  if (scan) {
+    const uint64_t ntiles = (t.cap + 1023) / 1024;
+    DevBuf desc(ctx, (size_t)(ntiles + 2) * 8);   // tile descriptors, then the tile counter and the group count
+    desc.zero();
+    unsigned long long* d = desc.as<unsigned long long>();
+    lookup_scan_emit_kernel<<<kNumSMs * 8, 256, 0, ctx->stream>>>(t, p->rows_word, ec, (unsigned int*)(d + ntiles), d, d + ntiles + 1, (uint64_t)groups);
+    DF_LAUNCH_CHECK(ctx);
+    const int64_t found = (int64_t)read_scalar(ctx, d + ntiles + 1);
+    scan = found <= groups;   // more records reached than the lookup holds rows: emit through the index path instead
+    if (scan) {
+      groups = found;
+      for (DCol& c : out) c.length = groups;
+      p->m_groups = groups;
+      if (groups == 0) return;
+    }
   }
-  add_agg_columns(p->aggs, p->rows_word, partial, p->left_kind == DFGPU_STAGE_LEFT, add);
-  lookup_emit_kernel<<<grid_for(groups, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), groups, p->rows_word, ec);
-  DF_LAUNCH_CHECK(ctx);
+  if (!scan) {
+    if (try_scan) {   // an emission the single pass does not make: the columns again, at the group count
+      out.clear(); ec.n = 0;
+      scan_groups();
+      p->m_groups = groups;
+      if (groups == 0) return;
+      add_columns();
+    }
+    lookup_emit_kernel<<<grid_for(groups, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), groups, p->rows_word, ec);
+    DF_LAUNCH_CHECK(ctx);
+  }
   if (dec_avg) {
     unsigned long long h_err = 0;
     DF_CUDA(cudaMemcpyAsync(&h_err, err.ptr, 8, cudaMemcpyDeviceToHost, ctx->stream));
