@@ -28,7 +28,7 @@ NULL_EQUALS_NOTHING, NULL_EQUALS_NULL = 0, 1
 
 AGG_PARTIAL, AGG_FINAL, AGG_FINAL_PARTITIONED, AGG_SINGLE, AGG_SINGLE_PARTITIONED, AGG_PARTIAL_REDUCE = range(6)
 AGG_SUM, AGG_COUNT, AGG_MIN, AGG_MAX, AGG_AVG, AGG_COUNT_STAR = range(1, 7)
-STAGE_INNER, STAGE_SEMI, STAGE_ANTI, STAGE_MAYBE, STAGE_LEFT, STAGE_LEFT_ANTI = range(6)
+STAGE_INNER, STAGE_SEMI, STAGE_ANTI, STAGE_MAYBE, STAGE_LEFT, STAGE_LEFT_ANTI, STAGE_RIGHT = range(7)
 DENSE_MAX_GROUPS = 256   # DFGPU_DENSE_MAX_GROUPS: slots of a dense aggregate's key domain
 
 GEN_SEQ, GEN_UNIFORM, GEN_SPLITMIX, GEN_PERM, GEN_SPARSE_OF = range(5)

@@ -227,7 +227,8 @@ __device__ __forceinline__ i128 cast_value_dec(const ENode& nd, i128 v, bool val
   return (i128)(u128)(uint64_t)wrap_to_type((uint64_t)q, to);
 }
 
-// one row of a program that touches decimals: value (128 bits) + validity
+// one row of a program that touches decimals: value (128 bits) + validity; XN: nullable payload fields (expr_dev.cuh)
+template <bool XN = false>
 __device__ __forceinline__ i128 eval_nodes_dec(const ENode* __restrict__ nodes, int n_nodes, int64_t row, bool* ok_out, int* err, const uint64_t* ext = nullptr) {
   i128 sv[kMaxStack];
   bool sk[kMaxStack];
@@ -252,7 +253,7 @@ __device__ __forceinline__ i128 eval_nodes_dec(const ENode* __restrict__ nodes, 
         const int w = type_width(nd.out_type);
         if (w < 8) { v &= (1ull << (8 * w)) - 1ull; if (type_is_signed_int(nd.out_type)) v = (uint64_t)(((int64_t)(v << (64 - 8 * w))) >> (64 - 8 * w)); }
         if (nd.out_type == DFGPU_FLOAT32) { float f = __uint_as_float((uint32_t)v); v = (uint64_t)__double_as_longlong((double)f); }
-        sk[sp] = true; sv[sp] = (i128)(u128)v; ++sp;
+        sk[sp] = XN ? ((ext[kExtValid] >> nd.voff) & 1ull) != 0 : true; sv[sp] = (i128)(u128)v; ++sp;
         break;
       }
       case DFGPU_EXPR_BINARY: {

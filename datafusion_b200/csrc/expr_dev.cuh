@@ -10,6 +10,9 @@ namespace dfgpu {
 // internal node kind (never crosses the C ABI): a field of a 64-bit payload word fetched by a fused join probe.
 // voff = index of the payload word in the per-row `ext` array, lit = bit shift, out_type = field type.
 constexpr int kExprExt = 100;
+// The interpreters' XN parameter (nullable payload fields: the fused pipeline's RIGHT stages): ext[kExtValid], behind the payload words,
+// holds the row's validity bits, bit s = the fields of payload word s are valid.  Without XN a payload field is never NULL.
+constexpr int kExtValid = 3;
 
 constexpr int kMaxNodes = 48;
 constexpr int kMaxStack = 16;
@@ -214,6 +217,7 @@ __device__ __forceinline__ uint64_t cast_value(uint64_t v, int from, int to, boo
 }
 
 // evaluate the post-order program for one row: value bits + validity
+template <bool XN = false>
 __device__ __forceinline__ uint64_t eval_nodes(const ENode* __restrict__ nodes, int n_nodes, int64_t row, bool* ok_out, int* err, const uint64_t* ext = nullptr) {
   uint64_t sv[kMaxStack];
   bool sk[kMaxStack];
@@ -235,7 +239,7 @@ __device__ __forceinline__ uint64_t eval_nodes(const ENode* __restrict__ nodes, 
     const int w = type_width_prim(nd.out_type);
     if (w < 8) { v &= (1ull << (8 * w)) - 1ull; if (type_is_signed_int(nd.out_type)) v = (uint64_t)(((int64_t)(v << (64 - 8 * w))) >> (64 - 8 * w)); }
     if (nd.out_type == DFGPU_FLOAT32) { float f = __uint_as_float((uint32_t)v); v = (uint64_t)__double_as_longlong((double)f); }
-    sk[sp] = true; sv[sp] = v; ++sp;
+    sk[sp] = XN ? ((ext[kExtValid] >> nd.voff) & 1ull) != 0 : true; sv[sp] = v; ++sp;
     break;
       }
       case DFGPU_EXPR_BINARY: {
@@ -281,7 +285,7 @@ __device__ __forceinline__ uint64_t eval_nodes(const ENode* __restrict__ nodes, 
 // Register-resident variant for shallow programs (stack depth <= DEPTH): every stack slot is addressed through fully
 // unrolled selects, so the stack never leaves the register file (the indexed arrays of eval_nodes live in local memory,
 // which costs an L1 round trip per push / pop and — in divergent consumers — real L2 / DRAM traffic).
-template <int DEPTH>
+template <int DEPTH, bool XN = false>
 __device__ __forceinline__ uint64_t eval_nodes_reg(const ENode* __restrict__ nodes, int n_nodes, int64_t row, bool* ok_out, int* err, const uint64_t* ext = nullptr) {
   uint64_t sv[DEPTH];
   bool sk[DEPTH];
@@ -303,7 +307,7 @@ __device__ __forceinline__ uint64_t eval_nodes_reg(const ENode* __restrict__ nod
       const int w = type_width_prim(nd.out_type);
       if (w < 8) { v &= (1ull << (8 * w)) - 1ull; if (type_is_signed_int(nd.out_type)) v = (uint64_t)(((int64_t)(v << (64 - 8 * w))) >> (64 - 8 * w)); }
       if (nd.out_type == DFGPU_FLOAT32) { float f = __uint_as_float((uint32_t)v); v = (uint64_t)__double_as_longlong((double)f); }
-      DF_PUSH(v, true);
+      DF_PUSH(v, XN ? ((ext[kExtValid] >> nd.voff) & 1ull) != 0 : true);
     } else if (nd.kind == DFGPU_EXPR_BINARY) {
       uint64_t a = 0, b = 0, r; bool ak = false, bk = false, ok;
       DF_GET(sp - 2, a, ak); DF_GET(sp - 1, b, bk);

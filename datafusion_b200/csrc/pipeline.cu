@@ -47,6 +47,7 @@ enum SinkKind : int { SINK_NONE = 0, SINK_COUNT = 1, SINK_BUILD = 2, SINK_AGG = 
                       SINK_DENSE = 7 /* aggregate over group keys in small declared domains: slot arithmetic, shared-memory accumulators */,
                       SINK_HASH = 8 /* aggregate over a packed group key: find-or-claim in the sink's own table */ };
 constexpr int kStageMaybe = 3;   // DFGPU_STAGE_MAYBE
+static_assert(kExtValid == kMaxStages, "the payload validity word follows the kMaxStages payload words (expr_dev.cuh)");
 constexpr int kPipeVarDefault = 11;   // pipe_kernel's VAR when DFGPU_PIPE_VAR is not set (H100 SXM at 400 W, Q3 SF100 lineitem pass: 17.5 ms; 43 20.4-20.9 ms)
 // ring-fed phase A: at most kMaxRing streamed columns, kMaxRingStages tiles per warp ring, the mbarriers in the first kRingBarBytes of the
 // dynamic shared memory; kGather gathered argument columns
@@ -225,30 +226,33 @@ __device__ __forceinline__ uint64_t eval_int_gathered(const ENode* __restrict__ 
   return s0;
 }
 
-// programs that touch Decimal128 values (small == 3): the 128-bit interpreter; returns the low word, *hi the high word
+// programs that touch Decimal128 values (small == 3): the 128-bit interpreter; returns the low word, *hi the high word.
+// XN (and in the functions below): nullable payload fields, ext[kExtValid] holds their validity bits (pipe_kernel VAR bit 1024)
+template <bool XN = false>
 __device__ __noinline__ uint64_t pipe_eval_dec(const ENode* nodes, int n, int64_t row, const uint64_t* ext, int* err_ok, unsigned long long* hi) {
   bool ok;
   int err = 0;
-  const i128 v = eval_nodes_dec(nodes, n, row, &ok, &err, ext);
+  const i128 v = eval_nodes_dec<XN>(nodes, n, row, &ok, &err, ext);
   err_ok[0] |= err; err_ok[1] = ok ? 1 : 0;
   *hi = (unsigned long long)((u128)v >> 64);
   return (uint64_t)v;
 }
 // one out-of-line copy of each interpreter: the kernel stays small enough for the instruction cache
-template <bool DEC>
+template <bool DEC, bool XN = false>
 __device__ __noinline__ uint64_t pipe_eval(const ENode* nodes, int n, int small, int64_t row, const uint64_t* ext, int* err_ok /* [0]=err bits (or-ed), [1]=valid */) {
-  if (DEC && small == 3) { unsigned long long hi; return pipe_eval_dec(nodes, n, row, ext, err_ok, &hi); }
+  if (DEC && small == 3) { unsigned long long hi; return pipe_eval_dec<XN>(nodes, n, row, ext, err_ok, &hi); }
   bool ok;
   int err = 0;
-  const uint64_t v = small ? eval_nodes_reg<4>(nodes, n, row, &ok, &err, ext) : eval_nodes(nodes, n, row, &ok, &err, ext);
+  const uint64_t v = small ? eval_nodes_reg<4, XN>(nodes, n, row, &ok, &err, ext) : eval_nodes<XN>(nodes, n, row, &ok, &err, ext);
   err_ok[0] |= err; err_ok[1] = ok ? 1 : 0;
   return v;
 }
 // SUM over a Decimal128 argument, evaluated and accumulated out of line (the hot integer path of the aggregate sink stays as it was):
 // i128 add_wrapping over two accumulator words — the carry out of the low word is decided by this add alone
+template <bool XN = false>
 __device__ __noinline__ void pipe_sum_dec(const ENode* nodes, int n, int64_t row, const uint64_t* ext, int* err_ok, unsigned long long* acc, unsigned long long* nn) {
   unsigned long long hi;
-  const unsigned long long lo = pipe_eval_dec(nodes, n, row, ext, err_ok, &hi);
+  const unsigned long long lo = pipe_eval_dec<XN>(nodes, n, row, ext, err_ok, &hi);
   if (!err_ok[1]) return;                                  // NULL inputs are skipped (accumulate.rs:373-470)
   if (nn) atomicAdd(nn, 1ull);
   const unsigned long long old = atomicAdd(acc, lo);
@@ -257,10 +261,11 @@ __device__ __noinline__ void pipe_sum_dec(const ENode* nodes, int n, int64_t row
 }
 // MIN / MAX over a Decimal128 argument, out of line like SUM: the {lo, hi} pair at acc (16-byte aligned in the record) is read in one
 // 128-bit load and replaced by a 128-bit CAS only when the value is better
+template <bool XN = false>
 __device__ __noinline__ void pipe_minmax_dec(const ENode* nodes, int n, int64_t row, const uint64_t* ext, int* err_ok, unsigned long long* acc, unsigned long long* nn,
                                              bool is_min) {
   unsigned long long hi;
-  const unsigned long long lo = pipe_eval_dec(nodes, n, row, ext, err_ok, &hi);
+  const unsigned long long lo = pipe_eval_dec<XN>(nodes, n, row, ext, err_ok, &hi);
   if (!err_ok[1]) return;                                  // NULL inputs are skipped
   if (nn) atomicAdd(nn, 1ull);
   minmax_i128(acc, Rec128{lo, hi}, is_min);
@@ -401,6 +406,11 @@ __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_
 //              not matched; a filtered bitmap ANTI stage is decided in phase B instead of phase A.
 //   bit 9 (512) output columns with validity bitmaps or 16 bytes wide, unordered output sink only (OutValid; pipeline_push picks it when a
 //              column of the push needs it, on top of the sink's default or filtered bits).
+//   bit 10 (1024) RIGHT stages (Right joins; launch_pipe, hash_push, launch_dense pick it whenever the pipeline has one, never with bits 6,
+//              7, 8 or DFGPU_PIPE_VAR): phase A skips a RIGHT stage (it drops nothing); phase B probes it like an INNER hash stage but keeps
+//              every row, with the stage's bit of pvalid cleared and its payload word 0 on a miss.  pvalid rides behind the payload words as
+//              ext[kExtValid], so the interpreters' XN instantiations see the fields as NULL; the output (with bit 9), dense and hash
+//              sinks read it for the fields they take directly.
 // DFGPU_PIPE_VAR selects the instantiation (aggregate sink; bits 1 and 5 also for the pack sink, bit 1 for the unordered-output sink); 0 is the
 // kernel without any of them, 11 the default.  Tried and removed: four instead of two survivors per lane and phase-B round; prefetching the
 // table record and the argument sectors already when a row passes the membership filter in phase A (the prefetches of five tiles queue up
@@ -481,6 +491,7 @@ constexpr int kFiltParamsOff = kDenseParamsOff + (int)(((sizeof(DenseParams) > s
 // when its input column has one in this push; payload fields never do.
 // ------------------------------------------------------------------------------------------
 constexpr int kVarOutCols = 512;
+constexpr int kVarRight = 1024, kStageRight = 6;   // pipe_kernel VAR bit 10; DFGPU_STAGE_RIGHT
 struct OutValid { uint32_t* valid[kMaxPipeCols]; /* nullptr: the column leaves without a bitmap */ };
 static_assert(kDenseParamsOff + (int)sizeof(OutValid) <= kFiltParamsOff, "OutValid fits the sink's block");
 // one 16-byte value (Decimal128): Arrow promises only 8-byte alignment of a sliced input buffer
@@ -606,6 +617,10 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
   constexpr bool RING = (VAR & 64) != 0, PART = (VAR & 128) != 0, FILT = (VAR & kVarFilt) != 0, OUTV = (VAR & kVarOutCols) != 0;
   static_assert(!FILT || !(RING || PART), "stage filters do not run on the ring-fed or partitioned paths");
   static_assert(!OUTV || SINK == SINK_OUTPUT_ANY, "output bitmaps and 16-byte columns belong to the unordered output sink");
+  constexpr bool RIGHT = (VAR & kVarRight) != 0;
+  static_assert(!RIGHT || (!RING && !PART && !FILT && (SINK == SINK_DENSE || SINK == SINK_HASH || (SINK == SINK_OUTPUT_ANY && OUTV))),
+                "RIGHT stages run with the dense, hash and unordered output (bitmap) sinks only");
+  constexpr int NX = kMaxStages + (RIGHT ? 1 : 0);   // a row's ext words: the stages' payload words, then (RIGHT) their validity bits
   __shared__ PipeParams sp;
   __shared__ uint32_t q_rows[kPipeWarps][QC];
   extern __shared__ __align__(128) unsigned char dyn_smem[];   // RING: mbarriers [warp][stage], then the rings [warp][stage][ring_bytes]
@@ -760,6 +775,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
 #pragma unroll 1
       for (int s = 0; s < sp.n_stages; ++s) {
         const StageDev& st = sp.stage[s];
+        if constexpr (RIGHT) if (st.kind == kStageRight) continue;   // drops nothing: no NULL-key mask, no membership test
         const bool bitmap = st.lk.mode == LK_BITMAP;
         if constexpr (FILT) if (bitmap && st.kind == DFGPU_STAGE_ANTI && fpp->n[s] > 0) continue;   // a key match alone drops nothing: phase B
         if (!bitmap && !(st.lk.bloom && st.kind != DFGPU_STAGE_ANTI)) {   // nothing cheap to test; NULL keys of an inner / semi stage still drop here
@@ -837,10 +853,12 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
       int64_t row[PB];
       uint64_t pay[kMaxStages][PB], pkey[PB];   // pkey: PART, the aggregate stage's key
       unsigned long long* arec[PB];
+      uint32_t pvalid[PB];                      // RIGHT: bit s = stage s's payload fields are valid (cleared by a RIGHT stage's miss)
 #pragma unroll
       for (int u = 0; u < PB; ++u) {
         const unsigned int e = u * 32 + lane;
         live[u] = e < take; row[u] = live[u] ? (int64_t)q_row[qbase + e] : 0; arec[u] = nullptr; pkey[u] = 0;
+        if constexpr (RIGHT) pvalid[u] = ~0u;
       }
       if ((VAR & 1) && SINK == SINK_AGG) {
 #pragma unroll 1
@@ -907,8 +925,9 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
 #pragma unroll
         for (int u = 0; u < PB; ++u) {
           found[u] = false; look[u] = live[u]; key[u] = 0;
+          if constexpr (RIGHT) if (st.lk.cap == 0) look[u] = false;   // an empty build side has no table (a Right join keeps its rows)
           if (look[u]) {
-            key[u] = ld_stream_int(kc.ptr, kc.width, kc.sgn, row[u], pol_stream);   // the line was streamed in moments ago: an L2 hit
+            key[u] = ld_stream_int(kc.ptr, kc.width, kc.sgn, row[u], pol_stream);   // streamed in moments ago by phase A: an L2 hit (not for a RIGHT stage, which phase A skips)
             if ((kc.valid && !bit_get(kc.valid, kc.voff + row[u])) || key[u] == kEmptyKey) look[u] = false;   // NULL keys never match
           }
           slot[u] = __umul64hi(lk_hash(key[u]), st.lk.cap); ck[u] = kEmptyKey; cp[u] = 0;
@@ -945,6 +964,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
               if (SINK == SINK_AGG && s == sp.agg_stage && (!FILT || found[u])) arec[u] = st.lk.recs + slot[u] * (uint64_t)st.lk.stride;
             }
           }
+          if constexpr (RIGHT) if (st.kind == kStageRight) { if (!found[u]) pvalid[u] &= ~(1u << s); continue; }   // keeps the row
           live[u] = live[u] && (st.kind == DFGPU_STAGE_ANTI ? !found[u] : found[u]);
         }
       }
@@ -990,8 +1010,15 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
             for (int c = 0; m && c < sp.n_out; ++c) {
               uint32_t* dv = ov->valid[c];
               if (!dv) continue;
-              const ColRef& col = sp.col[sp.out_src[c]];
-              const unsigned bits = __reduce_or_sync(0xffffffffu, live[u] && bit_get(col.valid, col.voff + row[u]) ? 1u << rank : 0u);
+              unsigned bits;
+              if constexpr (RIGHT) {   // a payload field's bit: its stage matched
+                const int src = sp.out_src[c];
+                const bool ok = live[u] && (src < sp.n_cols ? bit_get(sp.col[src].valid, sp.col[src].voff + row[u]) : ((pvalid[u] >> sp.ext[src - sp.n_cols].stage) & 1u) != 0);
+                bits = __reduce_or_sync(0xffffffffu, ok ? 1u << rank : 0u);
+              } else {
+                const ColRef& col = sp.col[sp.out_src[c]];
+                bits = __reduce_or_sync(0xffffffffu, live[u] && bit_get(col.valid, col.voff + row[u]) ? 1u << rank : 0u);
+              }
               const int sh = (int)(start & 31);
               if (lane == 0 && bits) {
                 atomicOr(dv + (start >> 5), bits << sh);
@@ -1072,9 +1099,10 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
 #pragma unroll 1
         for (int u = 0; u < PB; ++u) {
           if (!__any_sync(0xffffffffu, live[u])) continue;
-          uint64_t ext[kMaxStages];
+          uint64_t ext[NX];
 #pragma unroll
           for (int s = 0; s < kMaxStages; ++s) ext[s] = pay[s][u];
+          if constexpr (RIGHT) ext[kExtValid] = pvalid[u];
           int slot = -1;
           if (live[u]) {
             alive_cnt++;
@@ -1095,6 +1123,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
 #pragma unroll
                 for (int s = 0; s < kMaxStages; ++s) if (s == e.stage) wd = ext[s];
                 key = ext_field(wd, e.shift, e.width, e.type);
+                if constexpr (RIGHT) isnull = !((pvalid[u] >> e.stage) & 1u);
               }
               const uint64_t idx = isnull ? dk.nvals : key - dk.kmin;   // modular: one unsigned compare checks both bounds
               if (idx > dk.nvals || (!isnull && idx == dk.nvals)) { inside = false; break; }
@@ -1118,8 +1147,8 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
             unsigned ok = 0;
             if (slot >= 0) {
               if (ag.small == 2) { lo = eval_int_fast(sp.pool + ag.start, ag.n, row[u], ext); ok = 1; }
-              else if (DEC && ag.small == 3) { lo = pipe_eval_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, &hi); ok = err_ok[1] ? 1 : 0; }
-              else { lo = pipe_eval<DEC>(sp.pool + ag.start, ag.n, ag.small, row[u], ext, err_ok); ok = err_ok[1] ? 1 : 0; }
+              else if (DEC && ag.small == 3) { lo = pipe_eval_dec<RIGHT>(sp.pool + ag.start, ag.n, row[u], ext, err_ok, &hi); ok = err_ok[1] ? 1 : 0; }
+              else { lo = pipe_eval<DEC, RIGHT>(sp.pool + ag.start, ag.n, ag.small, row[u], ext, err_ok); ok = err_ok[1] ? 1 : 0; }
               if (ag.f64_key) lo = f64_to_ordered(__longlong_as_double((long long)lo));
             }
             if (!ok && ag.word >= 0) { lo = dp.ident[ag.word]; hi = ag.op == DO_MIN_128 || ag.op == DO_MAX_128 ? dp.ident[ag.word + 1] : 0ull; }
@@ -1158,6 +1187,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
 #pragma unroll
               for (int s = 0; s < kMaxStages; ++s) if (s == e.stage) wd = pay[s][u];
               v = ext_field(wd, e.shift, e.width, DFGPU_UINT64);
+              if constexpr (RIGHT) isnull = !((pvalid[u] >> e.stage) & 1u);   // v is 0 then: the payload word of a miss
             }
             if (isnull && hk.null_bit < 0) fail |= 4;   // a NULL in a column declared non-nullable
             if (hk.bits < 64) v &= (1ull << hk.bits) - 1ull;
@@ -1171,9 +1201,10 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
 #pragma unroll
       for (int u = 0; u < PB; ++u) {
         if (SINK == SINK_OUTPUT_ANY || SINK == SINK_DENSE || sunk) break;
-        uint64_t ext[kMaxStages];
+        uint64_t ext[NX];
 #pragma unroll
         for (int s = 0; s < kMaxStages; ++s) ext[s] = pay[s][u];
+        if constexpr (RIGHT) ext[kExtValid] = pvalid[u];
         if (!live[u]) continue;
         alive_cnt++;
         if (SINK == SINK_BUILD || SINK == SINK_PACK) {
@@ -1213,12 +1244,12 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
                                                   : eval_int_fast(sp.pool + ag.start, ag.n, row[u], ext);
             else if (DEC && ag.cls == C_DEC && ag.func != DFGPU_AGG_COUNT) {
               unsigned long long* nn = ag.nn_word >= 0 ? rec + ag.nn_word : nullptr;   // AVG: its count word
-              if (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) pipe_minmax_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, nn, ag.func == DFGPU_AGG_MIN);
-              else pipe_sum_dec(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, nn);   // SUM, and the sum of AVG
+              if (ag.func == DFGPU_AGG_MIN || ag.func == DFGPU_AGG_MAX) pipe_minmax_dec<RIGHT>(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, nn, ag.func == DFGPU_AGG_MIN);
+              else pipe_sum_dec<RIGHT>(sp.pool + ag.start, ag.n, row[u], ext, err_ok, rec + ag.word, nn);   // SUM, and the sum of AVG
               continue;
             } else {
               if (RING) { atomicOr(&counters[3], (unsigned long long)kErrRingAgg); continue; }   // fill_ring admits integer programs and COUNT(*) only
-              v = pipe_eval<DEC>(sp.pool + ag.start, ag.n, ag.small, row[u], ext, err_ok);
+              v = pipe_eval<DEC, RIGHT>(sp.pool + ag.start, ag.n, ag.small, row[u], ext, err_ok);
               if (!err_ok[1]) continue;                      // NULL inputs are skipped (accumulate.rs:373-470)
             }
             if (ag.nn_word >= 0) red_add_u64(rec + ag.nn_word, 1ull);
@@ -1374,8 +1405,10 @@ __global__ void __launch_bounds__(256) pipe_probe_agg_kernel(const ulonglong2* _
 struct OutCols { int n; int src[kMaxPipeCols]; int width[kMaxPipeCols]; void* dst[kMaxPipeCols]; };
 
 // FILT: the stage filters (FiltParams at offset 0 of the dynamic shared memory), evaluated on each candidate pair with the interpreter of
-// pipe_kernel's DEC instantiations.  COLS: output columns with bitmaps or 16 bytes wide (OutValid behind PipeParams; pipe_output_cols_kernel)
-template <bool FILT, bool COLS>
+// pipe_kernel's DEC instantiations.  COLS: output columns with bitmaps or 16 bytes wide (OutValid behind PipeParams; pipe_output_cols_kernel).
+// RIGHT (with COLS, without FILT): RIGHT stages keep every row; each survivor's payload validity bits (bit s = stage s matched) are staged
+// in the dynamic shared memory next to s_pay, and a RIGHT payload column's bitmap takes them (pipe_output_right_kernel)
+template <bool FILT, bool COLS, bool RIGHT = false>
 __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ gp, int64_t n, const OutCols& oc, unsigned long long* __restrict__ tile_desc,
                                                  unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
   __shared__ PipeParams sp;
@@ -1393,13 +1426,16 @@ __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ 
   __syncthreads();
   const int64_t tile = s_tile;
   const int64_t row0 = tile * kPipeTile + (int64_t)threadIdx.x * kPipeItems;   // consecutive rows per thread: rank order == row order
+  static_assert(!RIGHT || (COLS && !FILT), "RIGHT stages: output bitmaps, no stage filters");
   int err = 0;
   bool alive[kPipeItems];
   uint64_t pay[kMaxStages][kPipeItems];
+  uint32_t pvalid[kPipeItems];   // RIGHT: bit s = stage s's payload fields are valid
 #pragma unroll
   for (int k = 0; k < kPipeItems; ++k) {
     const int64_t row = row0 + k;
     alive[k] = row < n;
+    if constexpr (RIGHT) pvalid[k] = ~0u;
 #pragma unroll
     for (int s = 0; s < kMaxStages; ++s) pay[s][k] = 0;
     if (!alive[k]) continue;
@@ -1450,7 +1486,7 @@ __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ 
         if (st.lk.mode == LK_BITMAP) {
           const uint64_t i = key - st.lk.kmin;
           found = i < st.lk.ksize && ((__ldg(&st.lk.bits[i >> 5]) >> (i & 31)) & 1u);
-        } else if (key != kEmptyKey) {
+        } else if (key != kEmptyKey && (!RIGHT || st.lk.cap > 0)) {   // RIGHT: an empty build side has no table
           const uint64_t h = lk_hash(key);
           bool maybe = true;
           if (st.lk.coarse) { const CoarsePos cp = coarse_pos(key, st.lk.coarse_words); maybe = (st.lk.coarse[cp.word] & cp.mask) == cp.mask; }
@@ -1477,6 +1513,7 @@ __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ 
           err = eo[0];
         }
       }
+      if constexpr (RIGHT) if (st.kind == kStageRight) { if (!found) pvalid[k] &= ~(1u << s); continue; }   // keeps the row
       alive[k] = st.kind == DFGPU_STAGE_ANTI ? !found : found;
     }
   }
@@ -1491,6 +1528,7 @@ __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ 
       s_p[ex] = (uint32_t)(threadIdx.x * kPipeItems + k);
 #pragma unroll
       for (int s = 0; s < kMaxStages; ++s) s_pay[s][ex] = pay[s][k];
+      if constexpr (RIGHT) dyn_smem[ex] = (unsigned char)pvalid[k];
       ++ex;
     }
   if (threadIdx.x < 32) {
@@ -1529,12 +1567,15 @@ __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ 
     for (int c = 0; c < oc.n; ++c) {
       uint32_t* dv = ov->valid[c];
       if (!dv || nw == 0) continue;
-      const ColRef& col = sp.col[oc.src[c]];
+      const int src = oc.src[c];
       for (int i = threadIdx.x; i < nw; i += kPipeThreads) s_vw[i] = 0;
       __syncthreads();
       for (uint32_t j0 = 0; j0 < tot; j0 += kPipeThreads) {
         const uint32_t j = j0 + threadIdx.x;
-        const unsigned bits = __ballot_sync(0xffffffffu, j < tot && bit_get(col.valid, col.voff + prow0 + s_p[j]));
+        bool ok;
+        if constexpr (RIGHT) ok = j < tot && (src < sp.n_cols ? bit_get(sp.col[src].valid, sp.col[src].voff + prow0 + s_p[j]) : ((dyn_smem[j] >> sp.ext[src - sp.n_cols].stage) & 1u) != 0);
+        else { const ColRef& col = sp.col[src]; ok = j < tot && bit_get(col.valid, col.voff + prow0 + s_p[j]); }
+        const unsigned bits = __ballot_sync(0xffffffffu, ok);
         const uint32_t first = (uint32_t)sh + j0 + (threadIdx.x & ~31u);   // staged bit of this warp's lane 0
         if (lane == 0 && bits) {
           atomicOr(&s_vw[first >> 5], bits << (first & 31));
@@ -1563,6 +1604,11 @@ template <bool FILT>
 __global__ void __launch_bounds__(kPipeThreads) pipe_output_cols_kernel(const PipeParams* __restrict__ gp, int64_t n, OutCols oc, unsigned long long* __restrict__ tile_desc,
                                                                        unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
   pipe_output_tile<FILT, true>(gp, n, oc, tile_desc, tile_counter, totals, counters);
+}
+// the same for a pipeline with RIGHT stages (kPipeTile bytes of dynamic shared memory: the survivors' payload validity bits)
+__global__ void __launch_bounds__(kPipeThreads) pipe_output_right_kernel(const PipeParams* __restrict__ gp, int64_t n, OutCols oc, unsigned long long* __restrict__ tile_desc,
+                                                                        unsigned int* __restrict__ tile_counter, unsigned long long* __restrict__ totals, unsigned long long* __restrict__ counters) {
+  pipe_output_tile<false, true, true>(gp, n, oc, tile_desc, tile_counter, totals, counters);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1933,6 +1979,7 @@ struct dfgpu_pipeline {
   bool has_pred = false;
   ExprPlan pred;
   std::vector<dfgpu_pipeline_stage> stages;
+  bool has_right = false;   // a RIGHT stage: every kernel runs its VAR bit 1024 / pipe_output_right_kernel instantiation
   // stage filters (dfgpu_pipeline_set_stage_filter): per stage the program and the payload fields its virtual columns past the inputs name
   ExprPlan filt[kMaxStages]; bool has_filt[kMaxStages] = {false, false, false}; std::vector<ExtDef> filt_ext[kMaxStages]; int filt_nodes = 0;
   std::unique_ptr<FiltParams> filt_host;   // staging copy of the bound programs (upload_filters)
@@ -2098,24 +2145,31 @@ static int plan_depth(const ExprPlan& plan) {
   return mx;
 }
 
-// only integer columns without NULLs (in THIS batch), non-NULL integer literals, payload fields and + - *: eval_int_fast applies
+// virtual column c is a payload field of a RIGHT stage: NULL on the rows that stage did not match
+static bool is_right_field(const dfgpu_pipeline* p, int c) {
+  const int nin = (int)p->in_types.size();
+  return c >= nin && p->stages[p->exts[c - nin].stage].kind == DFGPU_STAGE_RIGHT;
+}
+
+// only integer columns without NULLs (in THIS batch), non-NULL integer literals, payload fields (not a RIGHT stage's: they can be NULL) and
+// + - *: eval_int_fast applies
 static bool plan_is_int_arith(const dfgpu_pipeline* p, const ExprPlan& plan, const std::vector<DCol>& cols) {
   for (size_t i = 0; i < plan.nodes.size(); ++i) {
     const dfgpu_expr_node& nd = plan.nodes[i];
     const int t = plan.out_type[i];
     if (!type_is_int(t)) return false;
-    if (nd.kind == DFGPU_EXPR_COLUMN) { if (nd.a < (int)cols.size() && cols[nd.a].validity) return false; }
+    if (nd.kind == DFGPU_EXPR_COLUMN) { if ((nd.a < (int)cols.size() && cols[nd.a].validity) || is_right_field(p, nd.a)) return false; }
     else if (nd.kind == DFGPU_EXPR_LITERAL) { if (nd.is_null) return false; }
     else if (nd.kind == DFGPU_EXPR_BINARY) { if (nd.a != DFGPU_OP_PLUS && nd.a != DFGPU_OP_MINUS && nd.a != DFGPU_OP_MULTIPLY) return false; }
     else return false;
   }
-  (void)p;
   return true;
 }
 
-static bool expr_can_be_null(const ExprPlan& plan, const std::vector<DCol>& cols) {
+static bool expr_can_be_null(const dfgpu_pipeline* p, const ExprPlan& plan, const std::vector<DCol>& cols) {
   for (const auto& nd : plan.nodes) {
     if (nd.kind == DFGPU_EXPR_COLUMN && nd.a < (int)cols.size() && cols[nd.a].validity) return true;
+    if (nd.kind == DFGPU_EXPR_COLUMN && is_right_field(p, nd.a)) return true;
     if (nd.kind == DFGPU_EXPR_LITERAL && nd.is_null) return true;
   }
   return false;
@@ -2234,7 +2288,7 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
         if (d.small && plan_is_int_arith(p, ag.plan, cols)) d.small = 2;
         if (ag.plan.has_decimal) d.small = 3;
         if (ag.nn_word < 0 && ag.func != DFGPU_AGG_COUNT)
-          DF_CHECK(!expr_can_be_null(ag.plan, cols), DFGPU_ERR_UNSUPPORTED, "pipeline: nullable aggregate input needs one more accumulator word in the lookup (n_acc_words)");
+          DF_CHECK(!expr_can_be_null(p, ag.plan, cols), DFGPU_ERR_UNSUPPORTED, "pipeline: nullable aggregate input needs one more accumulator word in the lookup (n_acc_words)");
       }
     }
     if (pp->n_aggs > 0 && pp->agg[0].small == 2) {
@@ -2309,8 +2363,10 @@ static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, cons
     return;
   }
   DF_CHECK(!part, DFGPU_ERR_INVALID, "internal: the partitioned aggregate needs the ring-fed pipeline kernel");
+  DF_CHECK(!p->has_right || (SINK == SINK_OUTPUT_ANY && out_cols), DFGPU_ERR_INVALID, "internal: RIGHT stages run the output kernel with bitmaps");
   if constexpr (SINK == SINK_OUTPUT_ANY) if (out_cols) {   // output bitmaps or 16-byte columns: the default bits of this sink plus OutValid
     void (*kern)(const PipeParams*, int64_t, unsigned long long*) = dec ? pipe_kernel<SINK, true, kVarOutCols> : pipe_kernel<SINK, false, 2 | kVarOutCols>;
+    if (p->has_right) kern = dec ? pipe_kernel<SINK, true, kVarOutCols | kVarRight> : pipe_kernel<SINK, false, 2 | kVarOutCols | kVarRight>;
     int blocks_per_sm = 0;
     DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, 0));
     const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
@@ -2361,7 +2417,7 @@ static std::vector<DCol> alloc_output(dfgpu_pipeline* p, const std::vector<DCol>
   std::vector<DCol> part;
   for (size_t c = 0; c < p->out_cols.size(); ++c) {
     const int src = p->out_cols[c];
-    const bool nullable = src < (int)cols.size() && cols[src].validity;
+    const bool nullable = (src < (int)cols.size() && cols[src].validity) || is_right_field(p, src);
     DCol d = alloc_col(p->ctx, p->vtypes[src], n, nullable);
     if (nullable) { d.own_validity->zero(); ov->valid[c] = d.own_validity->as<uint32_t>(); }
     part.push_back(std::move(d));
@@ -2370,6 +2426,7 @@ static std::vector<DCol> alloc_output(dfgpu_pipeline* p, const std::vector<DCol>
 }
 // the output kernels with bitmaps and 16-byte columns (pipe_kernel VAR bit 512, pipe_output_cols_kernel) run only when a column needs them
 static bool output_needs_cols(const dfgpu_pipeline* p, const OutValid* ov) {
+  if (p->has_right) return true;   // the RIGHT instantiations are the bitmap ones
   for (size_t c = 0; c < p->out_cols.size(); ++c)
     if (ov->valid[c] || type_width(p->vtypes[p->out_cols[c]]) == 16) return true;
   return false;
@@ -2483,6 +2540,7 @@ static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DensePar
   DF_CUDA(cudaStreamSynchronize(ctx->stream));   // `pp` and `dp` live on the caller's stack frame
   // programs that touch Decimal128 values run the instantiation with the 128-bit interpreter
   void (*kern)(const PipeParams*, int64_t, unsigned long long*) = pipeline_has_decimal(p) ? pipe_kernel<SINK_DENSE, true> : pipe_kernel<SINK_DENSE, false>;
+  if (p->has_right) kern = pipeline_has_decimal(p) ? pipe_kernel<SINK_DENSE, true, kVarRight> : pipe_kernel<SINK_DENSE, false, kVarRight>;   // no stage filters
   int smem = kDenseAccOff + (dp.per_warp ? kPipeWarps : 1) * p->dense_slots * p->dense_words * 8;
   if (pipeline_has_filters(p)) {   // the stage filters behind the slots
     kern = pipeline_has_decimal(p) ? pipe_kernel<SINK_DENSE, true, kVarFilt> : pipe_kernel<SINK_DENSE, false, filt_var(SINK_DENSE)>;
@@ -2559,6 +2617,7 @@ static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t 
   if (p->params_dev.bytes < pbytes) p->params_dev.alloc(ctx, pbytes);
   // programs that touch Decimal128 values run the instantiation with the 128-bit interpreter
   void (*kern)(const PipeParams*, int64_t, unsigned long long*) = pipeline_has_decimal(p) ? pipe_kernel<SINK_HASH, true> : pipe_kernel<SINK_HASH, false>;
+  if (p->has_right) kern = pipeline_has_decimal(p) ? pipe_kernel<SINK_HASH, true, kVarRight> : pipe_kernel<SINK_HASH, false, kVarRight>;   // no stage filters
   int smem = (int)sizeof(HashParams);
   if (pipeline_has_filters(p)) {   // the stage filters behind HashParams
     kern = pipeline_has_decimal(p) ? pipe_kernel<SINK_HASH, true, kVarFilt> : pipe_kernel<SINK_HASH, false, filt_var(SINK_HASH)>;
@@ -2892,7 +2951,10 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     unsigned int* counter = (unsigned int*)(totals + 2);
     {
       KernelTimer kt(ctx, "pipeline_output");
-      if (out_cols) {   // the instantiations above stay as they were for columns without bitmaps, <= 8 bytes wide
+      if (p->has_right) {   // RIGHT stages: the survivors' payload validity bits in the dynamic shared memory
+        pipe_output_right_kernel<<<(int)nt, kPipeThreads, kPipeTile, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, oc, desc.as<unsigned long long>(), counter, totals,
+                                                                                   p->counters.as<unsigned long long>());
+      } else if (out_cols) {   // the instantiations above stay as they were for columns without bitmaps, <= 8 bytes wide
         const bool filt = pipeline_has_filters(p);
         void (*kern)(const PipeParams*, int64_t, OutCols, unsigned long long*, unsigned int*, unsigned long long*, unsigned long long*) =
             filt ? pipe_output_cols_kernel<true> : pipe_output_cols_kernel<false>;
@@ -3230,6 +3292,11 @@ static void check_no_left_stage(const dfgpu_pipeline* p) {
     DF_CHECK(!is_left_kind(st.kind), DFGPU_ERR_UNSUPPORTED, "pipeline: a LEFT / LEFT_ANTI stage runs only with the join-keyed aggregate sink grouped on it");
 }
 
+// a RIGHT stage runs with the output, dense and hash sinks only
+static void check_no_right_stage(const dfgpu_pipeline* p, const char* what) {
+  DF_CHECK(!p->has_right, DFGPU_ERR_UNSUPPORTED, what);
+}
+
 // LEFT: a build row no probe row reached is emitted as one NULL-padded row without evaluating anything, so an aggregate argument must be
 // NULL on that row: it reads at least one probe-side input column, no payload field of the LEFT stage (that is the padded row's own
 // value), and every node propagates NULL (no IS [NOT] NULL, IS [NOT] DISTINCT FROM, AND, OR)
@@ -3465,7 +3532,10 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
   for (int s = 0; s < n_stages; ++s) {
     const dfgpu_pipeline_stage& st = stages[s];
     DF_CHECK(st.lookup, DFGPU_ERR_INVALID, "pipeline: stage without a lookup");
-    DF_CHECK(st.kind >= DFGPU_STAGE_INNER && st.kind <= DFGPU_STAGE_LEFT_ANTI, DFGPU_ERR_INVALID, "pipeline: unknown stage kind");
+    DF_CHECK(st.kind >= DFGPU_STAGE_INNER && st.kind <= DFGPU_STAGE_RIGHT, DFGPU_ERR_INVALID, "pipeline: unknown stage kind");
+    // a RIGHT stage keeps the row count only over unique keys: a lookup with payload (its build refuses duplicate keys)
+    DF_CHECK(st.kind != DFGPU_STAGE_RIGHT || (st.lookup->has_payload && st.lookup->mode == LK_HASH && !st.lookup->filter_only), DFGPU_ERR_UNSUPPORTED,
+             "pipeline: a RIGHT stage needs a lookup with payload (unique keys), not a key set, bitmap or filter-only lookup — use dfgpu_hashjoin");
     DF_CHECK(!st.lookup->filter_only || st.kind == DFGPU_STAGE_MAYBE, DFGPU_ERR_INVALID, "pipeline: a filter-only lookup can only back a MAYBE stage");
     DF_CHECK(st.key_col >= 0 && st.key_col < n_cols, DFGPU_ERR_INVALID, "pipeline: stage key column out of range");
     const int kt = input_types[st.key_col], lt = st.lookup->key_type;
@@ -3476,7 +3546,8 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
                "pipeline: probe key type differs from the lookup's key type");
     DF_CHECK(st.lookup->ctx->device == ctx->device, DFGPU_ERR_INVALID, "pipeline: lookup lives on another device");
     p->stages.push_back(st);
-    if (st.kind == DFGPU_STAGE_INNER || st.kind == DFGPU_STAGE_LEFT || st.kind == DFGPU_STAGE_LEFT_ANTI)
+    p->has_right = p->has_right || st.kind == DFGPU_STAGE_RIGHT;
+    if (st.kind == DFGPU_STAGE_INNER || st.kind == DFGPU_STAGE_LEFT || st.kind == DFGPU_STAGE_LEFT_ANTI || st.kind == DFGPU_STAGE_RIGHT)
       for (size_t f = 0; f < st.lookup->pay_types.size(); ++f) {
         DF_CHECK(p->exts.size() < (size_t)kMaxExt, DFGPU_ERR_UNSUPPORTED, "pipeline: at most 8 payload fields");
         ExtDef e; e.stage = s; e.shift = st.lookup->pay_shift[f]; e.width = type_width(st.lookup->pay_types[f]); e.type = st.lookup->pay_types[f];
@@ -3519,6 +3590,7 @@ int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t k
   DF_CHECK(p && target, DFGPU_ERR_INVALID, "null argument");
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
   check_no_left_stage(p);
+  check_no_right_stage(p, "pipeline build sink: a RIGHT stage's NULL payload fields cannot enter a lookup — use dfgpu_hashjoin");
   DF_CHECK(target->comp_types.empty(), DFGPU_ERR_INVALID, "pipeline build sink: a composite-key lookup is built by dfgpu_pipeline_sink_build_composite");
   DF_CHECK(key_col >= 0 && key_col < (int)p->in_types.size(), DFGPU_ERR_INVALID, "pipeline build sink: the key must be an input column");
   const int kt = p->in_types[key_col];
@@ -3534,6 +3606,7 @@ int dfgpu_pipeline_sink_build_composite(dfgpu_pipeline* p, dfgpu_lookup* target,
   DF_CHECK(p && target, DFGPU_ERR_INVALID, "null argument");
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
   check_no_left_stage(p);
+  check_no_right_stage(p, "pipeline build sink: a RIGHT stage's NULL payload fields cannot enter a lookup — use dfgpu_hashjoin");
   check_composite_keys(p, target, key_cols, n_keys, 1);
   set_build_sink(p, target, key_cols[0], payload_cols, n_payload);
   p->bkey_cols.assign(key_cols, key_cols + n_keys);
@@ -3558,6 +3631,7 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   DF_CHECK(p->sink == SINK_NONE && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline: the sink is chosen once, before the first push");
   DF_CHECK(n_aggs >= 0 && n_aggs <= kMaxPipeAggs && (n_aggs == 0 || aggs), DFGPU_ERR_UNSUPPORTED, "pipeline: 0..4 aggregates");
   DF_CHECK(mode == DFGPU_AGG_SINGLE || mode == DFGPU_AGG_SINGLE_PARTITIONED || mode == DFGPU_AGG_PARTIAL, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: Single / SinglePartitioned / Partial");
+  check_no_right_stage(p, "pipeline aggregate: the join-keyed sink does not run with a RIGHT stage — use the dense or hash aggregate sink");
   // a LEFT / LEFT_ANTI stage must be the last one, and the records grouped on are its own
   const int n_stages = (int)p->stages.size();
   int left = -1;
@@ -3773,6 +3847,7 @@ int dfgpu_pipeline_set_stage_filter(dfgpu_pipeline* p, int32_t stage, const dfgp
   DF_CHECK(!p->has_filt[stage], DFGPU_ERR_STATE, "pipeline stage filter: the stage already has one");
   const dfgpu_pipeline_stage& st = p->stages[stage];
   DF_CHECK(st.kind != DFGPU_STAGE_MAYBE, DFGPU_ERR_UNSUPPORTED, "pipeline stage filter: a MAYBE stage has no candidate row to test");
+  check_no_right_stage(p, "pipeline stage filter: a pipeline with a RIGHT stage takes no stage filters — use dfgpu_hashjoin");
   // the filter's columns: the inputs, the payload fields of the INNER / LEFT / LEFT_ANTI stages 0..stage, then a SEMI / ANTI stage's own
   const int nin = (int)p->in_types.size();
   std::vector<int> types(p->in_types);

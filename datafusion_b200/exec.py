@@ -632,7 +632,12 @@ class _Scan:
         for kind, _, build in self.stages:
             if kind in (D.STAGE_INNER, D.STAGE_LEFT, D.STAGE_LEFT_ANTI):
                 fields += [build.scan_field(n) for n in build.payload]
+            elif kind == D.STAGE_RIGHT:   # NULL on the probe rows no build row matched (build_join_schema(..., "Right"))
+                fields += [build.scan_field(n).with_nullable(True) for n in build.payload]
         return pa.schema(fields)
+
+    def has_right(self) -> bool:
+        return any(kind == D.STAGE_RIGHT for kind, _, _ in self.stages)
 
 
 _FILTER_NODES = 128   # the node pool of a pipeline's stage filters (dfgpu_pipeline_set_stage_filter)
@@ -731,14 +736,44 @@ def _stage_filter(sc: _Scan, join: GpuHashJoinExec, kind: int, payload: List[str
     return [(k, where[a], *rest) if k == D.EXPR_COLUMN else (k, a, *rest) for k, a, *rest in nodes]
 
 
-def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]:
-    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner, one key or a composite key
-    (_join_keys), fusable build)]* over a source.  join_filters: a join may carry a JoinFilter, which becomes its stage's filter
-    (fuse_join_filters)"""
+def _expr_names(e: Expr) -> set:
+    """the column names an expression reads"""
+    if isinstance(e, Column):
+        return {e.name}
+    if isinstance(e, BinaryExpr):
+        return _expr_names(e.left) | _expr_names(e.right)
+    if isinstance(e, (UnaryExpr, CastExpr)):
+        return _expr_names(e.arg)
+    return set()
+
+
+def _settle_right(sc: _Scan, read: set) -> bool:
+    """The RIGHT stages of sc (HashJoinExec(Right), planned by _as_scan with every build column) keep as payload exactly the build columns
+    read above the join (`read`), a build key included: it is NULL on the probe rows nothing matched, so it cannot stand in for the probe
+    key as an Inner join's can.  False when a RIGHT stage would carry no column (no payload lookup enforces unique keys then) or more than
+    64 bits, or when the pipeline has stage filters (they do not run beside a RIGHT stage).  Call before reading the virtual schema."""
+    if not sc.has_right():
+        return True
+    if sc.filters:
+        return False
+    for kind, _, build in sc.stages:
+        if kind != D.STAGE_RIGHT:
+            continue
+        build.payload = [n for n in build.payload if n in read]
+        if not build.payload or sum(D.WIDTH[type_id(build.scan_field(n).type)] * 8 for n in build.payload) > 64:
+            return False
+    return True
+
+
+def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False) -> Optional[_Scan]:
+    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner / Right, one key or a composite
+    key (_join_keys), fusable build)]* over a source.  join_filters: a join may carry a JoinFilter, which becomes its stage's filter
+    (fuse_join_filters); a Right join never does.  right_joins: Right joins are accepted (fuse_right_joins); such a stage carries every
+    build column until _settle_right keeps those read above it."""
     if isinstance(plan, GpuProjectionExec):
         if not all(isinstance(e, Column) and e.name == name for e, name in plan.exprs):
             return None
-        sc = _as_scan(plan.input, join_filters)
+        sc = _as_scan(plan.input, join_filters, right_joins)
         if sc is not None:
             sc.visible = [name for _, name in plan.exprs]
         return sc
@@ -753,17 +788,19 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]
             sc.visible = [inner.schema.field(i).name for i in plan.projection]
         return sc
     if isinstance(plan, GpuHashJoinExec):
-        if plan.join_type not in ("RightSemi", "RightAnti", "Inner") or (plan.filter is not None and not join_filters) or \
-                plan.null_aware or plan.null_equality != "NullEqualsNothing":
+        kinds = ("RightSemi", "RightAnti", "Inner") + (("Right",) if right_joins and plan.filter is None else ())
+        if plan.join_type not in kinds or (plan.filter is not None and not join_filters) or plan.null_aware or plan.null_equality != "NullEqualsNothing":
             return None
-        sc = _as_scan(plan.right, join_filters)
+        sc = _as_scan(plan.right, join_filters, right_joins)
         keys = None if sc is None else _join_keys(plan, sc)
         if keys is None or (isinstance(keys[1], str) and keys[1] not in [f.name for f in sc.source.schema]):
             return None
         bkey, pkey = keys
         bkeys = bkey if isinstance(bkey, list) else [bkey]
-        kind = {"RightSemi": D.STAGE_SEMI, "RightAnti": D.STAGE_ANTI, "Inner": D.STAGE_INNER}[plan.join_type]
+        kind = {"RightSemi": D.STAGE_SEMI, "RightAnti": D.STAGE_ANTI, "Inner": D.STAGE_INNER, "Right": D.STAGE_RIGHT}[plan.join_type]
         payload = [f.name for f in plan.left.schema if f.name not in bkeys] if kind == D.STAGE_INNER else []
+        if kind == D.STAGE_RIGHT:
+            payload = [f.name for f in plan.left.schema]
         if plan.filter is not None and kind != D.STAGE_INNER:   # a semi / anti lookup carries the build columns its filter reads
             read = {plan.left.schema.field(ix).name for sd, ix in plan.filter.column_indices if sd == "left"}
             payload = [f.name for f in plan.left.schema if f.name not in bkeys and f.name in read]
@@ -772,7 +809,7 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]
             filt = _stage_filter(sc, plan, kind, payload)
             if filt is None:
                 return None
-        build = _as_build(plan.left, bkey, payload, join_filters)
+        build = _as_build(plan.left, bkey, payload, join_filters, max_bits=None if kind == D.STAGE_RIGHT else 64)
         if build is None:
             return None
         if filt is not None:
@@ -786,9 +823,11 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False) -> Optional[_Scan]
     return _Scan(plan)
 
 
-def _as_build(plan: ExecutionPlan, key, payload: List[str], join_filters: bool = False) -> Optional["GpuPipelineExec"]:
+def _as_build(plan: ExecutionPlan, key, payload: List[str], join_filters: bool = False, max_bits: Optional[int] = 64) -> Optional["GpuPipelineExec"]:
     """the build pipeline of a fused join on `key` (a list of columns for a composite key: source columns with known bounds
-    (_source_bounds) whose domain, the product of max - min + 1, is at most 2^63 - 1, so that the tuple packs into one 64-bit key)"""
+    (_source_bounds) whose domain, the product of max - min + 1, is at most 2^63 - 1, so that the tuple packs into one 64-bit key).
+    max_bits None: the payload is settled later (a Right join's, _settle_right).  A build side with a Right join stays unfused: its NULL
+    payload fields cannot enter a lookup (_as_scan is not asked for Right joins here)."""
     sc = _as_scan(plan, join_filters)
     if sc is None or len(sc.stages) >= 3:
         return None
@@ -797,7 +836,7 @@ def _as_build(plan: ExecutionPlan, key, payload: List[str], join_filters: bool =
     if any(vs.get_field_index(k) < 0 or vs.get_field_index(k) >= len(sc.source.schema) for k in keys) or any(vs.get_field_index(n) < 0 for n in payload):
         return None
     bits = sum(D.WIDTH[type_id(vs.field(n).type)] * 8 for n in payload)
-    if bits > 64:
+    if max_bits is not None and bits > max_bits:
         return None
     ranges = []
     if isinstance(key, list):
@@ -912,6 +951,17 @@ class GpuPipelineExec(ExecutionPlan):
         if self.sink == "output":
             yield from self._execute_output(ctx)
             return
+        if self.fallback is not None:   # a RIGHT stage: its build's keys are known unique only once it ran; the sinks emit after finish
+            try:
+                out = list(self._execute_aggregate(ctx))
+            except D.DfgpuError as e:
+                yield from self._fall_back(ctx, e)
+                return
+            yield from out
+            return
+        yield from self._execute_aggregate(ctx)
+
+    def _execute_aggregate(self, ctx):
         vs = self.scan.virtual_schema()
         pipe, keep = self._make_pipeline(ctx)
         try:
@@ -998,7 +1048,7 @@ def _source_bounds(source: ExecutionPlan, name: str) -> Optional[Tuple[int, int]
         c = b.column(i)
         if c.null_count == len(c):
             continue
-        mm = pc.min_max(c.cast(pa.int64()) if pa.types.is_date32(t) else c)
+        mm = pc.min_max(c.cast(pa.int32()).cast(pa.int64()) if pa.types.is_date32(t) else c)   # date32 casts to int64 through int32 only
         lo = mm["min"].as_py() if lo is None else min(lo, mm["min"].as_py())
         hi = mm["max"].as_py() if hi is None else max(hi, mm["max"].as_py())
     if lo is None or hi > (1 << 63) - 1:
@@ -1006,25 +1056,28 @@ def _source_bounds(source: ExecutionPlan, name: str) -> Optional[Tuple[int, int]
     return lo, hi
 
 
-def _fuse_dense(plan: "GpuAggregateExec") -> Optional["GpuPipelineExec"]:
+def _fuse_dense(plan: "GpuAggregateExec", right_joins: bool = False) -> Optional["GpuPipelineExec"]:
     """AggregateExec over [ProjectionExec] over FilterExec over a source (no join) whose GROUP BY columns are source columns with known
     bounds spanning at most DENSE_MAX_GROUPS slots (NULL included) -> a GpuPipelineExec with the dense sink; None otherwise"""
     below, proj = plan.input, None
     if isinstance(below, GpuProjectionExec):
         proj, below = below, below.input
-    if not isinstance(below, GpuFilterExec):
+    right = right_joins and isinstance(below, GpuHashJoinExec) and below.join_type == "Right"
+    if not (isinstance(below, GpuFilterExec) or right):
         return None
-    sc = _as_scan(below)
-    if sc is None or sc.stages:
+    sc = _as_scan(below, right_joins=right)
+    if sc is None or (sc.stages and not right):
         return None
-    src = sc.source.schema
     exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
+    if right and not _settle_right(sc, _read_names(plan, exprs)):
+        return None
+    vs = sc.virtual_schema()
     group, ranges, slots = [], [], 1
     for g in plan.group_by:
         e = exprs.get(g)
-        if not isinstance(e, Column) or e.name not in sc.visible or src.get_field_index(e.name) < 0:
+        if not isinstance(e, Column) or e.name not in sc.visible or vs.get_field_index(e.name) < 0:
             return None
-        b = _source_bounds(sc.source, e.name)
+        b = _field_bounds(sc, e.name)
         if b is None:
             return None
         slots *= b[1] - b[0] + 2
@@ -1043,8 +1096,8 @@ def _fuse_dense(plan: "GpuAggregateExec") -> Optional["GpuPipelineExec"]:
             return None
         if e is not None:
             try:
-                e.rpn(src, [])                             # every referenced name must be a source column
-                t = e.data_type(src)
+                e.rpn(vs, [])                              # every referenced name must be a column of the virtual schema
+                t = e.data_type(vs)
             except KeyError:
                 return None
             if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
@@ -1052,7 +1105,28 @@ def _fuse_dense(plan: "GpuAggregateExec") -> Optional["GpuPipelineExec"]:
             if a.func in ("min", "max") and t == pa.float32():
                 return None
         aggs.append((a.func, e, a.alias))
-    return GpuPipelineExec(sc, sink="dense", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, key_range=ranges)
+    return GpuPipelineExec(sc, sink="dense", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, key_range=ranges,
+                           fallback=plan if right else None)
+
+
+def _read_names(plan: "GpuAggregateExec", exprs: dict) -> set:
+    """the input column names an aggregate's GROUP BY and arguments read (through its projection's expressions)"""
+    read = set()
+    for n in list(plan.group_by) + [a.arg for a in plan.aggr_expr if a.arg is not None]:
+        if n in exprs:
+            read |= _expr_names(exprs[n])
+    return read
+
+
+def _field_bounds(sc: _Scan, name: str) -> Optional[Tuple[int, int]]:
+    """(min, max) of a column of sc's virtual schema: a source column's (_source_bounds), or a RIGHT stage's payload field taken from a
+    source column of its build side (a NULL field goes to its own dense slot)"""
+    if sc.source.schema.get_field_index(name) >= 0:
+        return _source_bounds(sc.source, name)
+    for kind, _, build in sc.stages:
+        if kind == D.STAGE_RIGHT and name in build.payload and build.scan.source.schema.get_field_index(name) >= 0:
+            return _source_bounds(build.scan.source, name)
+    return None
 
 
 def _acc_words(funcs: Sequence[str], types: Sequence[Optional[pa.DataType]], has_payload: bool) -> int:
@@ -1077,7 +1151,7 @@ def _acc_words(funcs: Sequence[str], types: Sequence[Optional[pa.DataType]], has
     return n
 
 
-def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False) -> ExecutionPlan:
+def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a): AggregateExec(Single / SinglePartitioned / Partial) over [ProjectionExec] over
     HashJoinExec(Inner) whose GROUP BY is the probe key plus build-side columns becomes ONE GpuPipelineExec; its build side (filters, semi
     joins, column projections) becomes build pipelines.  The same AggregateExec over [ProjectionExec] over FilterExec over a source, with
@@ -1092,7 +1166,7 @@ def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False) -> Execution
         return plan if fused is None else fused
     if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial"):
         return plan
-    dense = _fuse_dense(plan)
+    dense = _fuse_dense(plan, right_joins)
     if dense is not None:
         return dense
     if not plan.group_by:
@@ -1256,7 +1330,7 @@ def _fuse_left_filter(join: GpuHashJoinExec, join_filters: bool = False) -> Opti
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, mode="Single", out_schema=join.schema, project=project)
 
 
-def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False) -> ExecutionPlan:
+def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_pipelines: its result when that rule fuses; otherwise an
     AggregateExec(Single / SinglePartitioned / Partial) with at least one GROUP BY column over [ProjectionExec] over an Inner join chain or a
     FilterExec (as _as_scan accepts them) becomes ONE GpuPipelineExec with the hash-keyed sink (dfgpu_pipeline_sink_aggregate_hash: TPC-H
@@ -1264,7 +1338,7 @@ def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False) -> Exe
     (each column at its width, one more bit per nullable column) at most 128 bits; no FILTER clause, at most 4 aggregates, and the argument
     types the library accepts.  Anything else, a bare scan included, is returned unchanged (dfgpu_agg runs).  join_filters: joins with a
     JoinFilter fuse too (fuse_join_filters)."""
-    fused = fuse_pipelines(plan, join_filters)
+    fused = fuse_pipelines(plan, join_filters, right_joins)
     if fused is not plan:
         return fused
     if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial") or not plan.group_by:
@@ -1272,15 +1346,17 @@ def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False) -> Exe
     below, proj = plan.input, None
     if isinstance(below, GpuProjectionExec):
         proj, below = below, below.input
-    if not ((isinstance(below, GpuHashJoinExec) and below.join_type == "Inner") or isinstance(below, GpuFilterExec)):
+    if not ((isinstance(below, GpuHashJoinExec) and below.join_type in (("Inner", "Right") if right_joins else ("Inner",))) or isinstance(below, GpuFilterExec)):
         return plan
-    sc = _as_scan(below, join_filters)
+    sc = _as_scan(below, join_filters, right_joins)
     # a composite-key stage under the hash-keyed sink (TPC-H Q9's lineitem x partsupp profit by supplier) measured slower than the
     # unfused dfgpu_hashjoin -> dfgpu_agg (README): that shape stays unfused
     if sc is None or any(isinstance(k, list) for _, k, _ in sc.stages):
         return plan
-    vs = sc.virtual_schema()
     exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
+    if not _settle_right(sc, _read_names(plan, exprs)):
+        return plan
+    vs = sc.virtual_schema()
     group, nullable, bits = [], [], 0
     for g in plan.group_by:
         e = exprs.get(g)
@@ -1314,23 +1390,24 @@ def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False) -> Exe
             if pa.types.is_boolean(t) and a.func != "count":
                 return plan
         aggs.append((a.func, e, a.alias))
-    return GpuPipelineExec(sc, sink="hash", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, nullable=nullable)
+    return GpuPipelineExec(sc, sink="hash", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, nullable=nullable,
+                           fallback=plan if sc.has_right() else None)
 
 
-def fuse_join_filters(plan: ExecutionPlan) -> ExecutionPlan:
+def fuse_join_filters(plan: ExecutionPlan, right_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_hash_aggregates: its result when that rule fuses; otherwise the same
     shapes again with JoinFilters allowed on the Inner / RightSemi / RightAnti joins of a probe chain and on a Left / LeftSemi / LeftAnti
     join that is the last stage.  Each filter becomes its stage's filter (dfgpu_pipeline_set_stage_filter): a probe-side column maps to
     the probe chain's column, the build key to the probe key, other build columns to the stage's payload fields (a RightSemi /
     RightAnti build carries exactly the columns its filter reads).  A plan is left unchanged when a payload would exceed 64 bits, the
     filters 128 nodes, or an AND / OR has a right operand that can raise (÷, %, CAST, Decimal128 arithmetic)."""
-    fused = fuse_hash_aggregates(plan)
+    fused = fuse_hash_aggregates(plan, right_joins=right_joins)
     if fused is not plan:
         return fused
-    return fuse_hash_aggregates(plan, join_filters=True)
+    return fuse_hash_aggregates(plan, join_filters=True, right_joins=right_joins)
 
 
-def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
+def fuse_output_pipelines(plan: ExecutionPlan, right_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_join_filters: its result when that rule fuses; otherwise a top-level
     [ProjectionExec(columns only)] over a HashJoinExec(Inner / RightSemi / RightAnti) chain, as _as_scan accepts it with JoinFilters and
     with at least one stage, becomes ONE GpuPipelineExec over the ordered output sink (dfgpu_pipeline_sink_output) that emits the plan's
@@ -1341,18 +1418,26 @@ def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
     NULL payloads) runs the unfused joins instead, before any row is emitted.  The fused Inner join emits its rows in probe order, the
     reference's order for unique build keys.  Anything else (a bare FilterExec, Left / Right / Full joins, several keys,
     null-aware joins, computed projections) is returned unchanged."""
-    fused = fuse_join_filters(plan)
+    fused = fuse_join_filters(plan, right_joins)
     if fused is not plan:
         return fused
     join = plan.input if isinstance(plan, GpuProjectionExec) else plan
-    if not isinstance(join, GpuHashJoinExec) or join.join_type not in ("Inner", "RightSemi", "RightAnti"):
+    if not isinstance(join, GpuHashJoinExec) or join.join_type not in ("Inner", "RightSemi", "RightAnti") + (("Right",) if right_joins else ()):
         return plan
-    sc = _as_scan(join, join_filters=True)
+    sc = _as_scan(join, join_filters=True, right_joins=right_joins)
     if sc is None or not sc.stages:
+        return plan
+    pick = list(range(len(join.column_indices)))                                # the join's columns that form the output
+    if isinstance(plan, GpuProjectionExec):
+        names = [f.name for f in join.schema]
+        if not all(isinstance(e, Column) and names.count(e.name) == 1 for e, _ in plan.exprs):
+            return plan
+        pick = [names.index(e.name) for e, _ in plan.exprs]
+    if not _settle_right(sc, {join.schema.field(i).name for i in pick}):
         return plan
     vs = sc.virtual_schema()
     kind, pkey, build = sc.stages[-1]
-    n_below = len(vs) - (len(build.payload) if kind == D.STAGE_INNER else 0)   # the virtual columns the top join's probe side sees
+    n_below = len(vs) - (len(build.payload) if kind in (D.STAGE_INNER, D.STAGE_RIGHT) else 0)   # the virtual columns the top join's probe side sees
     keys = {bk: (pk, b) for k, p, b in sc.stages if k == D.STAGE_INNER for bk, pk in _key_pairs(p, b)}   # an Inner stage's build key -> its probe key
 
     def probe_col(name: str) -> int:
@@ -1365,19 +1450,13 @@ def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
             return i if i >= 0 and b.scan_field(name).type == vs.field(i).type else -1
         return -1
 
-    pick = list(range(len(join.column_indices)))                                # the join's columns that form the output
-    if isinstance(plan, GpuProjectionExec):
-        names = [f.name for f in join.schema]
-        if not all(isinstance(e, Column) and names.count(e.name) == 1 for e, _ in plan.exprs):
-            return plan
-        pick = [names.index(e.name) for e, _ in plan.exprs]
     cols = []
     for side, ix in (join.column_indices[i] for i in pick):
         if side == 1:
             at = probe_col(join.right.schema.field(ix).name)
         else:
             name = join.left.schema.field(ix).name
-            paired = dict(_key_pairs(pkey, build))
+            paired = dict(_key_pairs(pkey, build)) if kind != D.STAGE_RIGHT else {}   # a Right join's build key is NULL when unmatched
             if name in paired:
                 at = probe_col(paired[name])
                 at = at if at >= 0 and join.left.schema.field(ix).type == vs.field(at).type else -1
@@ -1390,6 +1469,24 @@ def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
         if k == D.STAGE_INNER and not b.payload:
             b.n_acc_words = max(b.n_acc_words, 1)
     return GpuPipelineExec(sc, sink="output", out_schema=plan.schema, out_cols=cols, fallback=plan)
+
+
+def fuse_right_joins(plan: ExecutionPlan) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_output_pipelines: its result when that rule fuses; otherwise the same
+    shapes again with HashJoinExec(Right) joins allowed in the probe chain (DFGPU_STAGE_RIGHT) — DataFusion's join selection puts the
+    smaller input on the build side, so `fact LEFT JOIN dimension` arrives as a Right join with the dimension as the build.  A Right join
+    qualifies with one key or a composite key, NullEqualsNothing, not null-aware and without a JoinFilter; its stage carries the build
+    columns read above it (a build key too: it is NULL on unmatched rows, so it never stands in for the probe key), at least one and at
+    most 64 bits, since only a lookup with payload enforces the unique keys a Right stage needs.  Its payload fields are nullable in the
+    virtual schema, as build_join_schema(..., "Right") makes them.  Sinks: the ordered output sink, the dense sink (group columns with
+    known bounds: source columns, or payload fields taken from a source column of the build side) and the hash sink (a RIGHT payload
+    group column declared nullable); never a build side or the join-keyed sink.  Whether the build keys are unique is known only once the
+    build has run, so every fused node keeps the plan as its fallback (a duplicate key runs the unfused joins, before any row is
+    emitted)."""
+    fused = fuse_output_pipelines(plan)
+    if fused is not plan:
+        return fused
+    return fuse_output_pipelines(plan, right_joins=True)
 
 
 def collect(plan: ExecutionPlan, ctx: Optional[TaskContext] = None) -> List[pa.RecordBatch]:

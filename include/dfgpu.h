@@ -406,8 +406,9 @@ void dfgpu_agg_destroy(dfgpu_agg* a);
  *                 optional accumulator words per record for an aggregation whose group keys are functionally
  *                 determined by the join key (group id == build row).
  * dfgpu_pipeline= source batch -> predicate -> probe stage(s) -> sink.
- * "virtual columns" of a pipeline: the input columns [0, n_cols) followed by the payload fields of every INNER, LEFT and
- * LEFT_ANTI stage in stage order; expressions, group columns, build payloads and outputs address this space. */
+ * "virtual columns" of a pipeline: the input columns [0, n_cols) followed by the payload fields of every INNER, LEFT, LEFT_ANTI and
+ * RIGHT stage in stage order; expressions, group columns, build payloads and outputs address this space.  A RIGHT stage's payload
+ * fields are the only nullable ones (NULL on a probe row that matched nothing; the slot then holds 0). */
 /* ===================================================================================== */
 typedef struct dfgpu_lookup dfgpu_lookup;
 typedef struct dfgpu_pipeline dfgpu_pipeline;
@@ -474,11 +475,19 @@ enum dfgpu_stage_kind {
   DFGPU_STAGE_MAYBE = 3,  /* membership pre-filter only (may have false positives, never false negatives): the dynamic filter a downstream
                            * join pushes into this scan (joins/hash_join/shared_bounds.rs); the exact join runs after the exchange */
   DFGPU_STAGE_LEFT = 4,   /* Left join (every build row, NULL-padded when no probe row matches) and LeftAnti join (the build rows no     */
-  DFGPU_STAGE_LEFT_ANTI = 5 /* probe row matches): the last stage only, with dfgpu_pipeline_sink_aggregate grouped on it (see there); the
+  DFGPU_STAGE_LEFT_ANTI = 5, /* probe row matches): the last stage only, with dfgpu_pipeline_sink_aggregate grouped on it (see there); the
                            * probe runs as for INNER (unmatched probe rows are dropped, the payload fields are virtual columns) */
+  DFGPU_STAGE_RIGHT = 6   /* Right join (every probe row, NULL-padded when no build row matches): every row reaching the stage continues,
+                           * a matched one with its build row's payload fields, an unmatched one (no partner, a NULL key, a composite key
+                           * that packs to the sentinel D) with every payload field of the stage NULL.  The row count never changes, so the
+                           * lookup must hold unique keys: it needs payload (its build refuses duplicate keys), and a key-only, bitmap or
+                           * filter-only lookup is DFGPU_ERR_UNSUPPORTED at dfgpu_pipeline_create.  Sinks: output (ordered: probe order,
+                           * unmatched rows where they occur, as dfgpu_hashjoin's Right join), dense and hash aggregates; the build, pack
+                           * and join-keyed aggregate sinks are DFGPU_ERR_UNSUPPORTED, and so is dfgpu_pipeline_set_stage_filter on any
+                           * stage of a pipeline with a RIGHT stage.  An aggregate argument reading a RIGHT payload field skips its NULLs. */
 };
 typedef struct dfgpu_pipeline_stage {
-  int32_t kind;          /* dfgpu_stage_kind: the pipeline input is the PROBE (right) side — Inner / RightSemi / RightAnti, and Left /
+  int32_t kind;          /* dfgpu_stage_kind: the pipeline input is the PROBE (right) side — Inner / RightSemi / RightAnti / Right, and Left /
                           * LeftAnti (LEFT / LEFT_ANTI) through the join-keyed aggregate sink.  LeftSemi is an INNER stage + the join-keyed
                           * aggregate sink with no aggregates, grouped on the key and payload of a lookup with unique keys */
   int32_t key_col;       /* input column holding the probe key (NULL keys never match, utils.rs:2146-2155) */
@@ -532,8 +541,8 @@ int dfgpu_pipeline_sink_build_composite(dfgpu_pipeline* p, dfgpu_lookup* target,
 int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, int32_t n_group,
                                   const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size);
 /* dense aggregate: AggregateExec over the surviving rows whose 0..8 group columns (virtual columns: input columns or payload
- * fields of INNER stages, integer-like, <= 64 bits) take values in small declared domains [key_min[g], key_max[g]] (column
- * statistics).  The group of a row is arithmetic, slot = sum_g stride_g * idx_g with idx_g = key - key_min[g] for a value and
+ * fields of INNER and RIGHT stages — an unmatched RIGHT row's field takes its column's NULL slot —, integer-like, <= 64 bits) take
+ * values in small declared domains [key_min[g], key_max[g]] (column statistics).  The group of a row is arithmetic, slot = sum_g stride_g * idx_g with idx_g = key - key_min[g] for a value and
  * key_max[g] - key_min[g] + 1 for NULL (a group of its own), row-major strides; no hash table.  The domain may have at most
  * DFGPU_DENSE_MAX_GROUPS slots, prod_g (key_max[g] - key_min[g] + 2), else DFGPU_ERR_UNSUPPORTED; a key outside its range at run
  * time is DFGPU_ERR_INVALID.  n_group = 0 is AggregateStream: exactly one output row, also for empty input (COUNT 0; SUM, MIN, MAX,
@@ -548,11 +557,12 @@ int dfgpu_pipeline_sink_aggregate_dense(dfgpu_pipeline* p, const int32_t* group_
                                         int32_t n_group, const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size);
 /* hash aggregate: AggregateExec over the surviving rows whose GROUP BY keys the join key does not determine (TPC-H Q15's revenue0:
  * l_suppkey; Q3 grouped by o_custkey).  The sink owns its group table.
- *  group_cols: 1..8 virtual columns (input columns or payload fields of INNER stages), integer-like, <= 8 bytes (Int8..Int64,
+ *  group_cols: 1..8 virtual columns (input columns or payload fields of INNER and RIGHT stages), integer-like, <= 8 bytes (Int8..Int64,
  *    UInt8..UInt64, Date32, Date64, Timestamp; dictionary-coded strings as their Int32 codes).  group_nullable[g] is the column's
  *    declared nullability (DataFusion's Field::is_nullable); NULL = none is nullable.  The columns are packed into a 128-bit tag,
  *    each at its width followed by one NULL bit when it is nullable; a key wider than 128 bits is DFGPU_ERR_UNSUPPORTED (dfgpu_agg
- *    carries wide keys).  NULL is a group of its own; a NULL in a column declared non-nullable is DFGPU_ERR_INVALID at the push.
+ *    carries wide keys).  NULL is a group of its own; a NULL in a column declared non-nullable is DFGPU_ERR_INVALID at the push
+ *    (a RIGHT stage's payload field is NULL on every unmatched row, so it is declared nullable).
  *  aggs: the functions, limits and result / state types of dfgpu_pipeline_sink_aggregate (<= 4; COUNT(*), COUNT, SUM, MIN, MAX, AVG
  *    over Float64 and Decimal128; Decimal128 AVG in Single modes only; MIN / MAX over Float32 rejected).  The sink sizes the record
  *    words itself: {tag_lo | tag_hi | row counter | the aggregates' words as dfgpu_pipeline_sink_aggregate lays them out, every SUM /
@@ -572,9 +582,9 @@ int dfgpu_pipeline_sink_aggregate_hash(dfgpu_pipeline* p, const int32_t* group_c
                                        int64_t capacity_hint);
 /* output: the surviving rows, columns = out_cols (1..16) of the virtual schema, input order preserved, sliced by batch_size (0 = one
  * batch).  Any input column may leave: widths 1, 2, 4, 8 and 16 bytes (Decimal128(p, s) included), with or without a validity bitmap
- * at any Arrow bit offset; payload fields leave too (they are never nullable).  An output column has a bitmap exactly when its input
- * column had one in that push (a column pushed with null_count 0 has none); once several pushes are merged, a column has one when any
- * push gave it one.  Returned bitmap columns report null_count = -1 (unknown), as dfgpu_exchange_columns does.  Boolean input
+ * at any Arrow bit offset; payload fields leave too: those of a RIGHT stage always with a bitmap (bit = the row matched), the others
+ * never nullable.  An input column leaves with a bitmap exactly when it had one in that push (a column pushed with null_count 0 has
+ * none); once several pushes are merged, a column has one when any push gave it one.  Returned bitmap columns report null_count = -1 (unknown), as dfgpu_exchange_columns does.  Boolean input
  * columns are refused by the push (DFGPU_ERR_UNSUPPORTED), so they cannot be output. */
 int dfgpu_pipeline_sink_output(dfgpu_pipeline* p, const int32_t* out_cols, int32_t n_out, int64_t batch_size);
 /* the same, row order unspecified (what a RepartitionExec consumer sees anyway, repartition/mod.rs:1320-1400): runs on the two-phase
