@@ -890,7 +890,7 @@ __global__ void __launch_bounds__(256) wide_key_kernel(WideKeyCols kc, int64_t n
           case 0: v = bit_get((const uint8_t*)kc.ptr[c], kc.voff[c] + row) ? 1ull : 0ull; break;
           case 1: v = ((const uint8_t*)kc.ptr[c])[row]; break;
           case 2: v = ((const uint16_t*)kc.ptr[c])[row]; break;
-          case 4: v = ((const uint32_t*)kc.ptr[c])[row]; if (kc.is_float[c] && (v & 0x7FFFFFFFull) == 0) v = 0; break;   // -0.0 = +0.0
+          case 4: v = ((const uint32_t*)kc.ptr[c])[row]; if (kc.is_float[c] && (v & 0x7FFFFFFFull) == 0) v = 0; break;   // -0.0 hashes as +0.0: only the equality conjunct tells them apart
           case 16: v = ((const uint64_t*)kc.ptr[c])[2 * row]; v2 = ((const uint64_t*)kc.ptr[c])[2 * row + 1]; break;
           default: v = ((const uint64_t*)kc.ptr[c])[row]; if (kc.is_float[c] && (v << 1) == 0) v = 0; break;
         }
@@ -946,6 +946,11 @@ static void make_keycols(const std::vector<DCol>& cols, const std::vector<int>& 
   }
 }
 
+// the wide-key equality conjunct reads a float key component as the unsigned type of its width, so it compares the bits: -0.0 does not
+// join +0.0 and a NaN joins a NaN with the same bits, as on the exact 64-bit tag (the reference hashes a float by its bits,
+// hash_utils.rs hash_float_value, so unequal bits never reach its equality check)
+static int wide_key_eq_type(int t) { return t == DFGPU_FLOAT32 ? DFGPU_UINT32 : (t == DFGPU_FLOAT64 ? DFGPU_UINT64 : t); }
+
 static void check_join_keys(dfgpu_hashjoin* j) {
   int bits = 0;
   bool wide = false;
@@ -971,8 +976,8 @@ static void check_join_keys(dfgpu_hashjoin* j) {
     const int nk = (int)j->on_build.size();
     std::vector<int32_t> types;
     for (int c = 0; c < nk; ++c) {
-      j->filt_side.push_back(0); j->filt_index.push_back(j->wide_on_build[c]); types.push_back(j->build_types[j->wide_on_build[c]]);
-      j->filt_side.push_back(1); j->filt_index.push_back(j->wide_on_probe[c]); types.push_back(j->probe_types[j->wide_on_probe[c]]);
+      j->filt_side.push_back(0); j->filt_index.push_back(j->wide_on_build[c]); types.push_back(wide_key_eq_type(j->build_types[j->wide_on_build[c]]));
+      j->filt_side.push_back(1); j->filt_index.push_back(j->wide_on_probe[c]); types.push_back(wide_key_eq_type(j->probe_types[j->wide_on_probe[c]]));
     }
     const int eq = j->opt.null_equality == DFGPU_NULL_EQUALS_NULL ? DFGPU_OP_IS_NOT_DISTINCT_FROM : DFGPU_OP_EQ;
     auto node = [](int kind, int a) { dfgpu_expr_node nd; memset(&nd, 0, sizeof(nd)); nd.kind = kind; nd.a = a; return nd; };
@@ -1247,9 +1252,11 @@ static void push_probe_filtered(dfgpu_hashjoin* j, const std::vector<DCol>& cols
   int64_t kept = 0;
   if (total > 0) {
     std::vector<DCol> inter;
-    for (size_t c = 0; c < j->filt_side.size(); ++c)
+    for (size_t c = 0; c < j->filt_side.size(); ++c) {
       inter.push_back(j->filt_side[c] == 0 ? take_column(ctx, j->build_cols[j->filt_index[c]], bidx.as<uint32_t>(), total, false)
                                            : take_column(ctx, cols[j->filt_index[c]], pidx.as<uint32_t>(), total, false));
+      if (j->wide && c < 2 * j->wide_on_build.size()) inter.back().type = wide_key_eq_type(inter.back().type);   // planned by check_join_keys
+    }
     EvalResult ev = evaluate_expr(ctx, j->filt_plan, inter, total, false, true);
     DevBuf sel;
     kept = compact_flag_indices(ctx, ev.select_words.as<uint32_t>(), total, 1, &sel);
@@ -1832,7 +1839,7 @@ int dfgpu_hashjoin_set_filter(dfgpu_hashjoin* j, const int32_t* col_side, const 
   if (j->wide) {   // key equality stays the first conjunct; the user's column references move behind the key columns
     DF_CHECK(j->filt_side.size() == 2 * j->wide_on_build.size(), DFGPU_ERR_STATE, "set_filter called twice");
     fside = j->filt_side; findex = j->filt_index;
-    for (size_t c = 0; c < fside.size(); ++c) types.push_back((fside[c] == 0 ? j->build_types : j->probe_types)[findex[c]]);
+    for (size_t c = 0; c < fside.size(); ++c) types.push_back(wide_key_eq_type((fside[c] == 0 ? j->build_types : j->probe_types)[findex[c]]));
     nodes = j->wide_expr;
     shift = (int)fside.size();
   }
@@ -1923,6 +1930,7 @@ int64_t dfgpu_hashjoin_metric(dfgpu_hashjoin* j, const char* name) {
   if (s == "output_rows") return j->m_output_rows;
   if (s == "output_batches") return j->m_output_batches;
   if (s == "array_map_created_count") return j->m_array_map;
+  if (s == "inline_payload_words") return j->inline_ok ? j->inline_words : 0;   // 2: the build payload rides beside the key in the table
   if (s == "probe_hits") return j->m_probe_hits;
   if (s == "radix_partitioned_probes") return j->m_radix_probes;
   if (s == "pipelined_host_probes") return j->m_pipelined_probes;   // host pushes probed by push_probe_host_pipelined

@@ -305,7 +305,9 @@ void dfgpu_hashjoin_default_options(dfgpu_hashjoin_options* o);
  * (0 = build/left, 1 = probe/right, 2 = mark column) — ColumnIndex of joins/utils.rs:1332-1387.
  * Keys: up to 4 columns of <= 64 bits together are stored exactly in the table (one probe = one compare); anything else — up to 8
  * columns, wider together, a Decimal128 / Boolean key — is looked up by a hash of the key columns and verified on the candidate
- * pairs like the reference's equal_rows_arr (joins/utils.rs:2191-2257): same results, generic probe path. */
+ * pairs like the reference's equal_rows_arr (joins/utils.rs:2191-2257): same results, generic probe path.
+ * Float key components compare by their bits on both paths, as the reference hashes them (hash_utils.rs hash_float_value): -0.0 does
+ * not join +0.0, and a NaN joins a NaN with the same bits only.  (GROUP BY folds -0.0 into +0.0: a different rule.) */
 int dfgpu_hashjoin_create(dfgpu_ctx* ctx,
                           const int32_t* build_types, int32_t n_build_cols,
                           const int32_t* probe_types, int32_t n_probe_cols,
