@@ -13,6 +13,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdfgpu.so")
+STRINGS_LIB_PATH = os.path.join(_HERE, "libdfgpu_strings.so")   # include/dfgpu_strings.h: LIKE over string columns (own library)
 
 # ---- enums (mirror include/dfgpu.h) -------------------------------------------------------
 OK, END = 0, 1
@@ -1023,3 +1024,123 @@ class Exchange:
         if self.h:
             self.ctx.lib.dfgpu_exchange_destroy(self.h)
             self.h = C.c_void_p()
+
+
+# ---- string predicates: libdfgpu_strings.so (include/dfgpu_strings.h) -------------------------
+STRING_UTF8, STRING_LARGE_UTF8, STRING_UTF8_VIEW = 1, 2, 3
+LIKE_NEGATED, LIKE_CASE_INSENSITIVE = 1, 2
+LIKE_MAX_PATTERN_BYTES, LIKE_MAX_SEGMENTS = 256, 16
+
+# every symbol include/dfgpu_strings.h declares
+STRINGS_EXPORTS = ["dfgpu_like", "dfgpu_like_codes", "dfgpu_strings_last_error"]
+
+
+class StringColumn(C.Structure):
+    _fields_ = [("layout", C.c_int32), ("n_data_buffers", C.c_int32), ("length", C.c_int64), ("offset", C.c_int64),
+                ("null_count", C.c_int64), ("offsets_or_views", C.c_void_p), ("data_buffers", C.POINTER(C.c_void_p)),
+                ("validity", C.c_void_p)]
+
+
+_strings_lib = None
+
+
+def load_strings_library() -> C.CDLL:
+    """dlopen libdfgpu_strings.so (built next to libdfgpu.so by __graft_entry__.build()). Raises if absent."""
+    global _strings_lib
+    if _strings_lib is not None:
+        return _strings_lib
+    if not os.path.exists(STRINGS_LIB_PATH):
+        raise ImportError(f"{STRINGS_LIB_PATH} not built: run `python -c 'import __graft_entry__ as g; g.build()'` (there is no CPU fallback)")
+    lib = C.CDLL(STRINGS_LIB_PATH)
+    vp = C.c_void_p
+    lib.dfgpu_like.restype = C.c_int
+    lib.dfgpu_like.argtypes = [vp, C.POINTER(StringColumn), C.c_char_p, C.c_int64, C.c_int32, vp, vp]
+    lib.dfgpu_like_codes.restype = C.c_int
+    lib.dfgpu_like_codes.argtypes = [vp, C.POINTER(Column), vp, C.c_int64, vp, vp]
+    lib.dfgpu_strings_last_error.restype = C.c_char_p
+    lib.dfgpu_strings_last_error.argtypes = []
+    _strings_lib = lib
+    return lib
+
+
+def _strings_check(rc: int):
+    if rc < 0:
+        raise DfgpuError(rc, load_strings_library().dfgpu_strings_last_error().decode())
+
+
+class DeviceStrings:
+    """a pyarrow string / large_string / string_view array copied to HBM buffer for buffer, so the array's slice offset (rows into the
+    offsets or views and the validity bitmap) is kept as it is"""
+
+    def __init__(self, ctx: Context, arr):
+        import pyarrow as pa
+        if isinstance(arr, pa.ChunkedArray):
+            arr = arr.combine_chunks()
+        t = arr.type
+        if pa.types.is_string(t):
+            self.layout, width = STRING_UTF8, 4
+        elif pa.types.is_large_string(t):
+            self.layout, width = STRING_LARGE_UTF8, 8
+        elif pa.types.is_string_view(t):
+            self.layout, width = STRING_UTF8_VIEW, 16
+        else:
+            raise NotImplementedError(f"This feature is not implemented: LIKE on the GPU over Arrow type {t}")
+        self.ctx, self.length, self.offset, self.null_count = ctx, len(arr), arr.offset, arr.null_count
+        bufs = arr.buffers()
+
+        def up(buf, nbytes=None):
+            raw = np.frombuffer(buf, np.uint8) if buf is not None else np.zeros(0, np.uint8)
+            return ctx.to_device(raw if nbytes is None else raw[:nbytes])
+        nel = arr.offset + len(arr) + (0 if self.layout == STRING_UTF8_VIEW else 1)
+        self.index = up(bufs[1], nel * width)                  # offsets or views of rows [0, offset + length)
+        self.validity = up(bufs[0]) if bufs[0] is not None and arr.null_count > 0 else None
+        self.data = [up(b) for b in bufs[2:]]
+        self._ptrs = (C.c_void_p * max(len(self.data), 1))(*[d.ptr for d in self.data])
+
+    def c(self) -> StringColumn:
+        s = StringColumn()
+        s.layout, s.n_data_buffers, s.length, s.offset, s.null_count = self.layout, len(self.data), self.length, self.offset, self.null_count
+        s.offsets_or_views = self.index.ptr
+        s.data_buffers = C.cast(self._ptrs, C.POINTER(C.c_void_p))
+        s.validity = self.validity.ptr if self.validity is not None else None
+        return s
+
+
+def _pattern_bytes(pattern) -> bytes:
+    return pattern if isinstance(pattern, (bytes, bytearray)) else str(pattern).encode("utf-8")
+
+
+def like(ctx: Context, strings, pattern, negated: bool = False, case_insensitive: bool = False) -> DeviceColumn:
+    """`strings [NOT] LIKE pattern` (dfgpu_like) -> a UINT8 DeviceColumn in {0, 1}, NULL where the string is NULL.  strings: a
+    DeviceStrings or a pyarrow string / large_string / string_view array.  DfgpuError(DFGPU_ERR_UNSUPPORTED) for what the GPU refuses."""
+    ds = strings if isinstance(strings, DeviceStrings) else DeviceStrings(ctx, strings)
+    lib = load_strings_library()
+    n = ds.length
+    values = DeviceBuffer(ctx, n)
+    validity = DeviceBuffer(ctx, (n + 7) // 8) if ds.validity is not None else None
+    pat = _pattern_bytes(pattern)
+    flags = (LIKE_NEGATED if negated else 0) | (LIKE_CASE_INSENSITIVE if case_insensitive else 0)
+    col = ds.c()
+    _strings_check(lib.dfgpu_like(ctx.lib.dfgpu_ctx_stream(ctx.h), C.byref(col), pat, len(pat), flags, C.c_void_p(values.ptr),
+                                  C.c_void_p(validity.ptr) if validity is not None else None))
+    return DeviceColumn(ctx, UINT8, n, values, validity, ds.null_count if validity is not None else 0)
+
+
+def like_codes(ctx: Context, codes, code_match: DeviceColumn, n_codes: int) -> DeviceColumn:
+    """the predicate over dictionary codes (dfgpu_like_codes): codes is an INT32 DeviceColumn / Column, code_match the UINT8 value of
+    each distinct string (like() over the dictionary values) -> a UINT8 DeviceColumn, NULL where the code is NULL"""
+    col = codes.c() if not isinstance(codes, Column) else codes
+    lib = load_strings_library()
+    n = int(col.length)
+    values = DeviceBuffer(ctx, n)
+    validity = DeviceBuffer(ctx, (n + 7) // 8) if col.validity else None
+    _strings_check(lib.dfgpu_like_codes(ctx.lib.dfgpu_ctx_stream(ctx.h), C.byref(col), C.c_void_p(code_match.values.ptr), int(n_codes),
+                                        C.c_void_p(values.ptr), C.c_void_p(validity.ptr) if validity is not None else None))
+    return DeviceColumn(ctx, UINT8, n, values, validity, int(col.null_count) if validity is not None else 0)
+
+
+def device_column_numpy(col: DeviceColumn):
+    """(values, valid mask or None) of a DeviceColumn on the host"""
+    v = col.values.to_numpy(NP_OF_TYPE[col.type], col.length) if col.length else np.zeros(0, NP_OF_TYPE[col.type])
+    valid = None if col.validity is None else unpack_bits(col.validity.to_numpy(np.uint8), col.length)
+    return v, valid

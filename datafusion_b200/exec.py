@@ -197,6 +197,22 @@ class CastExpr(Expr):
         out.append((D.EXPR_CAST, 0, type_id(self.to), 0, 0, 0.0))
 
 
+class LikeExpr(Expr):
+    """expressions/like.rs: `expr [NOT] [I]LIKE pattern`, evaluated by arrow-string's like / nlike / ilike / nilike.  Boolean.  It has no
+    expression program of its own: plan_like_predicates computes a LIKE on a string column with a literal pattern as a UINT8 mask column
+    (GpuLikeExec, libdfgpu_strings.so) and compares `mask = 1`.  A str pattern is a Utf8 literal."""
+
+    def __init__(self, expr: Expr, pattern: Union[Expr, str, None], negated: bool = False, case_insensitive: bool = False):
+        self.expr, self.negated, self.case_insensitive = expr, negated, case_insensitive
+        self.pattern = pattern if isinstance(pattern, Expr) else Literal(pattern, pa.string())
+
+    def data_type(self, schema): return pa.bool_()
+
+    def rpn(self, schema, out):
+        raise NotImplementedError("This feature is not implemented: LikeExpr has no GPU expression program (plan_like_predicates turns a LIKE "
+                                  "on a string column with a literal pattern into a mask column)")
+
+
 def col(name: str) -> Column: return Column(name)
 def lit(value, type: Optional[pa.DataType] = None) -> Literal: return Literal(value, type)
 
@@ -344,6 +360,41 @@ class DictionaryDecodeExec(ExecutionPlan):
         for rb in self.input.execute(ctx):
             cols = [sd.decode(rb.column(i), self.to) if f.name in self.names else rb.column(i) for i, f in enumerate(rb.schema)]
             yield pa.RecordBatch.from_arrays(cols, schema=self.schema)
+
+
+class GpuLikeExec(ExecutionPlan):
+    """LikeExpr over string columns -> one UINT8 mask column per LIKE (`name`, appended; NULL where the string is NULL), and the input
+    without the columns `drop`.  A Utf8 / LargeUtf8 / Utf8View column runs dfgpu_like; an INT32 column of DictionaryEncodeExec codes
+    (`dictionary_of` given) matches the dictionary's distinct values with dfgpu_like, then maps each row's code with dfgpu_like_codes."""
+
+    def __init__(self, input: ExecutionPlan, likes: Sequence[Tuple[LikeExpr, str]], drop: Sequence[str] = (), dictionary_of: Optional["callable"] = None):
+        self.input, self.likes, self.drop, self.dictionary_of = input, list(likes), set(drop), dictionary_of
+        self.schema = pa.schema([f for f in input.schema if f.name not in self.drop] + [pa.field(name, pa.uint8(), True) for _, name in self.likes])
+
+    def children(self): return [self.input]
+
+    def _mask(self, ctx: TaskContext, arr: pa.Array, e: LikeExpr) -> pa.Array:
+        import numpy as np
+        if isinstance(arr, pa.ChunkedArray):
+            arr = arr.combine_chunks()
+        if _is_string_like(arr.type):
+            m = D.like(ctx.gpu, arr, e.pattern.value, e.negated)
+        else:                                              # INT32 codes of DictionaryEncodeExec
+            dic = self.dictionary_of(ctx).dic
+            n = dic.size()
+            values = pa.array([dic.value(i) for i in range(n)], pa.binary()).cast(pa.string())
+            code_match = D.like(ctx.gpu, values, e.pattern.value, e.negated)
+            codes = D.DeviceColumn.from_host(ctx.gpu, D.HostColumn(np.asarray(arr.fill_null(0)), None if arr.null_count == 0 else np.asarray(arr.is_valid())))
+            m = D.like_codes(ctx.gpu, codes, code_match, n)
+        v, valid = D.device_column_numpy(m)
+        return pa.array(v, pa.uint8(), mask=None if valid is None else ~valid)
+
+    def execute(self, ctx):
+        isch = self.input.schema
+        for rb in self.input.execute(ctx):
+            masks = [self._mask(ctx, rb.column(isch.get_field_index(e.expr.name)), e) for e, _ in self.likes]
+            cols = [rb.column(i) for i, f in enumerate(isch) if f.name not in self.drop]
+            yield pa.RecordBatch.from_arrays(cols + masks, schema=self.schema)
 
 
 def plan_string_dictionary():
@@ -744,6 +795,8 @@ def _expr_names(e: Expr) -> set:
         return _expr_names(e.left) | _expr_names(e.right)
     if isinstance(e, (UnaryExpr, CastExpr)):
         return _expr_names(e.arg)
+    if isinstance(e, LikeExpr):
+        return _expr_names(e.expr) | _expr_names(e.pattern)
     return set()
 
 
@@ -1036,6 +1089,8 @@ _ERR_UNSUPPORTED = -3   # DFGPU_ERR_UNSUPPORTED (include/dfgpu.h)
 def _source_bounds(source: ExecutionPlan, name: str) -> Optional[Tuple[int, int]]:
     """(min, max) of an integer-like source column, when known at planning time.  The twin reads a MemoryExec's batches; DataFusion
     has them as ColumnStatistics::{min_value, max_value} of partition_statistics.  None when unknown (or no non-NULL value)."""
+    if isinstance(source, GpuLikeExec) and source.input.schema.get_field_index(name) >= 0:
+        return _source_bounds(source.input, name)        # a column the LIKE pass carries through
     if not isinstance(source, MemoryExec):
         return None
     t = source.schema.field(name).type
@@ -1487,6 +1542,97 @@ def fuse_right_joins(plan: ExecutionPlan) -> ExecutionPlan:
     if fused is not plan:
         return fused
     return fuse_output_pipelines(plan, right_joins=True)
+
+
+# ---------------------------------------------------------------------------------------------
+# LIKE predicates — a mask column computed ahead of the filter (libdfgpu_strings.so)
+# ---------------------------------------------------------------------------------------------
+def _like_on_gpu(e: LikeExpr, schema: pa.Schema, coded: set) -> bool:
+    """LIKE / NOT LIKE of a Utf8, LargeUtf8 or Utf8View column (or one DictionaryEncodeExec coded: `coded`) with a Utf8 literal pattern
+    without `\\`; a NULL pattern too (the predicate folds to NULL)"""
+    if e.case_insensitive or not isinstance(e.expr, Column) or not isinstance(e.pattern, Literal):
+        return False
+    p = e.pattern.value
+    if p is not None and (not isinstance(p, str) or "\\" in p):
+        return False
+    ix = schema.get_field_index(e.expr.name)
+    return ix >= 0 and (e.expr.name in coded or (_is_string_like(schema.field(ix).type) and not pa.types.is_dictionary(schema.field(ix).type)))
+
+
+def _rewrite_likes(e: Expr, schema: pa.Schema, coded: set, taken: set, likes: list) -> Optional[Expr]:
+    """e with every LIKE that runs on the GPU replaced by `mask = 1` (appended to likes as (LikeExpr, mask name)); None when a LIKE that
+    cannot run there remains"""
+    if isinstance(e, LikeExpr):
+        if not _like_on_gpu(e, schema, coded):
+            return None
+        if e.pattern.value is None:
+            return Literal(None, pa.bool_())
+        name = f"__like_{len(likes)}"
+        while name in taken:
+            name = "_" + name
+        taken.add(name)
+        likes.append((e, name))
+        return BinaryExpr(Column(name), D.OP_EQ, Literal(1, pa.uint8()))
+    if isinstance(e, BinaryExpr):
+        l = _rewrite_likes(e.left, schema, coded, taken, likes)
+        r = None if l is None else _rewrite_likes(e.right, schema, coded, taken, likes)
+        return None if r is None else (e if (l is e.left and r is e.right) else BinaryExpr(l, e.op, r))
+    if isinstance(e, (UnaryExpr, CastExpr)):
+        a = _rewrite_likes(e.arg, schema, coded, taken, likes)
+        if a is None:
+            return None
+        if a is e.arg:
+            return e
+        return UnaryExpr(e.kind, a) if isinstance(e, UnaryExpr) else CastExpr(a, e.to)
+    return e
+
+
+def _with_children(plan: ExecutionPlan, fn) -> ExecutionPlan:
+    """plan with fn applied to its input / left / right children (a shallow copy when one changes)"""
+    import copy
+    changed = {}
+    for attr in ("input", "left", "right"):
+        ch = getattr(plan, attr, None)
+        if isinstance(ch, ExecutionPlan):
+            new = fn(ch)
+            if new is not ch:
+                changed[attr] = new
+    if not changed:
+        return plan
+    out = copy.copy(plan)
+    for k, v in changed.items():
+        setattr(out, k, v)
+    if hasattr(out, "_metrics"):
+        out._metrics = {}
+    return out
+
+
+def plan_like_predicates(plan: ExecutionPlan) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §2c), ahead of the fusion rules: every FilterExec whose predicate holds LikeExpr(column,
+    Utf8 literal) over a Utf8, LargeUtf8 or Utf8View column, or over a column DictionaryEncodeExec coded, gets a GpuLikeExec under it that
+    appends one UINT8 mask per LIKE and drops the string columns nothing else reads; each LIKE becomes `mask = 1` (Kleene logic holds: a
+    NULL mask gives NULL) and the filter projects exactly its old output, so its schema is unchanged.  A filter stays as it was when its
+    predicate holds any other LIKE (ILIKE, a column pattern, a `\\` in the pattern) or when a Utf8 column a LIKE reads is also read
+    above the filter.  A NULL literal pattern folds to a NULL predicate.  The fusion rules then treat the GpuLikeExec as the pipeline's
+    source, as they treat any other node under a filter."""
+    plan = _with_children(plan, plan_like_predicates)
+    if not isinstance(plan, GpuFilterExec):
+        return plan
+    inner = plan.input
+    isch = inner.schema
+    coded = {isch.field(i).name for i in inner.string_cols} if isinstance(inner, DictionaryEncodeExec) else set()
+    likes: list = []
+    pred = _rewrite_likes(plan.predicate, isch, coded, set(isch.names), likes)
+    if pred is None or pred is plan.predicate:
+        return plan
+    out_names = [f.name for f in plan.schema]
+    raw = {e.expr.name for e, _ in likes if e.expr.name not in coded}
+    if raw & set(out_names):
+        return plan                                       # a string column read above the filter
+    drop = raw - _expr_names(pred)
+    below = GpuLikeExec(inner, likes, drop, inner.dictionary_of if coded else None) if likes else inner
+    projection = [below.schema.get_field_index(n) for n in out_names]
+    return GpuFilterExec(pred, below, projection, plan.fetch)
 
 
 def collect(plan: ExecutionPlan, ctx: Optional[TaskContext] = None) -> List[pa.RecordBatch]:
