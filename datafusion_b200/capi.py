@@ -170,7 +170,7 @@ EXPORTS = [
     "dfgpu_pipeline_sink_aggregate_hash", "dfgpu_pipeline_sink_output",
     "dfgpu_pipeline_push_host", "dfgpu_pipeline_push_device", "dfgpu_pipeline_push_arrow", "dfgpu_pipeline_finish",
     "dfgpu_pipeline_next", "dfgpu_pipeline_metric", "dfgpu_pipeline_destroy",
-    "dfgpu_lookup_create_composite", "dfgpu_pipeline_set_stage_keys", "dfgpu_pipeline_sink_build_composite",
+    "dfgpu_lookup_create_composite", "dfgpu_pipeline_set_stage_keys", "dfgpu_pipeline_sink_build_composite", "dfgpu_pipeline_set_stage_full",
     "dfgpu_dictionary_create", "dfgpu_dictionary_unify", "dfgpu_dictionary_code", "dfgpu_dictionary_size", "dfgpu_dictionary_value",
     "dfgpu_dictionary_remap", "dfgpu_dictionary_destroy",
 ]
@@ -296,6 +296,7 @@ def load_library() -> C.CDLL:
     sig("dfgpu_pipeline_sink_build", C.c_int, [vp, vp, i32, P(i32), i32])
     sig("dfgpu_pipeline_sink_build_composite", C.c_int, [vp, vp, P(i32), i32, P(i32), i32])
     sig("dfgpu_pipeline_set_stage_keys", C.c_int, [vp, i32, P(i32), i32])
+    sig("dfgpu_pipeline_set_stage_full", C.c_int, [vp, i32])
     sig("dfgpu_pipeline_sink_aggregate", C.c_int, [vp, P(i32), i32, P(PipelineAgg), i32, i32, i64])
     sig("dfgpu_pipeline_sink_aggregate_dense", C.c_int, [vp, P(i32), P(i64), P(i64), i32, P(PipelineAgg), i32, i32, i64])
     sig("dfgpu_pipeline_sink_aggregate_hash", C.c_int, [vp, P(i32), P(i32), i32, P(PipelineAgg), i32, i32, i64, i64])
@@ -858,6 +859,11 @@ class Pipeline(_Operator):
     def set_stage_keys(self, stage: int, key_cols):
         """composite key of probe stage `stage`: the input columns of the lookup's components, in order"""
         self.ctx.check(self.ctx.lib.dfgpu_pipeline_set_stage_keys(self.h, int(stage), _i32arr(list(key_cols)), len(key_cols)))
+
+    def set_stage_full(self, stage: int):
+        """turn RIGHT stage `stage` into a Full join: at finish, the build rows no probe row matched follow as rows whose input columns are
+        NULL (the lookup needs payload and n_acc_words >= 1; call before the sink)"""
+        self.ctx.check(self.ctx.lib.dfgpu_pipeline_set_stage_full(self.h, int(stage)))
 
     def set_stage_filter(self, stage: int, nodes):
         """JoinFilter of probe stage `stage`: RPN over the input columns, the payload fields of the INNER / LEFT / LEFT_ANTI stages up to

@@ -410,7 +410,8 @@ __device__ __forceinline__ uint32_t valid8(const ColRef& c, int64_t row0, int64_
 //              7, 8 or DFGPU_PIPE_VAR): phase A skips a RIGHT stage (it drops nothing); phase B probes it like an INNER hash stage but keeps
 //              every row, with the stage's bit of pvalid cleared and its payload word 0 on a miss.  pvalid rides behind the payload words as
 //              ext[kExtValid], so the interpreters' XN instantiations see the fields as NULL; the output (with bit 9), dense and hash
-//              sinks read it for the fields they take directly.
+//              sinks read it for the fields they take directly.  A FULL stage (kStageFull: a RIGHT stage turned into a Full join by
+//              dfgpu_pipeline_set_stage_full) runs the same path and also marks each record it matches (mark_visited).
 // DFGPU_PIPE_VAR selects the instantiation (aggregate sink; bits 1 and 5 also for the pack sink, bit 1 for the unordered-output sink); 0 is the
 // kernel without any of them, 11 the default.  Tried and removed: four instead of two survivors per lane and phase-B round; prefetching the
 // table record and the argument sectors already when a row passes the membership filter in phase A (the prefetches of five tiles queue up
@@ -492,6 +493,14 @@ constexpr int kFiltParamsOff = kDenseParamsOff + (int)(((sizeof(DenseParams) > s
 // ------------------------------------------------------------------------------------------
 constexpr int kVarOutCols = 512;
 constexpr int kVarRight = 1024, kStageRight = 6;   // pipe_kernel VAR bit 10; DFGPU_STAGE_RIGHT
+// a RIGHT stage of a Full join (dfgpu_pipeline_set_stage_full), a kind private to the library: StageDev.kind of that stage, which the host
+// keeps as DFGPU_STAGE_RIGHT.  The RIGHT instantiations treat both kinds alike (kind >= kStageRight)
+constexpr int kStageFull = 7, kVisitedWord = 2;   // the visited mark: word 2 of the {key, payload, acc...} record, the first accumulator word
+// a FULL stage's match: mark the record visited.  The word shares the 32-byte sector of the {key, payload} just read; the store is made
+// only while the word is 0 (once per record, not once per matching row) and needs no atomic, as every writer stores the same 1
+__device__ __forceinline__ void mark_visited(unsigned long long* rec) {
+  if (__ldcg(rec + kVisitedWord) == 0ull) __stcg(rec + kVisitedWord, 1ull);
+}
 struct OutValid { uint32_t* valid[kMaxPipeCols]; /* nullptr: the column leaves without a bitmap */ };
 static_assert(kDenseParamsOff + (int)sizeof(OutValid) <= kFiltParamsOff, "OutValid fits the sink's block");
 // one 16-byte value (Decimal128): Arrow promises only 8-byte alignment of a sliced input buffer
@@ -775,7 +784,7 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
 #pragma unroll 1
       for (int s = 0; s < sp.n_stages; ++s) {
         const StageDev& st = sp.stage[s];
-        if constexpr (RIGHT) if (st.kind == kStageRight) continue;   // drops nothing: no NULL-key mask, no membership test
+        if constexpr (RIGHT) if (st.kind >= kStageRight) continue;   // RIGHT / FULL drop nothing: no NULL-key mask, no membership test
         const bool bitmap = st.lk.mode == LK_BITMAP;
         if constexpr (FILT) if (bitmap && st.kind == DFGPU_STAGE_ANTI && fpp->n[s] > 0) continue;   // a key match alone drops nothing: phase B
         if (!bitmap && !(st.lk.bloom && st.kind != DFGPU_STAGE_ANTI)) {   // nothing cheap to test; NULL keys of an inner / semi stage still drop here
@@ -964,8 +973,12 @@ __global__ void __launch_bounds__(kPipeThreads, (((VAR & 64) && SINK == SINK_PAC
               if (SINK == SINK_AGG && s == sp.agg_stage && (!FILT || found[u])) arec[u] = st.lk.recs + slot[u] * (uint64_t)st.lk.stride;
             }
           }
-          if constexpr (RIGHT) if (st.kind == kStageRight) { if (!found[u]) pvalid[u] &= ~(1u << s); continue; }   // keeps the row
+          if constexpr (RIGHT) if (st.kind >= kStageRight) { if (!found[u]) pvalid[u] &= ~(1u << s); continue; }   // keeps the row
           live[u] = live[u] && (st.kind == DFGPU_STAGE_ANTI ? !found[u] : found[u]);
+        }
+        if constexpr (RIGHT) if (st.kind == kStageFull) {   // a FULL stage's matches mark their records
+#pragma unroll
+          for (int u = 0; u < PB; ++u) if (found[u]) mark_visited(st.lk.recs + slot[u] * (uint64_t)st.lk.stride);
         }
       }
       // ---- sink ----
@@ -1496,7 +1509,12 @@ __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ 
             while (true) {
               const unsigned long long* r = st.lk.recs + slot * (uint64_t)st.lk.stride;
               const unsigned long long ck = __ldcg(r);
-              if (ck == key) { found = true; if (st.lk.has_payload) pay[s][k] = __ldcg(r + 1); break; }
+              if (ck == key) {
+                found = true;
+                if (st.lk.has_payload) pay[s][k] = __ldcg(r + 1);
+                if constexpr (RIGHT) if (st.kind == kStageFull) mark_visited(st.lk.recs + slot * (uint64_t)st.lk.stride);
+                break;
+              }
               if (ck == kEmptyKey) break;
               if (++slot == st.lk.cap) slot = 0;
             }
@@ -1513,7 +1531,7 @@ __device__ __forceinline__ void pipe_output_tile(const PipeParams* __restrict__ 
           err = eo[0];
         }
       }
-      if constexpr (RIGHT) if (st.kind == kStageRight) { if (!found) pvalid[k] &= ~(1u << s); continue; }   // keeps the row
+      if constexpr (RIGHT) if (st.kind >= kStageRight) { if (!found) pvalid[k] &= ~(1u << s); continue; }   // keeps the row
       alive[k] = st.kind == DFGPU_STAGE_ANTI ? !found : found;
     }
   }
@@ -1966,6 +1984,7 @@ struct dfgpu_lookup {
   int64_t rows = 0, rehashes = 0;
   int64_t null_keys = 0;   // build rows pushed with a NULL key (counted before the predicate): never inserted, so a LEFT / LEFT_ANTI stage cannot emit them
   bool acc_claimed = false, filter_only = false;
+  bool marks_taken = false;   // a FULL stage's visited marks live in the first accumulator word: one FULL pipeline, until dfgpu_lookup_clear
   // composite key (dfgpu_lookup_create_composite): the key is the packed tuple of these components, in [0, domain)
   std::vector<int> comp_types; std::vector<int64_t> comp_min; std::vector<uint64_t> comp_range, comp_stride; uint64_t domain = 0;
 };
@@ -1980,6 +1999,10 @@ struct dfgpu_pipeline {
   ExprPlan pred;
   std::vector<dfgpu_pipeline_stage> stages;
   bool has_right = false;   // a RIGHT stage: every kernel runs its VAR bit 1024 / pipe_output_right_kernel instantiation
+  // Full join (dfgpu_pipeline_set_stage_full): the RIGHT stage that marks its records (kStageFull on the device), or -1.  in_tail: the push
+  // of the unmatched build rows at finish, whose FULL stage reads the emitted keys from the hidden column behind the inputs
+  int full_stage = -1; bool in_tail = false; int64_t m_unmatched_build_rows = 0;
+  std::vector<DCol> tail_part; int64_t tail_rows = 0;   // output sinks: the tail push's columns, emitted after the probe rows' batches
   // stage filters (dfgpu_pipeline_set_stage_filter): per stage the program and the payload fields its virtual columns past the inputs name
   ExprPlan filt[kMaxStages]; bool has_filt[kMaxStages] = {false, false, false}; std::vector<ExtDef> filt_ext[kMaxStages]; int filt_nodes = 0;
   std::unique_ptr<FiltParams> filt_host;   // staging copy of the bound programs (upload_filters)
@@ -2229,6 +2252,7 @@ static bool conjunction_terms(const dfgpu_pipeline* p, int max_terms, std::vecto
 // behind the input columns (pack_batch_keys' order), else the key column itself
 static int key_slot(const dfgpu_pipeline* p, int s) {
   int k = (int)p->in_types.size();
+  if (p->in_tail && s == p->full_stage) return k;   // the Full join's tail: the emitted keys, the only hidden column (its stage is the only one)
   for (int t = 0; t < (int)p->stages.size() && t < s; ++t) k += p->stage_keys[t].empty() ? 0 : 1;
   if (s == kMaxStages) return p->bkey_cols.empty() ? p->bkey_col : k;
   return p->stage_keys[s].empty() ? p->stages[s].key_col : k;
@@ -2243,7 +2267,7 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
   for (size_t k = 0; k < p->packed.size(); ++k) pp->col[cols.size() + k] = col_ref(p->packed[k]);   // hidden: n_cols stays the inputs'
   int pool_used = 0;
   pp->pred_mode = 0;
-  if (p->has_pred) {
+  if (p->has_pred && !p->in_tail) {   // the Full join's tail rows are build rows: the predicate over the probe side does not apply
     // fast path: conjunction of `column <cmp> literal` terms over integer-class columns
     std::vector<std::array<long long, 4>> terms;  // col, op, uns, lit
     if (conjunction_terms(p, kMaxTerms, &terms)) {
@@ -2263,6 +2287,7 @@ static void fill_params(dfgpu_pipeline* p, const std::vector<DCol>& cols, PipePa
     // a LEFT / LEFT_ANTI stage probes as an INNER one: the build rows no probe row reached are found in the records at finish
     const int kind = p->stages[s].kind;
     pp->stage[s].kind = kind == DFGPU_STAGE_LEFT || kind == DFGPU_STAGE_LEFT_ANTI ? DFGPU_STAGE_INNER : kind; pp->stage[s].key_col = key_slot(p, (int)s); pp->stage[s].lk = lookup_dev(p->stages[s].lookup);
+    if ((int)s == p->full_stage) pp->stage[s].kind = kStageFull;
   }
   pp->n_ext = (int)p->exts.size();
   for (size_t e = 0; e < p->exts.size(); ++e) pp->ext[e] = p->exts[e];
@@ -2316,6 +2341,14 @@ static bool pipeline_has_decimal(const dfgpu_pipeline* p);
 // the sink's default VAR bits (launch_pipe below) plus the stage filters
 constexpr int filt_var(int sink) { return kVarFilt | (sink == SINK_AGG ? kPipeVarDefault : (sink == SINK_PACK || sink == SINK_OUTPUT_ANY ? 2 : 0)); }
 
+// the timing family of a push's pipeline kernel: "pipe:<name>" (`unnamed` without a name); the Full join's tail push at finish is timed
+// as its own family, "pipe_full_tail[:<name>]", so it is not counted in the probe pushes' family
+static std::string tail_timer(const dfgpu_pipeline* p) { return p->name.empty() ? std::string("pipe_full_tail") : "pipe_full_tail:" + p->name; }
+static std::string pipe_timer(const dfgpu_pipeline* p, const char* unnamed) {
+  if (p->in_tail) return tail_timer(p);
+  return p->name.empty() ? std::string(unnamed) : "pipe:" + p->name;
+}
+
 template <int SINK>
 static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, const char* timer_name, bool part = false, bool out_cols = false) {
   dfgpu_ctx* ctx = p->ctx;
@@ -2333,7 +2366,7 @@ static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, cons
     int blocks_per_sm = blocks_env_f;
     if (blocks_per_sm <= 0) DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, sizeof(FiltParams)));
     const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
-    const std::string tname = p->name.empty() ? std::string(timer_name) : "pipe:" + p->name;
+    const std::string tname = pipe_timer(p, timer_name);
     KernelTimer kt(ctx, tname.c_str());
     kern<<<grid, kPipeThreads, sizeof(FiltParams), ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, p->counters.as<unsigned long long>());
     DF_LAUNCH_CHECK(ctx);
@@ -2345,7 +2378,7 @@ static void launch_pipe(dfgpu_pipeline* p, const PipeParams& pp, int64_t n, cons
   for (const auto& ag : p->aggs) dec = dec || (ag.has_expr && ag.plan.has_decimal);
   const PipeParams* gp = (const PipeParams*)p->params_dev.ptr;
   unsigned long long* cnt = p->counters.as<unsigned long long>();
-  const std::string tname = p->name.empty() ? std::string(timer_name) : "pipe:" + p->name;
+  const std::string tname = pipe_timer(p, timer_name);
   if constexpr (SINK == SINK_AGG || SINK == SINK_PACK) if (!dec && pp.ring_stages > 0 && !getenv("DFGPU_PIPE_VAR")) {
     constexpr int RV = SINK == SINK_AGG ? 64 | 8 : 64;   // ring + lane-paired REDs for the aggregate sink, ring alone for the pack sink
     // the partitioned aggregate: ring + records instead of lookups
@@ -2551,7 +2584,7 @@ static void launch_dense(dfgpu_pipeline* p, const PipeParams& pp, const DensePar
   DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, smem));
   const int64_t ntiles = (n + kPipeTile - 1) / kPipeTile;
   const int grid = (int)std::min<int64_t>(ntiles, (int64_t)kNumSMs * std::max(1, blocks_per_sm));
-  const std::string tname = p->name.empty() ? std::string("pipeline_dense") : "pipe:" + p->name;
+  const std::string tname = pipe_timer(p, "pipeline_dense");
   KernelTimer kt(ctx, tname.c_str());
   kern<<<grid, kPipeThreads, smem, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, p->counters.as<unsigned long long>());
   DF_LAUNCH_CHECK(ctx);
@@ -2626,7 +2659,7 @@ static void hash_push(dfgpu_pipeline* p, const std::vector<DCol>& cols, int64_t 
   }
   int blocks_per_sm = 0;
   DF_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kern, kPipeThreads, smem));
-  const std::string tname = p->name.empty() ? std::string("pipeline_hash") : "pipe:" + p->name;
+  const std::string tname = pipe_timer(p, "pipeline_hash");
   constexpr int64_t kMaxChunk = 1ll << 26;
   int64_t chunk = std::max<int64_t>((int64_t)p->hash_cap / 2, 1 << 20);
   DevBuf overflow;
@@ -2688,6 +2721,9 @@ static void check_left_build(const dfgpu_pipeline* p) {
   if (p->left_kind)
     DF_CHECK(p->stages[p->agg_stage].lookup->null_keys == 0, DFGPU_ERR_UNSUPPORTED,
              "pipeline: a LEFT / LEFT_ANTI stage needs a build side without NULL keys (they are not in the lookup) — use dfgpu_hashjoin");
+  if (p->full_stage >= 0)   // the same for a Full join's build rows
+    DF_CHECK(p->stages[p->full_stage].lookup->null_keys == 0, DFGPU_ERR_UNSUPPORTED,
+             "pipeline: a FULL stage needs a build side without NULL keys (they are not in the lookup) — use dfgpu_hashjoin");
 }
 
 // rows of a build push whose key is NULL, from the key column's validity (before the predicate: an upper bound of the rows dropped for it)
@@ -2754,10 +2790,10 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     DF_CHECK(cols[c].type != DFGPU_BOOL && (type_width(cols[c].type) <= 8 || type_is_decimal(cols[c].type)), DFGPU_ERR_UNSUPPORTED,
              "pipeline: fixed-width columns of <= 8 bytes (and Decimal128 inside expressions) only");
   }
-  p->m_input_rows += n;
+  if (!p->in_tail) p->m_input_rows += n;   // the Full join's unmatched build rows are not input rows
   if (n == 0) return;
   if (!p->counters.ptr) p->counters.alloc(ctx, 64);
-  pack_batch_keys(p, cols, n);
+  if (!p->in_tail) pack_batch_keys(p, cols, n);   // the tail brings its keys in p->packed
   PipeParams pp;
   unsigned long long h[4];
   if (p->sink == SINK_BUILD) {
@@ -2950,7 +2986,8 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
     unsigned long long* totals = (unsigned long long*)((char*)desc.ptr + (size_t)nt * 8);
     unsigned int* counter = (unsigned int*)(totals + 2);
     {
-      KernelTimer kt(ctx, "pipeline_output");
+      const std::string tname = p->in_tail ? tail_timer(p) : std::string("pipeline_output");
+      KernelTimer kt(ctx, tname.c_str());
       if (p->has_right) {   // RIGHT stages: the survivors' payload validity bits in the dynamic shared memory
         pipe_output_right_kernel<<<(int)nt, kPipeThreads, kPipeTile, ctx->stream>>>((const PipeParams*)p->params_dev.ptr, n, oc, desc.as<unsigned long long>(), counter, totals,
                                                                                    p->counters.as<unsigned long long>());
@@ -3035,21 +3072,80 @@ static void add_agg_columns(const std::vector<PipeAgg>& aggs, int rows_word, boo
 
 static void dense_finish(dfgpu_pipeline* p);
 
+// Full join, second part: the build rows no probe row matched go once more through the pipeline, as one push at finish (timed as
+// "pipe_full_tail:<name>").  Their records are the occupied ones whose visited word is still 0 (lookup_groups_kernel's LEFT_ANTI
+// selection); their keys, emitted in slot order, are the FULL stage's hidden key column.  Every input column is NULL (zeroed values, an
+// all-zero bitmap) and the predicate is off, so each row finds its record and carries its payload fields, and the sink takes it like any
+// other row: the output sinks write it with bitmaps, the dense and hash sinks put its NULL probe columns in their NULL groups, and the
+// aggregate arguments are evaluated on it.
+static void full_tail(dfgpu_pipeline* p) {
+  check_left_build(p);
+  dfgpu_lookup* l = p->stages[p->full_stage].lookup;
+  if (l->cap == 0 || l->rows == 0) return;
+  dfgpu_ctx* ctx = p->ctx;
+  DCol keys;
+  int64_t m = 0;
+  {   // the selection and the key emission; the push below times its kernels under the same family, one timer after the other
+    const std::string tname = tail_timer(p);
+    KernelTimer kt(ctx, tname.c_str());
+    const LookupDev t = lookup_dev(l);
+    const uint64_t nw = (t.cap + 31) / 32;
+    DevBuf words(ctx, (size_t)nw * 4 + 8), idx;
+    lookup_groups_kernel<<<grid_for((int64_t)nw * 32, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, kVisitedWord, 1, words.as<uint32_t>());
+    DF_LAUNCH_CHECK(ctx);
+    m = compact_flag_indices(ctx, words.as<uint32_t>(), (int64_t)t.cap, 1, &idx);
+    p->m_unmatched_build_rows = m;
+    if (m == 0) return;
+    keys = alloc_col(ctx, DFGPU_INT64, m, false);   // the record's key word as stored: a composite key's packed tuple
+    EmitCols ec;
+    memset(&ec, 0, sizeof(ec));
+    ec.n = 1; ec.c[0].kind = 0; ec.c[0].width = 8; ec.c[0].nn_word = -1; ec.c[0].dst = keys.own_values->ptr;
+    lookup_emit_kernel<<<grid_for(m, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(t, idx.as<uint32_t>(), m, kVisitedWord, ec);
+    DF_LAUNCH_CHECK(ctx);
+  }
+  std::vector<DCol> cols;
+  for (int type : p->in_types) {
+    DCol c = alloc_col(ctx, type, m, true);
+    c.own_values->zero(); c.own_validity->zero();
+    c.null_count = m;
+    cols.push_back(std::move(c));
+  }
+  p->packed.clear();
+  p->packed.push_back(std::move(keys));
+  const size_t parts = p->out_parts.size();
+  const int64_t pending = p->out_rows_pending;
+  p->in_tail = true;
+  try { pipeline_push(p, cols); } catch (...) { p->in_tail = false; throw; }
+  p->in_tail = false;
+  if (p->sink == SINK_OUTPUT && p->out_parts.size() > parts) {   // the output sinks emit the tail's rows as batches of their own
+    p->tail_part = std::move(p->out_parts.back());
+    p->out_parts.pop_back();
+    p->tail_rows = p->out_rows_pending - pending;
+    p->out_rows_pending = pending;
+  }
+}
+
 static void pipeline_finish(dfgpu_pipeline* p) {
   DF_CHECK(!p->finished, DFGPU_ERR_STATE, "finish called twice");
+  if (p->full_stage >= 0) {   // a tail that fails leaves the pipeline finished: a second finish must not push the rows again
+    set_device(p->ctx);
+    try { full_tail(p); } catch (...) { p->finished = true; throw; }
+  }
   p->finished = true;
   dfgpu_ctx* ctx = p->ctx;
   set_device(ctx);
   if (p->sink == SINK_OUTPUT) {
-    if (p->out_rows_pending == 0) return;
-    std::vector<DCol> merged;
-    for (size_t c = 0; c < p->out_cols.size(); ++c) {
-      std::vector<DCol> parts;
-      for (auto& b : p->out_parts) parts.push_back(b[c]);
-      merged.push_back(parts.size() == 1 ? parts[0] : concat_columns(ctx, parts, p->vtypes[p->out_cols[c]]));
+    if (p->out_rows_pending > 0) {
+      std::vector<DCol> merged;
+      for (size_t c = 0; c < p->out_cols.size(); ++c) {
+        std::vector<DCol> parts;
+        for (auto& b : p->out_parts) parts.push_back(b[c]);
+        merged.push_back(parts.size() == 1 ? parts[0] : concat_columns(ctx, parts, p->vtypes[p->out_cols[c]]));
+      }
+      p->out_parts.clear();
+      emit_sliced(p, merged, p->out_rows_pending);
     }
-    p->out_parts.clear();
-    emit_sliced(p, merged, p->out_rows_pending);
+    if (p->tail_rows > 0) emit_sliced(p, p->tail_part, p->tail_rows);   // behind the probe rows, not copied into their columns
     return;
   }
   if (p->sink == SINK_DENSE) { dense_finish(p); return; }
@@ -3437,7 +3533,7 @@ int dfgpu_lookup_clear(dfgpu_lookup* l) {
     if (l->cap) { lookup_init_kernel<<<grid_for((int64_t)l->cap * l->stride, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(l->recs.as<unsigned long long>(), l->cap, l->stride); DF_LAUNCH_CHECK(ctx); }
     if (l->bloom.ptr) l->bloom.zero();
   }
-  l->rows = 0; l->null_keys = 0;
+  l->rows = 0; l->null_keys = 0; l->marks_taken = false;   // the records' visited words are 0 again
   DF_API_END
 }
 int dfgpu_lookup_filter_buffer(dfgpu_lookup* l, void** words_dev, uint64_t* n_bytes) {
@@ -3625,6 +3721,26 @@ int dfgpu_pipeline_set_stage_keys(dfgpu_pipeline* p, int32_t stage, const int32_
   DF_API_END
 }
 
+int dfgpu_pipeline_set_stage_full(dfgpu_pipeline* p, int32_t stage) {
+  DF_API_BEGIN(p ? p->ctx : nullptr)
+  DF_CHECK(p, DFGPU_ERR_INVALID, "null argument");
+  DF_CHECK(stage >= 0 && stage < (int)p->stages.size(), DFGPU_ERR_INVALID, "pipeline full stage: stage out of range");
+  DF_CHECK(p->stages[stage].kind == DFGPU_STAGE_RIGHT, DFGPU_ERR_INVALID, "pipeline full stage: only a RIGHT stage becomes a Full join");
+  DF_CHECK(p->sink == SINK_NONE && !p->pushed && p->m_input_rows == 0, DFGPU_ERR_STATE, "pipeline full stage: set before the sink and the first push");
+  DF_CHECK(p->full_stage < 0, DFGPU_ERR_STATE, "pipeline full stage: the stage already is one");
+  // the unmatched build rows are pushed with every input column NULL: past other probe stages they would have to skip those stages
+  DF_CHECK(p->stages.size() == 1, DFGPU_ERR_UNSUPPORTED, "pipeline full stage: a FULL stage must be the pipeline's only probe stage — use dfgpu_hashjoin");
+  dfgpu_lookup* l = p->stages[stage].lookup;
+  DF_CHECK(l->has_payload && l->opt.n_acc_words >= 1, DFGPU_ERR_UNSUPPORTED,
+           "pipeline full stage: the lookup needs payload and an accumulator word for the visited marks (n_acc_words >= 1)");
+  DF_CHECK((int)p->in_types.size() + 1 <= kMaxPipeCols, DFGPU_ERR_UNSUPPORTED, "pipeline full stage: the input columns and the emitted build keys exceed 16 columns");
+  DF_CHECK(!l->marks_taken && !l->acc_claimed, DFGPU_ERR_STATE,
+           "pipeline full stage: the lookup's marks are taken by another pipeline (dfgpu_lookup_clear frees them)");
+  l->marks_taken = true;
+  p->full_stage = stage;
+  DF_API_END
+}
+
 int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, int32_t n_group, const dfgpu_pipeline_agg* aggs, int32_t n_aggs, int32_t mode, int64_t batch_size) {
   DF_API_BEGIN(p ? p->ctx : nullptr)
   DF_CHECK(p && group_cols && n_group >= 1, DFGPU_ERR_INVALID, "null argument");
@@ -3666,7 +3782,7 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   }
   DF_CHECK(stage >= 0, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: group keys are not determined by one join key — use the unfused dfgpu_agg");
   dfgpu_lookup* l = p->stages[stage].lookup;
-  DF_CHECK(!l->acc_claimed, DFGPU_ERR_STATE, "pipeline aggregate: the lookup's accumulators are already in use");
+  DF_CHECK(!l->acc_claimed && !l->marks_taken, DFGPU_ERR_STATE, "pipeline aggregate: the lookup's accumulators are already in use");
   const int base = 1 + (l->has_payload ? 1 : 0);
   int next = base;
   DF_CHECK(next < base + l->opt.n_acc_words, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: the lookup reserves no accumulator words (n_acc_words)");
@@ -3926,6 +4042,7 @@ int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name) {
   if (s == "partitioned_records") return p->m_partitioned_records;     // {key, value} records the partitioned aggregate's pass 1 wrote
   if (s == "group_rehashes") return p->m_group_rehashes;               // hash aggregate sink: times its group table grew
   if (s == "replayed_rows") return p->m_replayed_rows;                 // hash aggregate sink: rows deferred by the claim budget and pushed again
+  if (s == "unmatched_build_rows") return p->m_unmatched_build_rows;   // FULL stage: build rows no probe row matched, pushed at finish
   return -1;
 }
 void dfgpu_pipeline_destroy(dfgpu_pipeline* p) {

@@ -677,9 +677,11 @@ class _Scan:
         self.stages: List[Tuple[int, object, "GpuPipelineExec"]] = []  # (stage kind, probe key column — a list of them for a composite key, build pipeline)
         self.visible: List[str] = [f.name for f in source.schema]       # column names the operators above may still reference
         self.filters: dict = {}                                          # stage index -> its JoinFilter as stage-filter RPN nodes
+        self.full = False                                                # the only stage is a Full join's (fuse_full_joins)
 
     def virtual_schema(self) -> pa.Schema:
-        fields = list(self.source.schema)
+        # a Full join's unmatched build rows carry every probe column NULL (build_join_schema(..., "Full"))
+        fields = [f.with_nullable(True) for f in self.source.schema] if self.full else list(self.source.schema)
         for kind, _, build in self.stages:
             if kind in (D.STAGE_INNER, D.STAGE_LEFT, D.STAGE_LEFT_ANTI):
                 fields += [build.scan_field(n) for n in build.payload]
@@ -818,15 +820,17 @@ def _settle_right(sc: _Scan, read: set) -> bool:
     return True
 
 
-def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False) -> Optional[_Scan]:
+def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False, full_joins: bool = False) -> Optional[_Scan]:
     """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner / Right, one key or a composite
     key (_join_keys), fusable build)]* over a source.  join_filters: a join may carry a JoinFilter, which becomes its stage's filter
     (fuse_join_filters); a Right join never does.  right_joins: Right joins are accepted (fuse_right_joins); such a stage carries every
-    build column until _settle_right keeps those read above it."""
+    build column until _settle_right keeps those read above it.  full_joins (with right_joins): a Full join is accepted too, as a RIGHT
+    stage that also emits the unmatched build rows (fuse_full_joins), when it is the chain's only join: its probe side is [FilterExec]
+    over the source, and no join probes above it.  Its lookup takes one accumulator word, the visited marks."""
     if isinstance(plan, GpuProjectionExec):
         if not all(isinstance(e, Column) and e.name == name for e, name in plan.exprs):
             return None
-        sc = _as_scan(plan.input, join_filters, right_joins)
+        sc = _as_scan(plan.input, join_filters, right_joins, full_joins)
         if sc is not None:
             sc.visible = [name for _, name in plan.exprs]
         return sc
@@ -841,16 +845,19 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool 
             sc.visible = [inner.schema.field(i).name for i in plan.projection]
         return sc
     if isinstance(plan, GpuHashJoinExec):
-        kinds = ("RightSemi", "RightAnti", "Inner") + (("Right",) if right_joins and plan.filter is None else ())
+        kinds = ("RightSemi", "RightAnti", "Inner") + (("Right",) if right_joins and plan.filter is None else ()) + \
+            (("Full",) if right_joins and full_joins and plan.filter is None else ())
         if plan.join_type not in kinds or (plan.filter is not None and not join_filters) or plan.null_aware or plan.null_equality != "NullEqualsNothing":
             return None
-        sc = _as_scan(plan.right, join_filters, right_joins)
+        sc = _as_scan(plan.right, join_filters, right_joins, full_joins)
+        if sc is not None and (sc.full or (plan.join_type == "Full" and sc.stages)):
+            return None                                   # a FULL stage is the pipeline's only probe stage
         keys = None if sc is None else _join_keys(plan, sc)
         if keys is None or (isinstance(keys[1], str) and keys[1] not in [f.name for f in sc.source.schema]):
             return None
         bkey, pkey = keys
         bkeys = bkey if isinstance(bkey, list) else [bkey]
-        kind = {"RightSemi": D.STAGE_SEMI, "RightAnti": D.STAGE_ANTI, "Inner": D.STAGE_INNER, "Right": D.STAGE_RIGHT}[plan.join_type]
+        kind = {"RightSemi": D.STAGE_SEMI, "RightAnti": D.STAGE_ANTI, "Inner": D.STAGE_INNER, "Right": D.STAGE_RIGHT, "Full": D.STAGE_RIGHT}[plan.join_type]
         payload = [f.name for f in plan.left.schema if f.name not in bkeys] if kind == D.STAGE_INNER else []
         if kind == D.STAGE_RIGHT:
             payload = [f.name for f in plan.left.schema]
@@ -867,6 +874,9 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool 
             return None
         if filt is not None:
             sc.filters[len(sc.stages)] = filt
+        if plan.join_type == "Full":
+            sc.full = True
+            build.n_acc_words = 1                         # the visited marks (dfgpu_pipeline_set_stage_full)
         sc.stages.append((kind, pkey, build))
         names = [f.name for f in plan.schema]
         sc.visible = names
@@ -990,6 +1000,8 @@ class GpuPipelineExec(ExecutionPlan):
             raise
         pipe = D.Pipeline(ctx.gpu, [type_id(f.type) for f in ssch], nodes, stages)
         try:
+            if self.scan.full:
+                pipe.set_stage_full(0)
             for s, fnodes in sorted(self.scan.filters.items()):
                 pipe.set_stage_filter(s, fnodes)
         except BaseException:
@@ -1111,16 +1123,16 @@ def _source_bounds(source: ExecutionPlan, name: str) -> Optional[Tuple[int, int]
     return lo, hi
 
 
-def _fuse_dense(plan: "GpuAggregateExec", right_joins: bool = False) -> Optional["GpuPipelineExec"]:
+def _fuse_dense(plan: "GpuAggregateExec", right_joins: bool = False, full_joins: bool = False) -> Optional["GpuPipelineExec"]:
     """AggregateExec over [ProjectionExec] over FilterExec over a source (no join) whose GROUP BY columns are source columns with known
     bounds spanning at most DENSE_MAX_GROUPS slots (NULL included) -> a GpuPipelineExec with the dense sink; None otherwise"""
     below, proj = plan.input, None
     if isinstance(below, GpuProjectionExec):
         proj, below = below, below.input
-    right = right_joins and isinstance(below, GpuHashJoinExec) and below.join_type == "Right"
+    right = right_joins and isinstance(below, GpuHashJoinExec) and below.join_type in ("Right",) + (("Full",) if full_joins else ())
     if not (isinstance(below, GpuFilterExec) or right):
         return None
-    sc = _as_scan(below, right_joins=right)
+    sc = _as_scan(below, right_joins=right, full_joins=full_joins)
     if sc is None or (sc.stages and not right):
         return None
     exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
@@ -1206,7 +1218,7 @@ def _acc_words(funcs: Sequence[str], types: Sequence[Optional[pa.DataType]], has
     return n
 
 
-def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False) -> ExecutionPlan:
+def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a): AggregateExec(Single / SinglePartitioned / Partial) over [ProjectionExec] over
     HashJoinExec(Inner) whose GROUP BY is the probe key plus build-side columns becomes ONE GpuPipelineExec; its build side (filters, semi
     joins, column projections) becomes build pipelines.  The same AggregateExec over [ProjectionExec] over FilterExec over a source, with
@@ -1215,13 +1227,13 @@ def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False, right_joins:
     (_fuse_left: TPC-H Q13), and a top-level HashJoinExec(LeftSemi / LeftAnti) (_fuse_left_filter: Q18, Q20, Q22) become a GpuPipelineExec
     with the join-keyed sink.  Their rows come out in slot order: the reference does not keep the build side's order either
     (maintains_input_order is false for it).  Anything else is returned unchanged (the unfused Gpu*Exec operators run).
-    join_filters: joins with a JoinFilter fuse too (fuse_join_filters)."""
+    join_filters: joins with a JoinFilter fuse too (fuse_join_filters).  right_joins / full_joins: see _as_scan."""
     if isinstance(plan, GpuHashJoinExec) and plan.join_type in ("LeftSemi", "LeftAnti"):
         fused = _fuse_left_filter(plan, join_filters)
         return plan if fused is None else fused
     if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial"):
         return plan
-    dense = _fuse_dense(plan, right_joins)
+    dense = _fuse_dense(plan, right_joins, full_joins)
     if dense is not None:
         return dense
     if not plan.group_by:
@@ -1385,7 +1397,7 @@ def _fuse_left_filter(join: GpuHashJoinExec, join_filters: bool = False) -> Opti
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, mode="Single", out_schema=join.schema, project=project)
 
 
-def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False) -> ExecutionPlan:
+def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_pipelines: its result when that rule fuses; otherwise an
     AggregateExec(Single / SinglePartitioned / Partial) with at least one GROUP BY column over [ProjectionExec] over an Inner join chain or a
     FilterExec (as _as_scan accepts them) becomes ONE GpuPipelineExec with the hash-keyed sink (dfgpu_pipeline_sink_aggregate_hash: TPC-H
@@ -1393,7 +1405,7 @@ def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False, right_
     (each column at its width, one more bit per nullable column) at most 128 bits; no FILTER clause, at most 4 aggregates, and the argument
     types the library accepts.  Anything else, a bare scan included, is returned unchanged (dfgpu_agg runs).  join_filters: joins with a
     JoinFilter fuse too (fuse_join_filters)."""
-    fused = fuse_pipelines(plan, join_filters, right_joins)
+    fused = fuse_pipelines(plan, join_filters, right_joins, full_joins)
     if fused is not plan:
         return fused
     if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial") or not plan.group_by:
@@ -1401,9 +1413,10 @@ def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False, right_
     below, proj = plan.input, None
     if isinstance(below, GpuProjectionExec):
         proj, below = below, below.input
-    if not ((isinstance(below, GpuHashJoinExec) and below.join_type in (("Inner", "Right") if right_joins else ("Inner",))) or isinstance(below, GpuFilterExec)):
+    kinds = ("Inner",) + (("Right",) if right_joins else ()) + (("Full",) if right_joins and full_joins else ())
+    if not ((isinstance(below, GpuHashJoinExec) and below.join_type in kinds) or isinstance(below, GpuFilterExec)):
         return plan
-    sc = _as_scan(below, join_filters, right_joins)
+    sc = _as_scan(below, join_filters, right_joins, full_joins)
     # a composite-key stage under the hash-keyed sink (TPC-H Q9's lineitem x partsupp profit by supplier) measured slower than the
     # unfused dfgpu_hashjoin -> dfgpu_agg (README): that shape stays unfused
     if sc is None or any(isinstance(k, list) for _, k, _ in sc.stages):
@@ -1449,20 +1462,20 @@ def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False, right_
                            fallback=plan if sc.has_right() else None)
 
 
-def fuse_join_filters(plan: ExecutionPlan, right_joins: bool = False) -> ExecutionPlan:
+def fuse_join_filters(plan: ExecutionPlan, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_hash_aggregates: its result when that rule fuses; otherwise the same
     shapes again with JoinFilters allowed on the Inner / RightSemi / RightAnti joins of a probe chain and on a Left / LeftSemi / LeftAnti
     join that is the last stage.  Each filter becomes its stage's filter (dfgpu_pipeline_set_stage_filter): a probe-side column maps to
     the probe chain's column, the build key to the probe key, other build columns to the stage's payload fields (a RightSemi /
     RightAnti build carries exactly the columns its filter reads).  A plan is left unchanged when a payload would exceed 64 bits, the
     filters 128 nodes, or an AND / OR has a right operand that can raise (÷, %, CAST, Decimal128 arithmetic)."""
-    fused = fuse_hash_aggregates(plan, right_joins=right_joins)
+    fused = fuse_hash_aggregates(plan, right_joins=right_joins, full_joins=full_joins)
     if fused is not plan:
         return fused
-    return fuse_hash_aggregates(plan, join_filters=True, right_joins=right_joins)
+    return fuse_hash_aggregates(plan, join_filters=True, right_joins=right_joins, full_joins=full_joins)
 
 
-def fuse_output_pipelines(plan: ExecutionPlan, right_joins: bool = False) -> ExecutionPlan:
+def fuse_output_pipelines(plan: ExecutionPlan, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_join_filters: its result when that rule fuses; otherwise a top-level
     [ProjectionExec(columns only)] over a HashJoinExec(Inner / RightSemi / RightAnti) chain, as _as_scan accepts it with JoinFilters and
     with at least one stage, becomes ONE GpuPipelineExec over the ordered output sink (dfgpu_pipeline_sink_output) that emits the plan's
@@ -1473,13 +1486,14 @@ def fuse_output_pipelines(plan: ExecutionPlan, right_joins: bool = False) -> Exe
     NULL payloads) runs the unfused joins instead, before any row is emitted.  The fused Inner join emits its rows in probe order, the
     reference's order for unique build keys.  Anything else (a bare FilterExec, Left / Right / Full joins, several keys,
     null-aware joins, computed projections) is returned unchanged."""
-    fused = fuse_join_filters(plan, right_joins)
+    fused = fuse_join_filters(plan, right_joins, full_joins)
     if fused is not plan:
         return fused
     join = plan.input if isinstance(plan, GpuProjectionExec) else plan
-    if not isinstance(join, GpuHashJoinExec) or join.join_type not in ("Inner", "RightSemi", "RightAnti") + (("Right",) if right_joins else ()):
+    kinds = ("Inner", "RightSemi", "RightAnti") + (("Right",) if right_joins else ()) + (("Full",) if right_joins and full_joins else ())
+    if not isinstance(join, GpuHashJoinExec) or join.join_type not in kinds:
         return plan
-    sc = _as_scan(join, join_filters=True, right_joins=right_joins)
+    sc = _as_scan(join, join_filters=True, right_joins=right_joins, full_joins=full_joins)
     if sc is None or not sc.stages:
         return plan
     pick = list(range(len(join.column_indices)))                                # the join's columns that form the output
@@ -1542,6 +1556,22 @@ def fuse_right_joins(plan: ExecutionPlan) -> ExecutionPlan:
     if fused is not plan:
         return fused
     return fuse_output_pipelines(plan, right_joins=True)
+
+
+def fuse_full_joins(plan: ExecutionPlan) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_right_joins: its result when that rule fuses; otherwise the same
+    shapes again with a HashJoinExec(Full) allowed as the probe chain's only join (a RIGHT stage turned into a Full join,
+    dfgpu_pipeline_set_stage_full): its probe side is [FilterExec] over a source.  The conditions and sinks are fuse_right_joins': one key or
+    a composite key, NullEqualsNothing, not null-aware, no JoinFilter; the stage carries the build columns read above the join (the build
+    key included, NULL on unmatched probe rows), 1 to 64 bits, as nullable fields; the ordered output, dense and hash sinks.  Its lookup
+    takes one accumulator word for the visited marks.  The build rows no probe row matched follow the probe rows with every probe column
+    NULL, so the source columns are nullable in the virtual schema, and a probe-side group column of the hash sink is declared nullable.
+    The fused node's schema is the plan's (build_join_schema(..., "Full"), projected).  A build the library refuses (duplicate or NULL
+    keys) runs the plan instead, its fallback, before any row is emitted."""
+    fused = fuse_right_joins(plan)
+    if fused is not plan:
+        return fused
+    return fuse_output_pipelines(plan, right_joins=True, full_joins=True)
 
 
 # ---------------------------------------------------------------------------------------------

@@ -486,7 +486,8 @@ enum dfgpu_stage_kind {
                            * filter-only lookup is DFGPU_ERR_UNSUPPORTED at dfgpu_pipeline_create.  Sinks: output (ordered: probe order,
                            * unmatched rows where they occur, as dfgpu_hashjoin's Right join), dense and hash aggregates; the build, pack
                            * and join-keyed aggregate sinks are DFGPU_ERR_UNSUPPORTED, and so is dfgpu_pipeline_set_stage_filter on any
-                           * stage of a pipeline with a RIGHT stage.  An aggregate argument reading a RIGHT payload field skips its NULLs. */
+                           * stage of a pipeline with a RIGHT stage.  An aggregate argument reading a RIGHT payload field skips its NULLs.
+                           * dfgpu_pipeline_set_stage_full turns a RIGHT stage into a Full join (see there). */
 };
 typedef struct dfgpu_pipeline_stage {
   int32_t kind;          /* dfgpu_stage_kind: the pipeline input is the PROBE (right) side — Inner / RightSemi / RightAnti / Right, and Left /
@@ -621,6 +622,23 @@ int dfgpu_pipeline_set_stage_filter(dfgpu_pipeline* p, int32_t stage, const dfgp
  * decoded from the record's packed key, (key / stride_g) % r_g + key_min[g], at the component's type; for LEFT / LEFT_ANTI they are the
  * build key's components, never NULL.  The dense, hash and output sinks take the components as ordinary input columns. */
 int dfgpu_pipeline_set_stage_keys(dfgpu_pipeline* p, int32_t stage, const int32_t* key_cols, int32_t n_keys);
+/* Full join (HashJoinExec(Full), NullEqualsNothing, no JoinFilter): RIGHT stage `stage` also emits the build rows no probe row matched.
+ * The output is (1) every probe row reaching the stage exactly as a RIGHT stage produces it, then (2) at dfgpu_pipeline_finish, one row per
+ * build record that no surviving probe row matched: every input column NULL, the stage's payload fields the record's values.  The
+ * ordered output sink keeps probe order for (1) and appends (2) in the lookup's slot order (DataFusion emits them in build order); both
+ * output sinks emit (2) as batches of their own, after those of (1), each sliced by batch_size (batch_size 0: one batch each).  The
+ * rows of (2) go through the same sink as any row: the output sinks write them with bitmaps, the dense sink puts their NULL input group
+ * columns in the NULL slot, the hash sink sets their NULL bits (declare such group columns nullable), and every aggregate argument is
+ * evaluated on them.  They are not counted in "input_rows"; "unmatched_build_rows" counts them.  With kernel timing on, the family
+ * "pipe_full_tail:<name>" ("pipe_full_tail" without a name) times their selection and their push; "pipe:<name>" does not count them.
+ * A finish whose push of (2) fails leaves the pipeline finished (a second dfgpu_pipeline_finish is DFGPU_ERR_STATE).
+ * Each matched record is marked visited in the lookup's first accumulator word.  Call after dfgpu_pipeline_create, before the sink and
+ * the first push (DFGPU_ERR_STATE otherwise).  DFGPU_ERR_INVALID: the stage is not RIGHT.  DFGPU_ERR_UNSUPPORTED: the stage is not the
+ * pipeline's only stage; its lookup was not created with payload and n_acc_words >= 1; the inputs take all 16 column slots (the build
+ * keys of (2) need one); the build side had a NULL key (at push or finish: such a row is not in the lookup).  DFGPU_ERR_STATE: the
+ * lookup's marks (or accumulators) are already taken by another pipeline — one FULL pipeline per lookup until dfgpu_lookup_clear.  The
+ * build, pack and join-keyed aggregate sinks and stage filters stay DFGPU_ERR_UNSUPPORTED, as for any RIGHT stage. */
+int dfgpu_pipeline_set_stage_full(dfgpu_pipeline* p, int32_t stage);
 /* optional label: this pipeline's kernel is timed under the family "pipe:<name>" (dfgpu_set_kernel_timing / dfgpu_kernel_time) —
  * the per-operator metrics set of a plan node (metrics(), execution_plan.rs:713) */
 int dfgpu_pipeline_set_name(dfgpu_pipeline* p, const char* name);
@@ -630,7 +648,7 @@ int dfgpu_pipeline_push_arrow(dfgpu_pipeline* p, const struct ArrowArray* batch,
 int dfgpu_pipeline_finish(dfgpu_pipeline* p);
 int dfgpu_pipeline_next(dfgpu_pipeline* p, int host, dfgpu_batch** out);
 int64_t dfgpu_pipeline_metric(dfgpu_pipeline* p, const char* name); /* "input_rows","sink_rows","output_rows","num_groups","ring_launches","dense_block_launches","partitioned_launches",
-                                                                      "group_rehashes","replayed_rows",
+                                                                      "group_rehashes","replayed_rows","unmatched_build_rows",
                                                                       "partitioned_inserts": build sink pushes whose records went into a
                                                                       table larger than 40 MB (more than L2 holds) radix-partitioned by
                                                                       slot range, one L2-sized range at a time,
