@@ -1726,7 +1726,7 @@ __global__ void __launch_bounds__(256) bloom_fold_kernel(const ulonglong2* __res
     out[i] = v.x | v.y;
   }
 }
-// accumulator identities for MIN / MAX (SUM / COUNT start at the zero the table was initialised with)
+// accumulator identities for MIN / MAX (SUM / COUNT start at 0: the table's initialisation, or claim_acc_words on a reused lookup)
 __global__ void __launch_bounds__(256) lookup_init_acc_kernel(LookupDev t, int word, unsigned long long value) {
   for (uint64_t s = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; s < t.cap; s += (uint64_t)gridDim.x * blockDim.x) t.recs[s * (uint64_t)t.stride + word] = value;
 }
@@ -1985,6 +1985,9 @@ struct dfgpu_lookup {
   int64_t null_keys = 0;   // build rows pushed with a NULL key (counted before the predicate): never inserted, so a LEFT / LEFT_ANTI stage cannot emit them
   bool acc_claimed = false, filter_only = false;
   bool marks_taken = false;   // a FULL stage's visited marks live in the first accumulator word: one FULL pipeline, until dfgpu_lookup_clear
+  // a join-keyed aggregate sink or a FULL stage pushed into the accumulator words since creation or dfgpu_lookup_clear: the next one to
+  // claim them zeroes them first (claim_acc_words)
+  bool acc_written = false;
   // composite key (dfgpu_lookup_create_composite): the key is the packed tuple of these components, in [0, domain)
   std::vector<int> comp_types; std::vector<int64_t> comp_min; std::vector<uint64_t> comp_range, comp_stride; uint64_t domain = 0;
 };
@@ -2491,6 +2494,22 @@ static void prepare_acc(dfgpu_pipeline* p) {
   p->acc_ready = true;
 }
 
+// A join-keyed aggregate sink or a FULL stage takes the accumulator words of `l`.  When an earlier one pushed into them (acc_written), its
+// row counters, SUM / COUNT words and visited marks are still there: they go back to 0 here, one pass over the table timed as
+// "lookup_acc_reset".  A lookup fresh from creation or dfgpu_lookup_clear launches nothing.  The pass is a strided memset: words
+// [1 + payload, stride) of each record are one row of a 2D region whose pitch is the record (no kernel of the library's own).
+static void claim_acc_words(dfgpu_lookup* l) {
+  if (!l->acc_written) return;
+  dfgpu_ctx* ctx = l->ctx;
+  set_device(ctx);
+  const int base = 1 + (l->has_payload ? 1 : 0);
+  if (l->cap && base < l->stride) {
+    KernelTimer kt(ctx, "lookup_acc_reset");
+    DF_CUDA(cudaMemset2DAsync((char*)l->recs.ptr + (size_t)base * 8, (size_t)l->stride * 8, 0, (size_t)(l->stride - base) * 8, (size_t)l->cap, ctx->stream));
+  }
+  l->acc_written = false;
+}
+
 // ---- dense-group aggregate sink ----
 static int dense_op(const PipeAgg& ag) {
   const bool wide = ag.cls == C_DEC, f = ag.cls == C_F64, u = ag.cls == C_U64;
@@ -2792,6 +2811,8 @@ static void pipeline_push(dfgpu_pipeline* p, const std::vector<DCol>& cols) {
   }
   if (!p->in_tail) p->m_input_rows += n;   // the Full join's unmatched build rows are not input rows
   if (n == 0) return;
+  if (p->sink == SINK_AGG) p->stages[p->agg_stage].lookup->acc_written = true;
+  if (p->full_stage >= 0) p->stages[p->full_stage].lookup->acc_written = true;
   if (!p->counters.ptr) p->counters.alloc(ctx, 64);
   if (!p->in_tail) pack_batch_keys(p, cols, n);   // the tail brings its keys in p->packed
   PipeParams pp;
@@ -3533,7 +3554,7 @@ int dfgpu_lookup_clear(dfgpu_lookup* l) {
     if (l->cap) { lookup_init_kernel<<<grid_for((int64_t)l->cap * l->stride, 256, kNumSMs * 8), 256, 0, ctx->stream>>>(l->recs.as<unsigned long long>(), l->cap, l->stride); DF_LAUNCH_CHECK(ctx); }
     if (l->bloom.ptr) l->bloom.zero();
   }
-  l->rows = 0; l->null_keys = 0; l->marks_taken = false;   // the records' visited words are 0 again
+  l->rows = 0; l->null_keys = 0; l->marks_taken = false; l->acc_written = false;   // every accumulator word (visited marks included) is 0 again
   DF_API_END
 }
 int dfgpu_lookup_filter_buffer(dfgpu_lookup* l, void** words_dev, uint64_t* n_bytes) {
@@ -3736,6 +3757,7 @@ int dfgpu_pipeline_set_stage_full(dfgpu_pipeline* p, int32_t stage) {
   DF_CHECK((int)p->in_types.size() + 1 <= kMaxPipeCols, DFGPU_ERR_UNSUPPORTED, "pipeline full stage: the input columns and the emitted build keys exceed 16 columns");
   DF_CHECK(!l->marks_taken && !l->acc_claimed, DFGPU_ERR_STATE,
            "pipeline full stage: the lookup's marks are taken by another pipeline (dfgpu_lookup_clear frees them)");
+  claim_acc_words(l);
   l->marks_taken = true;
   p->full_stage = stage;
   DF_API_END
@@ -3792,6 +3814,7 @@ int dfgpu_pipeline_sink_aggregate(dfgpu_pipeline* p, const int32_t* group_cols, 
   DF_CHECK(left_kind != DFGPU_STAGE_LEFT_ANTI || n_aggs == 0, DFGPU_ERR_UNSUPPORTED, "pipeline aggregate: a LEFT_ANTI stage emits its build rows without aggregates");
   if (left_kind == DFGPU_STAGE_LEFT) check_left_args(p, new_aggs, left);
   layout_agg_words(new_aggs, next, base + l->opt.n_acc_words, l->stride % 2 == 0);
+  claim_acc_words(l);
   p->rows_word = rows_word;
   p->group_cols.assign(group_cols, group_cols + n_group);
   p->aggs = std::move(new_aggs);

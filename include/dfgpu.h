@@ -451,7 +451,11 @@ int dfgpu_lookup_create(dfgpu_ctx* ctx, int32_t key_type, const int32_t* payload
  *    and read again by the pipeline kernel. */
 int dfgpu_lookup_create_composite(dfgpu_ctx* ctx, const int32_t* key_types, const int64_t* key_min, const int64_t* key_max, int32_t n_keys,
                                   const int32_t* payload_types, int32_t n_payload, const dfgpu_lookup_options* opts, dfgpu_lookup** out);
-/* forget every record / key / filter bit, keep the allocations (a persistent build side refilled per query) */
+/* forget every record / key / filter bit, keep the allocations (a persistent build side refilled per query).  Every accumulator word
+ * (a FULL stage's visited marks included) is 0 again, and "rows" and "null_keys" restart at 0.  DFGPU_ERR_STATE while a pipeline with the
+ * join-keyed aggregate sink over this lookup is alive.  A clear is not needed between two aggregates or Full joins over the same build
+ * rows: dfgpu_pipeline_sink_aggregate zeroes words an earlier one wrote (one FULL stage per lookup still needs a clear, see
+ * dfgpu_pipeline_set_stage_full). */
 int dfgpu_lookup_clear(dfgpu_lookup* l);
 /* the membership filter as raw 64-bit blocks (device pointer + size): exported with dfgpu_ipc_export for the peer all-reduce below */
 int dfgpu_lookup_filter_buffer(dfgpu_lookup* l, void** words_dev, uint64_t* n_bytes);
@@ -533,6 +537,11 @@ int dfgpu_pipeline_create(dfgpu_ctx* ctx, const int32_t* input_types, int32_t n_
  *                and for both, a lookup whose build pushes held a NULL key ("null_keys" > 0) is DFGPU_ERR_UNSUPPORTED at the first
  *                push (those rows are not in the lookup, but the join emits them);
  *              every other sink over a LEFT / LEFT_ANTI stage is DFGPU_ERR_UNSUPPORTED;
+ *              one such sink per lookup at a time (a second one, or a FULL stage, while it is alive: DFGPU_ERR_STATE).  A lookup
+ *              serves any number of them in a row: each starts from zero.  When an earlier aggregate sink or FULL stage pushed into
+ *              the words, this call zeroes the accumulator words of every record first (kernel-timing family "lookup_acc_reset",
+ *              one write pass over capacity x stride x 8 bytes, not measured); a lookup fresh from creation or
+ *              dfgpu_lookup_clear launches nothing;
  *  output    : surviving rows, columns = out_cols of the virtual schema, input order preserved. */
 int dfgpu_pipeline_sink_build(dfgpu_pipeline* p, dfgpu_lookup* target, int32_t key_col, const int32_t* payload_cols, int32_t n_payload);
 /* the build sink of a composite-key lookup (dfgpu_lookup_create_composite): key = the packed tuple of the INPUT columns key_cols[0..n_keys),
@@ -636,7 +645,8 @@ int dfgpu_pipeline_set_stage_keys(dfgpu_pipeline* p, int32_t stage, const int32_
  * the first push (DFGPU_ERR_STATE otherwise).  DFGPU_ERR_INVALID: the stage is not RIGHT.  DFGPU_ERR_UNSUPPORTED: the stage is not the
  * pipeline's only stage; its lookup was not created with payload and n_acc_words >= 1; the inputs take all 16 column slots (the build
  * keys of (2) need one); the build side had a NULL key (at push or finish: such a row is not in the lookup).  DFGPU_ERR_STATE: the
- * lookup's marks (or accumulators) are already taken by another pipeline — one FULL pipeline per lookup until dfgpu_lookup_clear.  The
+ * lookup's marks (or accumulators) are already taken by another pipeline — one FULL pipeline per lookup until dfgpu_lookup_clear.  Words
+ * an earlier join-keyed aggregate sink wrote are zeroed by this call, as dfgpu_pipeline_sink_aggregate does.  The
  * build, pack and join-keyed aggregate sinks and stage filters stay DFGPU_ERR_UNSUPPORTED, as for any RIGHT stage. */
 int dfgpu_pipeline_set_stage_full(dfgpu_pipeline* p, int32_t stage);
 /* optional label: this pipeline's kernel is timed under the family "pipe:<name>" (dfgpu_set_kernel_timing / dfgpu_kernel_time) —
