@@ -12,7 +12,7 @@ datafusion/ffi/src/record_batch_stream.rs:101-167 does).
 """
 from __future__ import annotations
 
-from typing import Iterable, Iterator, List, Optional, Sequence, Tuple, Union
+from typing import Iterable, Iterator, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import pyarrow as pa
 
@@ -677,7 +677,7 @@ class _Scan:
         self.stages: List[Tuple[int, object, "GpuPipelineExec"]] = []  # (stage kind, probe key column — a list of them for a composite key, build pipeline)
         self.visible: List[str] = [f.name for f in source.schema]       # column names the operators above may still reference
         self.filters: dict = {}                                          # stage index -> its JoinFilter as stage-filter RPN nodes
-        self.full = False                                                # the only stage is a Full join's (fuse_full_joins)
+        self.full = False                                                # the only stage is a Full join's
 
     def virtual_schema(self) -> pa.Schema:
         # a Full join's unmatched build rows carry every probe column NULL (build_join_schema(..., "Full"))
@@ -691,6 +691,15 @@ class _Scan:
 
     def has_right(self) -> bool:
         return any(kind == D.STAGE_RIGHT for kind, _, _ in self.stages)
+
+
+class _Chain(NamedTuple):
+    """what a probe chain may contain (_as_scan): the join types its stages come from, and whether a join may carry a JoinFilter"""
+    joins: frozenset = frozenset({"Inner", "RightSemi", "RightAnti"})
+    filters: bool = False
+
+    def without_outer(self) -> "_Chain":
+        return self._replace(joins=self.joins - {"Right", "Full"})
 
 
 _FILTER_NODES = 128   # the node pool of a pipeline's stage filters (dfgpu_pipeline_set_stage_filter)
@@ -725,6 +734,11 @@ def _has_fallible_rhs(e: Expr, schema: pa.Schema) -> bool:
 _MAX_PIPE_COLS = 16   # input columns plus packed composite keys of one pipeline (dfgpu_pipeline_set_stage_keys)
 
 
+def _room_for_composite(sc: _Scan) -> bool:
+    """whether the pipeline of sc can pack one more composite key beside its source columns and the composite keys it packs already"""
+    return len(sc.source.schema) + sum(isinstance(k, list) for _, k, _ in sc.stages) + 1 <= _MAX_PIPE_COLS
+
+
 def _key_pairs(pkey, build: "GpuPipelineExec") -> List[Tuple[str, str]]:
     """(build key, probe key) of every key column of a stage: one pair, or one per component of a composite key"""
     if isinstance(pkey, list):
@@ -752,7 +766,7 @@ def _join_keys(join: GpuHashJoinExec, sc: _Scan):
         bt, pt = join.left.schema.field(b).type, sc.source.schema.field(pk).type
         if bt != pt or not _integer_like(bt):
             return None
-    if len(src) + sum(isinstance(k, list) for _, k, _ in sc.stages) + 1 > _MAX_PIPE_COLS:
+    if not _room_for_composite(sc):
         return None
     return [b for b, _ in join.on], [pk for _, pk in join.on]
 
@@ -761,7 +775,8 @@ def _stage_filter(sc: _Scan, join: GpuHashJoinExec, kind: int, payload: List[str
     """The join's JoinFilter as the RPN program of the stage it becomes (appended next to sc.stages), or None when it cannot run there.
     Its columns: a probe-side column -> that column of the probe chain's virtual schema, the build key -> the probe key, any other build
     column -> the stage's payload field (`payload`, in order; a SEMI / ANTI stage's fields are seen by its filter only).  Each column of
-    a composite key maps to its paired probe key."""
+    a composite key maps to its paired probe key.  None too when the pipeline's filters would exceed _FILTER_NODES nodes, or an AND / OR
+    has a right operand that can raise (÷, %, CAST, Decimal128 arithmetic)."""
     f = join.filter
     vs = sc.virtual_schema()
     fields = list(vs) + [join.left.schema.field(n) for n in payload]
@@ -820,17 +835,19 @@ def _settle_right(sc: _Scan, read: set) -> bool:
     return True
 
 
-def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False, full_joins: bool = False) -> Optional[_Scan]:
-    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(RightSemi / RightAnti / Inner / Right, one key or a composite
-    key (_join_keys), fusable build)]* over a source.  join_filters: a join may carry a JoinFilter, which becomes its stage's filter
-    (fuse_join_filters); a Right join never does.  right_joins: Right joins are accepted (fuse_right_joins); such a stage carries every
-    build column until _settle_right keeps those read above it.  full_joins (with right_joins): a Full join is accepted too, as a RIGHT
-    stage that also emits the unmatched build rows (fuse_full_joins), when it is the chain's only join: its probe side is [FilterExec]
-    over the source, and no join probes above it.  Its lookup takes one accumulator word, the visited marks."""
+def _as_scan(plan: ExecutionPlan, ch: _Chain = _Chain()) -> Optional[_Scan]:
+    """[ProjectionExec(columns only)]* over [FilterExec]? over [HashJoinExec(a join type of ch.joins, one key or a composite key
+    (_join_keys), NullEqualsNothing, not null-aware, fusable build)]* over a source.  When ch.filters allows it, a join may carry a
+    JoinFilter, which becomes its stage's filter (_stage_filter); a Right or Full join never does.  A Right join becomes a RIGHT stage
+    (DFGPU_STAGE_RIGHT) whose payload fields are nullable, as build_join_schema(..., "Right") makes them; it carries every build column
+    until _settle_right keeps those read above it.  A Full join becomes a RIGHT stage that also emits the unmatched build rows
+    (dfgpu_pipeline_set_stage_full) when it is the chain's only join: its probe side is [FilterExec] over the source, and no join probes
+    above it.  Those rows carry every probe column NULL, so the source columns are nullable in the virtual schema.  Its lookup takes one
+    accumulator word, the visited marks."""
     if isinstance(plan, GpuProjectionExec):
         if not all(isinstance(e, Column) and e.name == name for e, name in plan.exprs):
             return None
-        sc = _as_scan(plan.input, join_filters, right_joins, full_joins)
+        sc = _as_scan(plan.input, ch)
         if sc is not None:
             sc.visible = [name for _, name in plan.exprs]
         return sc
@@ -845,11 +862,10 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool 
             sc.visible = [inner.schema.field(i).name for i in plan.projection]
         return sc
     if isinstance(plan, GpuHashJoinExec):
-        kinds = ("RightSemi", "RightAnti", "Inner") + (("Right",) if right_joins and plan.filter is None else ()) + \
-            (("Full",) if right_joins and full_joins and plan.filter is None else ())
-        if plan.join_type not in kinds or (plan.filter is not None and not join_filters) or plan.null_aware or plan.null_equality != "NullEqualsNothing":
+        if plan.join_type not in ch.joins or (plan.filter is not None and (not ch.filters or plan.join_type in ("Right", "Full"))) or \
+                plan.null_aware or plan.null_equality != "NullEqualsNothing":
             return None
-        sc = _as_scan(plan.right, join_filters, right_joins, full_joins)
+        sc = _as_scan(plan.right, ch)
         if sc is not None and (sc.full or (plan.join_type == "Full" and sc.stages)):
             return None                                   # a FULL stage is the pipeline's only probe stage
         keys = None if sc is None else _join_keys(plan, sc)
@@ -869,7 +885,7 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool 
             filt = _stage_filter(sc, plan, kind, payload)
             if filt is None:
                 return None
-        build = _as_build(plan.left, bkey, payload, join_filters, max_bits=None if kind == D.STAGE_RIGHT else 64)
+        build = _as_build(plan.left, bkey, payload, ch, max_bits=None if kind == D.STAGE_RIGHT else 64)
         if build is None:
             return None
         if filt is not None:
@@ -886,12 +902,12 @@ def _as_scan(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool 
     return _Scan(plan)
 
 
-def _as_build(plan: ExecutionPlan, key, payload: List[str], join_filters: bool = False, max_bits: Optional[int] = 64) -> Optional["GpuPipelineExec"]:
+def _as_build(plan: ExecutionPlan, key, payload: List[str], ch: _Chain, max_bits: Optional[int] = 64) -> Optional["GpuPipelineExec"]:
     """the build pipeline of a fused join on `key` (a list of columns for a composite key: source columns with known bounds
     (_source_bounds) whose domain, the product of max - min + 1, is at most 2^63 - 1, so that the tuple packs into one 64-bit key).
-    max_bits None: the payload is settled later (a Right join's, _settle_right).  A build side with a Right join stays unfused: its NULL
-    payload fields cannot enter a lookup (_as_scan is not asked for Right joins here)."""
-    sc = _as_scan(plan, join_filters)
+    max_bits None: the payload is settled later (a Right join's, _settle_right).  A build side with a Right or Full join stays unfused:
+    its NULL payload fields cannot enter a lookup."""
+    sc = _as_scan(plan, ch.without_outer())
     if sc is None or len(sc.stages) >= 3:
         return None
     vs = sc.virtual_schema()
@@ -903,7 +919,7 @@ def _as_build(plan: ExecutionPlan, key, payload: List[str], join_filters: bool =
         return None
     ranges = []
     if isinstance(key, list):
-        if len(sc.source.schema) + sum(isinstance(k, list) for _, k, _ in sc.stages) + 1 > _MAX_PIPE_COLS:
+        if not _room_for_composite(sc):
             return None
         dom = 1
         for k in keys:
@@ -1123,20 +1139,51 @@ def _source_bounds(source: ExecutionPlan, name: str) -> Optional[Tuple[int, int]
     return lo, hi
 
 
-def _fuse_dense(plan: "GpuAggregateExec", right_joins: bool = False, full_joins: bool = False) -> Optional["GpuPipelineExec"]:
-    """AggregateExec over [ProjectionExec] over FilterExec over a source (no join) whose GROUP BY columns are source columns with known
-    bounds spanning at most DENSE_MAX_GROUPS slots (NULL included) -> a GpuPipelineExec with the dense sink; None otherwise"""
-    below, proj = plan.input, None
+def _agg_input(plan: "GpuAggregateExec") -> Tuple[ExecutionPlan, dict]:
+    """the plan under an aggregate and its optional ProjectionExec, and the expression over that plan of every column of the aggregate's
+    input"""
+    below = plan.input
     if isinstance(below, GpuProjectionExec):
-        proj, below = below, below.input
-    right = right_joins and isinstance(below, GpuHashJoinExec) and below.join_type in ("Right",) + (("Full",) if full_joins else ())
-    if not (isinstance(below, GpuFilterExec) or right):
+        return below.input, {name: e for e, name in below.exprs}
+    return below, {f.name: Column(f.name) for f in below.schema}
+
+
+def _agg_args(plan: "GpuAggregateExec", exprs: dict, vs: pa.Schema) -> Optional[list]:
+    """(aggregate, argument expression, its type, its RPN nodes over the virtual schema vs) of every aggregate of plan, the last three None
+    for COUNT(*); None when an aggregate has a FILTER clause or an argument that is no input column (`exprs`) or reads a name vs lacks,
+    or is an AVG whose state no sink holds: AVG(Decimal128) has no pinned Partial state, and any other AVG argument must be Float64"""
+    args = []
+    for a in plan.aggr_expr:
+        if a.filter is not None:
+            return None
+        if a.arg is None:
+            args.append((a, None, None, None))
+            continue
+        e = exprs.get(a.arg)
+        if e is None:
+            return None
+        nodes: list = []
+        try:
+            e.rpn(vs, nodes)
+            t = e.data_type(vs)
+        except KeyError:
+            return None
+        if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
+            return None
+        args.append((a, e, t, nodes))
+    return args
+
+
+def _fuse_dense(plan: "GpuAggregateExec", ch: _Chain) -> Optional["GpuPipelineExec"]:
+    """AggregateExec over [ProjectionExec] over FilterExec over a source (no join: TPC-H Q1, Q6), or over a chain that ch allows topped by
+    a Right or Full join, with no JoinFilter anywhere, whose GROUP BY columns have known bounds (_field_bounds) spanning at most
+    DENSE_MAX_GROUPS slots (NULL included); at most 8 aggregates, no Float32 MIN / MAX -> a GpuPipelineExec with the dense sink; None
+    otherwise"""
+    below, exprs = _agg_input(plan)
+    if not (isinstance(below, GpuFilterExec) or (isinstance(below, GpuHashJoinExec) and below.join_type in ("Right", "Full"))):
         return None
-    sc = _as_scan(below, right_joins=right, full_joins=full_joins)
-    if sc is None or (sc.stages and not right):
-        return None
-    exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
-    if right and not _settle_right(sc, _read_names(plan, exprs)):
+    sc = _as_scan(below, ch._replace(filters=False))
+    if sc is None or not _settle_right(sc, _read_names(plan, exprs)):
         return None
     vs = sc.virtual_schema()
     group, ranges, slots = [], [], 1
@@ -1154,26 +1201,11 @@ def _fuse_dense(plan: "GpuAggregateExec", right_joins: bool = False, full_joins:
         ranges.append(b)
     if len(plan.aggr_expr) > 8:
         return None
-    aggs = []
-    for a in plan.aggr_expr:
-        if a.filter is not None:
-            return None
-        e = None if a.arg is None else exprs.get(a.arg)
-        if a.arg is not None and e is None:
-            return None
-        if e is not None:
-            try:
-                e.rpn(vs, [])                              # every referenced name must be a column of the virtual schema
-                t = e.data_type(vs)
-            except KeyError:
-                return None
-            if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
-                return None                                # AVG(Decimal128) has no pinned Partial state
-            if a.func in ("min", "max") and t == pa.float32():
-                return None
-        aggs.append((a.func, e, a.alias))
-    return GpuPipelineExec(sc, sink="dense", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, key_range=ranges,
-                           fallback=plan if right else None)
+    args = _agg_args(plan, exprs, vs)
+    if args is None or any(a.func in ("min", "max") and t == pa.float32() for a, _, t, _ in args):
+        return None
+    return GpuPipelineExec(sc, sink="dense", group_by=group, aggs=[(a.func, e, a.alias) for a, e, _, _ in args], mode=plan.mode,
+                           out_schema=plan.schema, key_range=ranges, fallback=plan if sc.has_right() else None)
 
 
 def _read_names(plan: "GpuAggregateExec", exprs: dict) -> set:
@@ -1218,88 +1250,53 @@ def _acc_words(funcs: Sequence[str], types: Sequence[Optional[pa.DataType]], has
     return n
 
 
-def fuse_pipelines(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
-    """PhysicalOptimizerRule twin (INTEGRATION.md §2a): AggregateExec(Single / SinglePartitioned / Partial) over [ProjectionExec] over
-    HashJoinExec(Inner) whose GROUP BY is the probe key plus build-side columns becomes ONE GpuPipelineExec; its build side (filters, semi
-    joins, column projections) becomes build pipelines.  The same AggregateExec over [ProjectionExec] over FilterExec over a source, with
-    no join, becomes a GpuPipelineExec with the dense sink when its GROUP BY columns have small known bounds (_fuse_dense: TPC-H Q1, Q6).
-    Left joins (the build side kept): the same AggregateExec over HashJoinExec(Left) grouped on the build key plus build columns
-    (_fuse_left: TPC-H Q13), and a top-level HashJoinExec(LeftSemi / LeftAnti) (_fuse_left_filter: Q18, Q20, Q22) become a GpuPipelineExec
-    with the join-keyed sink.  Their rows come out in slot order: the reference does not keep the build side's order either
-    (maintains_input_order is false for it).  Anything else is returned unchanged (the unfused Gpu*Exec operators run).
-    join_filters: joins with a JoinFilter fuse too (fuse_join_filters).  right_joins / full_joins: see _as_scan."""
-    if isinstance(plan, GpuHashJoinExec) and plan.join_type in ("LeftSemi", "LeftAnti"):
-        fused = _fuse_left_filter(plan, join_filters)
-        return plan if fused is None else fused
-    if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial"):
-        return plan
-    dense = _fuse_dense(plan, right_joins, full_joins)
-    if dense is not None:
-        return dense
-    if not plan.group_by:
-        return plan
-    below, proj = plan.input, None
-    if isinstance(below, GpuProjectionExec):
-        proj, below = below, below.input
-    if isinstance(below, GpuHashJoinExec) and below.join_type == "Left":
-        fused = _fuse_left(plan, below, proj, join_filters)
-        return plan if fused is None else fused
+def _fuse_inner(plan: "GpuAggregateExec", ch: _Chain) -> Optional["GpuPipelineExec"]:
+    """AggregateExec over [ProjectionExec] over HashJoinExec(Inner), a chain that ch allows without its Right and Full joins, whose GROUP BY
+    is the probe key of that last Inner stage (or the equal build key; every component of a composite key) plus its payload fields ->
+    ONE GpuPipelineExec with the join-keyed sink, its build side (filters, semi joins, column projections) a build pipeline; at most 12
+    accumulator words (_acc_words); None otherwise"""
+    below, exprs = _agg_input(plan)
     if not isinstance(below, GpuHashJoinExec) or below.join_type != "Inner":
-        return plan
-    sc = _as_scan(below, join_filters)
-    if sc is None or not sc.stages or sc.stages[-1][0] != D.STAGE_INNER:
-        return plan
-    kind, pkey, build = sc.stages[-1]
+        return None
+    sc = _as_scan(below, ch.without_outer())
+    if sc is None:
+        return None
+    _, pkey, build = sc.stages[-1]
     vs = sc.virtual_schema()
-    exprs = {name: e for e, name in proj.exprs} if proj is not None else {f.name: Column(f.name) for f in below.schema}
-    # group keys: the probe key (or the equal build key; every component of a composite key) and payload fields of the LAST inner stage
     paired = dict(_key_pairs(pkey, build))
     pkeys = list(paired.values())
     group = []
     for g in plan.group_by:
         e = exprs.get(g)
         if not isinstance(e, Column):
-            return plan
+            return None
         n = paired.get(e.name, e.name)
         if n not in pkeys and n not in build.payload:
-            return plan
+            return None
         group.append(n)
     if any(k not in group for k in pkeys):
-        return plan
-    aggs = []
-    for a in plan.aggr_expr:
-        if a.filter is not None:
-            return plan
-        e = None if a.arg is None else exprs.get(a.arg)
-        if a.arg is not None and e is None:
-            return plan
-        aggs.append((a.func, e, a.alias))
-    try:
-        for _, e, _ in aggs:
-            if e is not None:
-                e.rpn(vs, [])                              # every referenced name must exist in the virtual schema
-        types = [None if e is None else e.data_type(vs) for _, e, _ in aggs]
-    except KeyError:
-        return plan
-    for (f, _, _), t in zip(aggs, types):
-        if f == "avg" and t is not None and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
-            return plan                                    # AVG(Decimal128) has no pinned Partial state
-    n_acc = _acc_words([f for f, _, _ in aggs], types, bool(build.payload))
-    if n_acc > 12:
-        return plan
-    build.n_acc_words = n_acc
-    return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
-
-
-def _left_join_scan(join: GpuHashJoinExec, kind: int, join_filters: bool = False) -> Optional[_Scan]:
-    """The probe chain of a Left / LeftSemi / LeftAnti join with the join as its last stage (kind), or None.  Conditions: one key or a
-    composite key (_join_keys), no JoinFilter, NullEqualsNothing, not null-aware; the right side is an _as_scan chain probing on its
-    source columns; the left side is a fusable build whose key fields are declared non-nullable (a NULL build key is never in the lookup,
-    but Left / LeftAnti emit its row) and have the probe keys' types.  The build's payload is every other left column.  join_filters: a
-    JoinFilter is allowed and becomes the stage's filter."""
-    if (join.filter is not None and not join_filters) or join.null_aware or join.null_equality != "NullEqualsNothing":
         return None
-    sc = _as_scan(join.right, join_filters)
+    args = _agg_args(plan, exprs, vs)
+    if args is None:
+        return None
+    n_acc = _acc_words([a.func for a, _, _, _ in args], [t for _, _, t, _ in args], bool(build.payload))
+    if n_acc > 12:
+        return None
+    build.n_acc_words = n_acc
+    return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=[(a.func, e, a.alias) for a, e, _, _ in args], mode=plan.mode,
+                           out_schema=plan.schema)
+
+
+def _left_join_scan(join: GpuHashJoinExec, kind: int, ch: _Chain) -> Optional[_Scan]:
+    """The probe chain of a Left / LeftSemi / LeftAnti join with the join as its last stage (kind), or None.  Conditions: one key or a
+    composite key (_join_keys), NullEqualsNothing, not null-aware; the right side is a chain that ch allows without its Right and Full
+    joins, probing on its source columns; the left side is a fusable build whose key fields are declared non-nullable (a NULL build key
+    is never in the lookup, but Left / LeftAnti emit its row) and have the probe keys' types.  The build's payload is every other left
+    column.  A JoinFilter, when ch allows one, becomes the stage's filter.  The fused join emits its rows in slot order: the reference
+    does not keep the build side's order either (maintains_input_order is false for it)."""
+    if (join.filter is not None and not ch.filters) or join.null_aware or join.null_equality != "NullEqualsNothing":
+        return None
+    sc = _as_scan(join.right, ch.without_outer())
     keys = None if sc is None or len(sc.stages) >= 3 else _join_keys(join, sc)
     if keys is None:
         return None
@@ -1318,7 +1315,7 @@ def _left_join_scan(join: GpuHashJoinExec, kind: int, join_filters: bool = False
         filt = _stage_filter(sc, join, kind, payload)
         if filt is None:
             return None
-    build = _as_build(join.left, bkey, payload, join_filters)
+    build = _as_build(join.left, bkey, payload, ch)
     if build is None:
         return None
     if filt is not None:
@@ -1327,16 +1324,19 @@ def _left_join_scan(join: GpuHashJoinExec, kind: int, join_filters: bool = False
     return sc
 
 
-def _fuse_left(plan: "GpuAggregateExec", join: GpuHashJoinExec, proj: Optional[GpuProjectionExec], join_filters: bool = False) -> Optional["GpuPipelineExec"]:
-    """AggregateExec over [ProjectionExec] over HashJoinExec(Left) -> the join-keyed sink over a LEFT stage, or None.  GROUP BY the build
-    key (not the probe key: NULL on a padded row) plus build columns; every aggregate COUNT(*) or an argument over right-side columns that
-    reads a probe source column and propagates NULL, so that it is NULL on a build row's padded row."""
-    sc = _left_join_scan(join, D.STAGE_LEFT, join_filters)
+def _fuse_left(plan: "GpuAggregateExec", ch: _Chain) -> Optional["GpuPipelineExec"]:
+    """AggregateExec over [ProjectionExec] over HashJoinExec(Left) -> the join-keyed sink over a LEFT stage (TPC-H Q13), or None.  GROUP BY
+    the build key (not the probe key: NULL on a padded row) plus build columns; every aggregate COUNT(*) or an argument over right-side
+    columns that reads a probe source column and propagates NULL, so that it is NULL on a build row's padded row; no Float32 MIN / MAX;
+    at most 12 accumulator words (_acc_words)."""
+    join, exprs = _agg_input(plan)
+    if not isinstance(join, GpuHashJoinExec) or join.join_type != "Left":
+        return None
+    sc = _left_join_scan(join, D.STAGE_LEFT, ch)
     if sc is None:
         return None
     _, pkey, build = sc.stages[-1]
     vs = sc.virtual_schema()
-    exprs = {name: e for e, name in proj.exprs} if proj is not None else {f.name: Column(f.name) for f in join.schema}
     paired = dict(_key_pairs(pkey, build))
     group = []
     for g in plan.group_by:
@@ -1346,45 +1346,34 @@ def _fuse_left(plan: "GpuAggregateExec", join: GpuHashJoinExec, proj: Optional[G
         group.append(paired.get(e.name, e.name))
     if any(k not in group for k in paired.values()):
         return None
+    args = _agg_args(plan, exprs, vs)                      # the build key is not in the virtual schema
+    if args is None:
+        return None
     n_src, left_payload = len(sc.source.schema), range(len(vs) - len(build.payload), len(vs))
-    aggs, types = [], []
-    for a in plan.aggr_expr:
-        if a.filter is not None:
-            return None
-        if a.arg is None:
-            aggs.append(("count_star", None, a.alias)); types.append(None)
-            continue
-        e = exprs.get(a.arg)
+    for a, e, t, nodes in args:
         if e is None:
-            return None
-        nodes: list = []
-        try:
-            e.rpn(vs, nodes)                               # the build key is not in the virtual schema
-            t = e.data_type(vs)
-        except KeyError:
-            return None
+            continue
         if not any(n[0] == D.EXPR_COLUMN and n[1] < n_src for n in nodes):
             return None
         for n in nodes:
             if (n[0] == D.EXPR_COLUMN and n[1] in left_payload) or n[0] in (D.EXPR_IS_NULL, D.EXPR_IS_NOT_NULL) or \
                     (n[0] == D.EXPR_BINARY and n[1] in (D.OP_AND, D.OP_OR, D.OP_IS_DISTINCT_FROM, D.OP_IS_NOT_DISTINCT_FROM)):
                 return None
-        if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
-            return None                                    # AVG(Decimal128) has no pinned Partial state
         if a.func in ("min", "max") and t == pa.float32():
             return None
-        aggs.append((a.func, e, a.alias)); types.append(t)
-    n_acc = _acc_words([f for f, _, _ in aggs], types, bool(build.payload))
+    aggs = [("count_star" if e is None else a.func, e, a.alias) for a, e, _, _ in args]
+    n_acc = _acc_words([f for f, _, _ in aggs], [t for _, _, t, _ in args], bool(build.payload))
     if n_acc > 12:
         return None
     build.n_acc_words = n_acc
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema)
 
 
-def _fuse_left_filter(join: GpuHashJoinExec, join_filters: bool = False) -> Optional["GpuPipelineExec"]:
-    """HashJoinExec(LeftSemi / LeftAnti) -> the join-keyed sink without aggregates, grouped on every left column, or None.  LeftSemi is an
-    INNER stage over the unique build keys (the records a probe row reached), LeftAnti a LEFT_ANTI stage (the records none reached)."""
-    sc = _left_join_scan(join, D.STAGE_INNER if join.join_type == "LeftSemi" else D.STAGE_LEFT_ANTI, join_filters)
+def _fuse_left_filter(join: GpuHashJoinExec, ch: _Chain) -> Optional["GpuPipelineExec"]:
+    """HashJoinExec(LeftSemi / LeftAnti) -> the join-keyed sink without aggregates, grouped on every left column, or None (TPC-H Q18, Q20,
+    Q22).  LeftSemi is an INNER stage over the unique build keys (the records a probe row reached), LeftAnti a LEFT_ANTI stage (the
+    records none reached)."""
+    sc = _left_join_scan(join, D.STAGE_INNER if join.join_type == "LeftSemi" else D.STAGE_LEFT_ANTI, ch)
     if sc is None:
         return None
     _, pkey, build = sc.stages[-1]
@@ -1397,113 +1386,67 @@ def _fuse_left_filter(join: GpuHashJoinExec, join_filters: bool = False) -> Opti
     return GpuPipelineExec(sc, sink="aggregate", group_by=group, mode="Single", out_schema=join.schema, project=project)
 
 
-def fuse_hash_aggregates(plan: ExecutionPlan, join_filters: bool = False, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
-    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_pipelines: its result when that rule fuses; otherwise an
-    AggregateExec(Single / SinglePartitioned / Partial) with at least one GROUP BY column over [ProjectionExec] over an Inner join chain or a
-    FilterExec (as _as_scan accepts them) becomes ONE GpuPipelineExec with the hash-keyed sink (dfgpu_pipeline_sink_aggregate_hash: TPC-H
-    Q15's revenue0, Q3 grouped by o_custkey).  Every group key must be a plain integer-like column of the virtual schema, the packed key
-    (each column at its width, one more bit per nullable column) at most 128 bits; no FILTER clause, at most 4 aggregates, and the argument
-    types the library accepts.  Anything else, a bare scan included, is returned unchanged (dfgpu_agg runs).  join_filters: joins with a
-    JoinFilter fuse too (fuse_join_filters)."""
-    fused = fuse_pipelines(plan, join_filters, right_joins, full_joins)
-    if fused is not plan:
-        return fused
-    if not isinstance(plan, GpuAggregateExec) or plan.mode not in ("Single", "SinglePartitioned", "Partial") or not plan.group_by:
-        return plan
-    below, proj = plan.input, None
-    if isinstance(below, GpuProjectionExec):
-        proj, below = below, below.input
-    kinds = ("Inner",) + (("Right",) if right_joins else ()) + (("Full",) if right_joins and full_joins else ())
-    if not ((isinstance(below, GpuHashJoinExec) and below.join_type in kinds) or isinstance(below, GpuFilterExec)):
-        return plan
-    sc = _as_scan(below, join_filters, right_joins, full_joins)
+def _fuse_hash(plan: "GpuAggregateExec", ch: _Chain) -> Optional["GpuPipelineExec"]:
+    """AggregateExec over [ProjectionExec] over an Inner, Right or Full join chain or a FilterExec (as _as_scan accepts them under ch) ->
+    ONE GpuPipelineExec with the hash-keyed sink (dfgpu_pipeline_sink_aggregate_hash: TPC-H Q15's revenue0, Q3 grouped by o_custkey), or
+    None.  Every group key must be a plain integer-like column of the virtual schema, the packed key (each column at its width, one more
+    bit per nullable column) at most 128 bits; at most 4 aggregates, no Float32 MIN / MAX and no SUM / MIN / MAX / AVG over Boolean."""
+    below, exprs = _agg_input(plan)
+    if not ((isinstance(below, GpuHashJoinExec) and below.join_type in ("Inner", "Right", "Full")) or isinstance(below, GpuFilterExec)):
+        return None
+    sc = _as_scan(below, ch)
     # a composite-key stage under the hash-keyed sink (TPC-H Q9's lineitem x partsupp profit by supplier) measured slower than the
     # unfused dfgpu_hashjoin -> dfgpu_agg (README): that shape stays unfused
     if sc is None or any(isinstance(k, list) for _, k, _ in sc.stages):
-        return plan
-    exprs = {name: e for e, name in proj.exprs} if proj is not None else {n: Column(n) for n in sc.visible}
+        return None
     if not _settle_right(sc, _read_names(plan, exprs)):
-        return plan
+        return None
     vs = sc.virtual_schema()
     group, nullable, bits = [], [], 0
     for g in plan.group_by:
         e = exprs.get(g)
         if not isinstance(e, Column) or e.name not in sc.visible or vs.get_field_index(e.name) < 0:
-            return plan
+            return None
         f = vs.field(e.name)
-        if not (pa.types.is_integer(f.type) or pa.types.is_date32(f.type) or pa.types.is_date64(f.type) or pa.types.is_timestamp(f.type)):
-            return plan
+        if not _integer_like(f.type):
+            return None
         bits += D.WIDTH[type_id(f.type)] * 8 + (1 if f.nullable else 0)
         group.append(e.name)
         nullable.append(f.nullable)
     if bits > 128 or len(plan.aggr_expr) > 4:
-        return plan
-    aggs = []
-    for a in plan.aggr_expr:
-        if a.filter is not None:
-            return plan
-        e = None if a.arg is None else exprs.get(a.arg)
-        if a.arg is not None and e is None:
-            return plan
-        if e is not None:
-            try:
-                e.rpn(vs, [])                              # every referenced name must exist in the virtual schema
-                t = e.data_type(vs)
-            except KeyError:
-                return plan
-            if a.func == "avg" and t != pa.float64() and not (pa.types.is_decimal128(t) and plan.mode != "Partial"):
-                return plan                                # AVG(Decimal128) has no pinned Partial state
-            if a.func in ("min", "max") and t == pa.float32():
-                return plan
-            if pa.types.is_boolean(t) and a.func != "count":
-                return plan
-        aggs.append((a.func, e, a.alias))
-    return GpuPipelineExec(sc, sink="hash", group_by=group, aggs=aggs, mode=plan.mode, out_schema=plan.schema, nullable=nullable,
-                           fallback=plan if sc.has_right() else None)
+        return None
+    args = _agg_args(plan, exprs, vs)
+    if args is None or any(a.func in ("min", "max") and t == pa.float32() for a, _, t, _ in args):
+        return None
+    if any(t is not None and pa.types.is_boolean(t) and a.func != "count" for a, _, t, _ in args):
+        return None
+    return GpuPipelineExec(sc, sink="hash", group_by=group, aggs=[(a.func, e, a.alias) for a, e, _, _ in args], mode=plan.mode,
+                           out_schema=plan.schema, nullable=nullable, fallback=plan if sc.has_right() else None)
 
 
-def fuse_join_filters(plan: ExecutionPlan, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
-    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_hash_aggregates: its result when that rule fuses; otherwise the same
-    shapes again with JoinFilters allowed on the Inner / RightSemi / RightAnti joins of a probe chain and on a Left / LeftSemi / LeftAnti
-    join that is the last stage.  Each filter becomes its stage's filter (dfgpu_pipeline_set_stage_filter): a probe-side column maps to
-    the probe chain's column, the build key to the probe key, other build columns to the stage's payload fields (a RightSemi /
-    RightAnti build carries exactly the columns its filter reads).  A plan is left unchanged when a payload would exceed 64 bits, the
-    filters 128 nodes, or an AND / OR has a right operand that can raise (÷, %, CAST, Decimal128 arithmetic)."""
-    fused = fuse_hash_aggregates(plan, right_joins=right_joins, full_joins=full_joins)
-    if fused is not plan:
-        return fused
-    return fuse_hash_aggregates(plan, join_filters=True, right_joins=right_joins, full_joins=full_joins)
-
-
-def fuse_output_pipelines(plan: ExecutionPlan, right_joins: bool = False, full_joins: bool = False) -> ExecutionPlan:
-    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_join_filters: its result when that rule fuses; otherwise a top-level
-    [ProjectionExec(columns only)] over a HashJoinExec(Inner / RightSemi / RightAnti) chain, as _as_scan accepts it with JoinFilters and
-    with at least one stage, becomes ONE GpuPipelineExec over the ordered output sink (dfgpu_pipeline_sink_output) that emits the plan's
-    schema: a probe-side column comes from the input, the build key of an Inner stage from its probe key (only when the two have the
-    same type), any other build column from the stage's payload field.  The fused lookups need unique build keys: an Inner stage without
-    payload gets a row-counter word, so its build refuses duplicate keys like one with payload.  Whether the keys are unique is known
-    only once the build side has run, so the fused node keeps the plan as its fallback: a build the library refuses (duplicate keys,
-    NULL payloads) runs the unfused joins instead, before any row is emitted.  The fused Inner join emits its rows in probe order, the
-    reference's order for unique build keys.  Anything else (a bare FilterExec, Left / Right / Full joins, several keys,
-    null-aware joins, computed projections) is returned unchanged."""
-    fused = fuse_join_filters(plan, right_joins, full_joins)
-    if fused is not plan:
-        return fused
+def _fuse_output(plan: ExecutionPlan, ch: _Chain) -> Optional["GpuPipelineExec"]:
+    """A top-level [ProjectionExec(columns only)] over a HashJoinExec chain that ch allows -> ONE GpuPipelineExec over the ordered output
+    sink (dfgpu_pipeline_sink_output) that emits the plan's schema: a probe-side column comes from the input, the build key of an Inner
+    stage from its probe key (only when the two have the same type), any other build column from the stage's payload field.  The fused
+    lookups need unique build keys: an Inner stage without payload gets a row-counter word, so its build refuses duplicate keys like one
+    with payload.  Whether the keys are unique is known only once the build side has run, so the fused node keeps the plan as its
+    fallback: a build the library refuses (duplicate keys, NULL payloads) runs the unfused joins instead, before any row is emitted.  The
+    fused Inner join emits its rows in probe order, the reference's order for unique build keys.  None for anything else (a bare
+    FilterExec, a Left join, a computed projection)."""
     join = plan.input if isinstance(plan, GpuProjectionExec) else plan
-    kinds = ("Inner", "RightSemi", "RightAnti") + (("Right",) if right_joins else ()) + (("Full",) if right_joins and full_joins else ())
-    if not isinstance(join, GpuHashJoinExec) or join.join_type not in kinds:
-        return plan
-    sc = _as_scan(join, join_filters=True, right_joins=right_joins, full_joins=full_joins)
-    if sc is None or not sc.stages:
-        return plan
+    if not isinstance(join, GpuHashJoinExec):
+        return None
+    sc = _as_scan(join, ch)
+    if sc is None:
+        return None
     pick = list(range(len(join.column_indices)))                                # the join's columns that form the output
     if isinstance(plan, GpuProjectionExec):
         names = [f.name for f in join.schema]
         if not all(isinstance(e, Column) and names.count(e.name) == 1 for e, _ in plan.exprs):
-            return plan
+            return None
         pick = [names.index(e.name) for e, _ in plan.exprs]
     if not _settle_right(sc, {join.schema.field(i).name for i in pick}):
-        return plan
+        return None
     vs = sc.virtual_schema()
     kind, pkey, build = sc.stages[-1]
     n_below = len(vs) - (len(build.payload) if kind in (D.STAGE_INNER, D.STAGE_RIGHT) else 0)   # the virtual columns the top join's probe side sees
@@ -1532,7 +1475,7 @@ def fuse_output_pipelines(plan: ExecutionPlan, right_joins: bool = False, full_j
             else:
                 at = n_below + build.payload.index(name) if name in build.payload else -1
         if at < 0:
-            return plan
+            return None
         cols.append(at)
     for k, _, b in sc.stages:
         if k == D.STAGE_INNER and not b.payload:
@@ -1540,38 +1483,60 @@ def fuse_output_pipelines(plan: ExecutionPlan, right_joins: bool = False, full_j
     return GpuPipelineExec(sc, sink="output", out_schema=plan.schema, out_cols=cols, fallback=plan)
 
 
+# the levels of the fusion rule, each fusing what the level before it does and more
+_JOIN_KEYED, _HASH_SINK, _JOIN_FILTERS, _OUTPUT_SINK, _RIGHT_JOINS, _FULL_JOINS = range(6)
+
+
+def _fuse(plan: ExecutionPlan, level: int) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §2a) at `level`: a top-level HashJoinExec(LeftSemi / LeftAnti) onto the join-keyed sink
+    (_fuse_left_filter); an AggregateExec(Single / SinglePartitioned / Partial) onto the first sink that takes it: the dense sink, the
+    join-keyed sink over a Left or an Inner join, and from _HASH_SINK on the hash sink; from _OUTPUT_SINK on, a plan none of those takes
+    onto the ordered output sink.  From _JOIN_FILTERS on a probe chain's joins may carry JoinFilters, from _RIGHT_JOINS on it may
+    contain Right joins, and at _FULL_JOINS a Full join.  Anything else is returned unchanged (the unfused Gpu*Exec operators run)."""
+    joins = _Chain().joins | ({"Right"} if level >= _RIGHT_JOINS else set()) | ({"Full"} if level >= _FULL_JOINS else set())
+    ch = _Chain(joins, filters=level >= _JOIN_FILTERS)
+    fused = None
+    if isinstance(plan, GpuHashJoinExec) and plan.join_type in ("LeftSemi", "LeftAnti"):
+        fused = _fuse_left_filter(plan, ch)
+    elif isinstance(plan, GpuAggregateExec) and plan.mode in ("Single", "SinglePartitioned", "Partial"):
+        fused = _fuse_dense(plan, ch)
+        if fused is None and plan.group_by:
+            fused = _fuse_left(plan, ch) or _fuse_inner(plan, ch) or (_fuse_hash(plan, ch) if level >= _HASH_SINK else None)
+    if fused is None and level >= _OUTPUT_SINK:
+        fused = _fuse_output(plan, ch)
+    return plan if fused is None else fused
+
+
+def fuse_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
+    """The fusion rule's first level (_fuse): the dense and join-keyed sinks"""
+    return _fuse(plan, _JOIN_KEYED)
+
+
+def fuse_hash_aggregates(plan: ExecutionPlan) -> ExecutionPlan:
+    """The fusion rule (_fuse) with the hash-keyed sink too"""
+    return _fuse(plan, _HASH_SINK)
+
+
+def fuse_join_filters(plan: ExecutionPlan) -> ExecutionPlan:
+    """The fusion rule (_fuse) with the hash-keyed sink and JoinFilters too"""
+    return _fuse(plan, _JOIN_FILTERS)
+
+
+def fuse_output_pipelines(plan: ExecutionPlan) -> ExecutionPlan:
+    """The fusion rule (_fuse) with the hash-keyed sink, JoinFilters and the ordered output sink too"""
+    return _fuse(plan, _OUTPUT_SINK)
+
+
 def fuse_right_joins(plan: ExecutionPlan) -> ExecutionPlan:
-    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_output_pipelines: its result when that rule fuses; otherwise the same
-    shapes again with HashJoinExec(Right) joins allowed in the probe chain (DFGPU_STAGE_RIGHT) — DataFusion's join selection puts the
-    smaller input on the build side, so `fact LEFT JOIN dimension` arrives as a Right join with the dimension as the build.  A Right join
-    qualifies with one key or a composite key, NullEqualsNothing, not null-aware and without a JoinFilter; its stage carries the build
-    columns read above it (a build key too: it is NULL on unmatched rows, so it never stands in for the probe key), at least one and at
-    most 64 bits, since only a lookup with payload enforces the unique keys a Right stage needs.  Its payload fields are nullable in the
-    virtual schema, as build_join_schema(..., "Right") makes them.  Sinks: the ordered output sink, the dense sink (group columns with
-    known bounds: source columns, or payload fields taken from a source column of the build side) and the hash sink (a RIGHT payload
-    group column declared nullable); never a build side or the join-keyed sink.  Whether the build keys are unique is known only once the
-    build has run, so every fused node keeps the plan as its fallback (a duplicate key runs the unfused joins, before any row is
-    emitted)."""
-    fused = fuse_output_pipelines(plan)
-    if fused is not plan:
-        return fused
-    return fuse_output_pipelines(plan, right_joins=True)
+    """The fusion rule (_fuse) with the hash-keyed sink, JoinFilters, the ordered output sink and Right joins too: DataFusion's join
+    selection puts the smaller input on the build side, so `fact LEFT JOIN dimension` arrives as a Right join with the dimension as the
+    build"""
+    return _fuse(plan, _RIGHT_JOINS)
 
 
 def fuse_full_joins(plan: ExecutionPlan) -> ExecutionPlan:
-    """PhysicalOptimizerRule twin (INTEGRATION.md §2a), after fuse_right_joins: its result when that rule fuses; otherwise the same
-    shapes again with a HashJoinExec(Full) allowed as the probe chain's only join (a RIGHT stage turned into a Full join,
-    dfgpu_pipeline_set_stage_full): its probe side is [FilterExec] over a source.  The conditions and sinks are fuse_right_joins': one key or
-    a composite key, NullEqualsNothing, not null-aware, no JoinFilter; the stage carries the build columns read above the join (the build
-    key included, NULL on unmatched probe rows), 1 to 64 bits, as nullable fields; the ordered output, dense and hash sinks.  Its lookup
-    takes one accumulator word for the visited marks.  The build rows no probe row matched follow the probe rows with every probe column
-    NULL, so the source columns are nullable in the virtual schema, and a probe-side group column of the hash sink is declared nullable.
-    The fused node's schema is the plan's (build_join_schema(..., "Full"), projected).  A build the library refuses (duplicate or NULL
-    keys) runs the plan instead, its fallback, before any row is emitted."""
-    fused = fuse_right_joins(plan)
-    if fused is not plan:
-        return fused
-    return fuse_output_pipelines(plan, right_joins=True, full_joins=True)
+    """The fusion rule (_fuse) at its widest: the hash-keyed sink, JoinFilters, the ordered output sink, Right joins and a Full join too"""
+    return _fuse(plan, _FULL_JOINS)
 
 
 # ---------------------------------------------------------------------------------------------
