@@ -13,7 +13,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdfgpu.so")
-STRINGS_LIB_PATH = os.path.join(_HERE, "libdfgpu_strings.so")   # include/dfgpu_strings.h: LIKE over string columns (own library)
+STRINGS_LIB_PATH = os.path.join(_HERE, "libdfgpu_strings.so")   # include/dfgpu_strings.h: string predicates (own library)
 
 # ---- enums (mirror include/dfgpu.h) -------------------------------------------------------
 OK, END = 0, 1
@@ -1036,9 +1036,12 @@ class Exchange:
 STRING_UTF8, STRING_LARGE_UTF8, STRING_UTF8_VIEW = 1, 2, 3
 LIKE_NEGATED, LIKE_CASE_INSENSITIVE = 1, 2
 LIKE_MAX_PATTERN_BYTES, LIKE_MAX_SEGMENTS = 256, 16
+STRING_EQ, STRING_NE, STRING_LT, STRING_LE, STRING_GT, STRING_GE = range(6)
+STRING_CMP_OPS = {"=": STRING_EQ, "<>": STRING_NE, "!=": STRING_NE, "<": STRING_LT, "<=": STRING_LE, ">": STRING_GT, ">=": STRING_GE}
+STRING_MAX_LITERAL_BYTES, STRING_IN_MAX_VALUES, STRING_IN_MAX_BYTES = 256, 64, 1024
 
 # every symbol include/dfgpu_strings.h declares
-STRINGS_EXPORTS = ["dfgpu_like", "dfgpu_like_codes", "dfgpu_strings_last_error"]
+STRINGS_EXPORTS = ["dfgpu_like", "dfgpu_like_codes", "dfgpu_string_compare", "dfgpu_string_in_list", "dfgpu_strings_last_error"]
 
 
 class StringColumn(C.Structure):
@@ -1063,6 +1066,11 @@ def load_strings_library() -> C.CDLL:
     lib.dfgpu_like.argtypes = [vp, C.POINTER(StringColumn), C.c_char_p, C.c_int64, C.c_int32, vp, vp]
     lib.dfgpu_like_codes.restype = C.c_int
     lib.dfgpu_like_codes.argtypes = [vp, C.POINTER(Column), vp, C.c_int64, vp, vp]
+    lib.dfgpu_string_compare.restype = C.c_int
+    lib.dfgpu_string_compare.argtypes = [vp, C.POINTER(StringColumn), C.c_int32, C.c_char_p, C.c_int64, vp, vp]
+    lib.dfgpu_string_in_list.restype = C.c_int
+    lib.dfgpu_string_in_list.argtypes = [vp, C.POINTER(StringColumn), C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.c_int64, C.c_int32,
+                                         C.c_int32, vp, vp]
     lib.dfgpu_strings_last_error.restype = C.c_char_p
     lib.dfgpu_strings_last_error.argtypes = []
     _strings_lib = lib
@@ -1090,7 +1098,7 @@ class DeviceStrings:
         elif pa.types.is_string_view(t):
             self.layout, width = STRING_UTF8_VIEW, 16
         else:
-            raise NotImplementedError(f"This feature is not implemented: LIKE on the GPU over Arrow type {t}")
+            raise NotImplementedError(f"This feature is not implemented: string predicates on the GPU over Arrow type {t}")
         self.ctx, self.length, self.offset, self.null_count = ctx, len(arr), arr.offset, arr.null_count
         bufs = arr.buffers()
 
@@ -1132,9 +1140,44 @@ def like(ctx: Context, strings, pattern, negated: bool = False, case_insensitive
     return DeviceColumn(ctx, UINT8, n, values, validity, ds.null_count if validity is not None else 0)
 
 
+def string_compare(ctx: Context, strings, op, literal) -> DeviceColumn:
+    """`strings op literal` (dfgpu_string_compare) -> a UINT8 DeviceColumn in {0, 1}, NULL where the string is NULL.  op: one of "=",
+    "<>" ("!="), "<", "<=", ">", ">=" or a STRING_* code; literal: str or UTF-8 bytes.  strings as in like()."""
+    ds = strings if isinstance(strings, DeviceStrings) else DeviceStrings(ctx, strings)
+    code = STRING_CMP_OPS[op] if isinstance(op, str) else int(op)
+    lib = load_strings_library()
+    n = ds.length
+    values = DeviceBuffer(ctx, n)
+    validity = DeviceBuffer(ctx, (n + 7) // 8) if ds.validity is not None else None
+    lit = _pattern_bytes(literal)
+    col = ds.c()
+    _strings_check(lib.dfgpu_string_compare(ctx.lib.dfgpu_ctx_stream(ctx.h), C.byref(col), code, lit, len(lit), C.c_void_p(values.ptr),
+                                            C.c_void_p(validity.ptr) if validity is not None else None))
+    return DeviceColumn(ctx, UINT8, n, values, validity, ds.null_count if validity is not None else 0)
+
+
+def string_in_list(ctx: Context, strings, values, negated: bool = False) -> DeviceColumn:
+    """`strings [NOT] IN (values)` (dfgpu_string_in_list) -> a UINT8 DeviceColumn in {0, 1} with SQL's three-valued IN: NULL where the
+    string is NULL, and where it is found nowhere while `values` holds a None.  values: str / UTF-8 bytes / None.  strings as in like()."""
+    ds = strings if isinstance(strings, DeviceStrings) else DeviceStrings(ctx, strings)
+    lib = load_strings_library()
+    vals = [_pattern_bytes(v) for v in values if v is not None]
+    has_null = any(v is None for v in values)
+    n = ds.length
+    out = DeviceBuffer(ctx, n)
+    validity = DeviceBuffer(ctx, (n + 7) // 8) if ds.validity is not None or has_null else None
+    ptrs = (C.c_char_p * max(len(vals), 1))(*vals)
+    lens = (C.c_int64 * max(len(vals), 1))(*[len(v) for v in vals])
+    col = ds.c()
+    _strings_check(lib.dfgpu_string_in_list(ctx.lib.dfgpu_ctx_stream(ctx.h), C.byref(col), ptrs, lens, len(vals), int(has_null), int(bool(negated)),
+                                            C.c_void_p(out.ptr), C.c_void_p(validity.ptr) if validity is not None else None))
+    return DeviceColumn(ctx, UINT8, n, out, validity, -1 if validity is not None else 0)
+
+
 def like_codes(ctx: Context, codes, code_match: DeviceColumn, n_codes: int) -> DeviceColumn:
     """the predicate over dictionary codes (dfgpu_like_codes): codes is an INT32 DeviceColumn / Column, code_match the UINT8 value of
-    each distinct string (like() over the dictionary values) -> a UINT8 DeviceColumn, NULL where the code is NULL"""
+    each distinct string (like(), string_compare() or string_in_list() over the dictionary values) -> a UINT8 DeviceColumn, NULL where
+    the code is NULL"""
     col = codes.c() if not isinstance(codes, Column) else codes
     lib = load_strings_library()
     n = int(col.length)

@@ -11,6 +11,7 @@
 #include <string>
 
 #include "../../include/dfgpu_strings.h"
+#include "strings.cuh"
 #include "tma.cuh"
 
 namespace dfgpu {
@@ -31,11 +32,9 @@ struct Program {
   uint32_t view_mask;
 };
 
-constexpr int kThreads = 256;
 constexpr int kTileRows = 512;                  // rows of one Utf8 tile (one block)
 constexpr int kStageBytes = 40 * 1024;          // shared-memory stage of one tile's bytes (512 TPC-H comments of up to 78 bytes fit)
 constexpr int kLongRow = 512;                   // longer rows are matched by a whole warp
-constexpr int kViewBufs = 240;                  // Utf8View data buffers one launch can reach (kernel parameters)
 
 __device__ __forceinline__ int cp_len(uint8_t b) { return b < 0x80 ? 1 : b < 0xE0 ? 2 : b < 0xF0 ? 3 : 4; }
 
@@ -127,20 +126,6 @@ __device__ bool match_row_warp(const Program& P, const uint8_t* s, int64_t n) {
   return true;
 }
 
-__device__ __forceinline__ bool bit(const uint8_t* bm, int64_t i) { return (bm[i >> 3] >> (i & 7)) & 1; }
-
-__device__ __forceinline__ void load_program(Program& dst, const Program& src) {
-  for (int i = threadIdx.x; i < (int)(sizeof(Program) / 4); i += blockDim.x)
-    reinterpret_cast<uint32_t*>(&dst)[i] = reinterpret_cast<const uint32_t*>(&src)[i];
-}
-
-// a warp's 32 consecutive rows [row0, row0 + 32) of validity -> out_valid bytes (row0 is a multiple of 32)
-__device__ __forceinline__ void store_validity(uint8_t* out_valid, int64_t row0, int64_t n, bool valid) {
-  const unsigned vb = __ballot_sync(0xffffffffu, valid);
-  const int lane = threadIdx.x & 31;
-  if (lane < 4 && row0 + lane * 8 < n) out_valid[(row0 >> 3) + lane] = (uint8_t)(vb >> (lane * 8));
-}
-
 // Utf8 / LargeUtf8: one block per tile of kTileRows rows.  The tile's rows are contiguous in the data buffer, so its byte range
 // [offsets[r0], offsets[r1]) is staged into shared memory when it fits: the 16-byte-aligned interior by one TMA bulk copy, the
 // unaligned head and tail bytes by the threads.  A tile that does not fit is matched from global memory.  Thread t of the block takes
@@ -202,11 +187,6 @@ __global__ void __launch_bounds__(kThreads) like_utf8_kernel(const __grid_consta
   }
 }
 
-struct ViewBufs {
-  const uint8_t* ptr[kViewBufs];
-  int32_t lo, count;   // this launch reaches buffers [lo, lo + count)
-};
-
 // Utf8View: one thread per row.  A string of at most 12 bytes is matched from its view; a longer one first against the view's 4-byte
 // prefix (an anchored-prefix mismatch is settled without reading its buffer), then from its data buffer.  With more data buffers than
 // one launch's parameters hold, launch g matches the rows whose buffer is in its range; launch 0 also writes every row no buffer
@@ -256,7 +236,7 @@ __global__ void __launch_bounds__(kThreads) like_view_kernel(const __grid_consta
   if (first && out_valid != nullptr) store_validity(out_valid, row0, n, valid);
 }
 
-// dictionary codes: out[i] = match[codes[i]]
+// dictionary codes: out[i] = match[codes[i]] (any predicate evaluated over the dictionary's distinct values)
 __global__ void __launch_bounds__(kThreads) like_codes_kernel(const int32_t* __restrict__ codes, const uint8_t* __restrict__ validity, int64_t in_off,
                                                               int64_t n, const uint8_t* __restrict__ match, int64_t n_codes,
                                                               uint8_t* __restrict__ out, uint8_t* __restrict__ out_valid) {
@@ -273,42 +253,13 @@ __global__ void __launch_bounds__(kThreads) like_codes_kernel(const int32_t* __r
 }
 
 // ---- host ----
-thread_local std::string g_error;
-
-int fail(int code, const std::string& msg) {
-  g_error = msg;
-  return code;
-}
-
-// length of the UTF-8 sequence at p[0 .. n), or 0 when it is not valid UTF-8 (overlong forms, surrogates, > U+10FFFF included)
-int utf8_seq(const uint8_t* p, int64_t n) {
-  const uint8_t b = p[0];
-  if (b < 0x80) return 1;
-  int len;
-  uint32_t cp;
-  if (b >= 0xC2 && b <= 0xDF) { len = 2; cp = b & 0x1F; }
-  else if (b >= 0xE0 && b <= 0xEF) { len = 3; cp = b & 0x0F; }
-  else if (b >= 0xF0 && b <= 0xF4) { len = 4; cp = b & 0x07; }
-  else return 0;
-  if (n < len) return 0;
-  for (int i = 1; i < len; ++i) {
-    if ((p[i] & 0xC0) != 0x80) return 0;
-    cp = (cp << 6) | (p[i] & 0x3F);
-  }
-  if ((len == 3 && (cp < 0x800 || (cp >= 0xD800 && cp <= 0xDFFF))) || (len == 4 && (cp < 0x10000 || cp > 0x10FFFF))) return 0;
-  return len;
-}
-
 int compile(const uint8_t* pat, int64_t len, int32_t flags, Program& P) {
   if (flags & ~(DFGPU_LIKE_NEGATED | DFGPU_LIKE_CASE_INSENSITIVE)) return fail(DFGPU_ERR_INVALID, "dfgpu_like: unknown flags");
   if (flags & DFGPU_LIKE_CASE_INSENSITIVE)
     return fail(DFGPU_ERR_UNSUPPORTED, "dfgpu_like: ILIKE (case-insensitive LIKE) is not supported on the GPU: it needs Unicode case folding");
   if (len < 0 || (len > 0 && pat == nullptr)) return fail(DFGPU_ERR_INVALID, "dfgpu_like: no pattern");
-  for (int64_t i = 0; i < len;) {
-    const int l = utf8_seq(pat + i, len - i);
-    if (l == 0) return fail(DFGPU_ERR_INVALID, "dfgpu_like: the pattern is not valid UTF-8 (byte " + std::to_string(i) + ")");
-    i += l;
-  }
+  const int64_t bad = utf8_invalid_at(pat, len);
+  if (bad >= 0) return fail(DFGPU_ERR_INVALID, "dfgpu_like: the pattern is not valid UTF-8 (byte " + std::to_string(bad) + ")");
   if (memchr(pat, '\\', (size_t)len) != nullptr)
     return fail(DFGPU_ERR_UNSUPPORTED, "dfgpu_like: a pattern with an escape character (\\) is not supported on the GPU");
   if (len > DFGPU_LIKE_MAX_PATTERN_BYTES)
@@ -353,12 +304,6 @@ int compile(const uint8_t* pat, int64_t len, int32_t flags, Program& P) {
   return DFGPU_OK;
 }
 
-int launched(const char* what) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return fail(DFGPU_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-  return DFGPU_OK;
-}
-
 }  // namespace like
 }  // namespace dfgpu
 
@@ -374,13 +319,11 @@ extern "C" int dfgpu_like(void* stream, const dfgpu_string_column* col, const ui
   if (rc != DFGPU_OK) return rc;
   if (col == nullptr || col->length < 0 || col->offset < 0) return fail(DFGPU_ERR_INVALID, "dfgpu_like: no column");
   if (col->length == 0) return DFGPU_OK;
-  if (out_values == nullptr || col->offsets_or_views == nullptr || (col->validity != nullptr && out_validity == nullptr))
-    return fail(DFGPU_ERR_INVALID, "dfgpu_like: missing buffer (a column with validity needs out_validity)");
+  if ((rc = check_column(col, out_values, out_validity, col->validity != nullptr, "dfgpu_like")) != DFGPU_OK) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   uint8_t* ov = col->validity != nullptr ? out_validity : nullptr;
   const int64_t n = col->length;
   if (col->layout == DFGPU_STRING_UTF8 || col->layout == DFGPU_STRING_LARGE_UTF8) {
-    if (col->n_data_buffers != 1 || col->data_buffers == nullptr) return fail(DFGPU_ERR_INVALID, "dfgpu_like: a Utf8 column has one data buffer");
     const unsigned grid = (unsigned)((n + kTileRows - 1) / kTileRows);
     if (col->layout == DFGPU_STRING_UTF8)
       like_utf8_kernel<int32_t><<<grid, kThreads, kStageBytes, st>>>(P, static_cast<const int32_t*>(col->offsets_or_views), col->data_buffers[0],
@@ -390,24 +333,11 @@ extern "C" int dfgpu_like(void* stream, const dfgpu_string_column* col, const ui
                                                                      col->validity, col->offset, n, out_values, ov);
     return launched("dfgpu_like");
   }
-  if (col->layout != DFGPU_STRING_UTF8_VIEW) return fail(DFGPU_ERR_INVALID, "dfgpu_like: unknown string layout");
-  if (reinterpret_cast<uintptr_t>(col->offsets_or_views) & 15) return fail(DFGPU_ERR_INVALID, "dfgpu_like: Utf8View views must be 16-byte aligned");
-  if (col->n_data_buffers < 0 || (col->n_data_buffers > 0 && col->data_buffers == nullptr))
-    return fail(DFGPU_ERR_INVALID, "dfgpu_like: Utf8View data buffers missing");
   const unsigned grid = (unsigned)((n + kThreads - 1) / kThreads);
-  int lo = 0;
-  do {
-    ViewBufs vb;
-    memset(&vb, 0, sizeof(vb));
-    vb.lo = lo;
-    vb.count = col->n_data_buffers - lo < kViewBufs ? col->n_data_buffers - lo : kViewBufs;
-    for (int i = 0; i < vb.count; ++i) vb.ptr[i] = col->data_buffers[lo + i];
+  return for_each_view_range(col, "dfgpu_like", [&](const ViewBufs& vb) {
     like_view_kernel<<<grid, kThreads, 0, st>>>(P, vb, static_cast<const uint4*>(col->offsets_or_views), col->validity, col->offset, n,
                                                 out_values, ov);
-    if ((rc = launched("dfgpu_like")) != DFGPU_OK) return rc;
-    lo += kViewBufs;
-  } while (lo < col->n_data_buffers);
-  return DFGPU_OK;
+  });
 }
 
 extern "C" int dfgpu_like_codes(void* stream, const dfgpu_column* codes, const uint8_t* code_match, int64_t n_codes, uint8_t* out_values,

@@ -96,11 +96,12 @@ class Column(Expr):
 
 
 class Literal(Expr):
-    """expressions/literal.rs:106; value None = NULL of the given type"""
+    """expressions/literal.rs:106; value None = NULL of the given type.  A str value is a Utf8 literal."""
 
     def __init__(self, value, type: Optional[pa.DataType] = None):
         if type is None:
-            type = pa.bool_() if isinstance(value, bool) else pa.int64() if isinstance(value, int) else pa.float64()
+            type = (pa.bool_() if isinstance(value, bool) else pa.int64() if isinstance(value, int) else pa.string() if isinstance(value, str)
+                    else pa.float64())
         self.value, self.type = value, type
 
     def data_type(self, schema): return self.type
@@ -211,6 +212,23 @@ class LikeExpr(Expr):
     def rpn(self, schema, out):
         raise NotImplementedError("This feature is not implemented: LikeExpr has no GPU expression program (plan_like_predicates turns a LIKE "
                                   "on a string column with a literal pattern into a mask column)")
+
+
+class InListExpr(Expr):
+    """expressions/in_list.rs: `expr [NOT] IN (list)` with a static list, SQL's three-valued IN: NULL when expr is NULL, or when expr is
+    found nowhere and the list holds a NULL.  Boolean.  It has no expression program of its own: plan_string_predicates computes an IN
+    list of Utf8 literals over a string column as a UINT8 mask column (GpuLikeExec, libdfgpu_strings.so) and compares `mask = 1`.  A str
+    or None item is a Utf8 literal."""
+
+    def __init__(self, expr: Expr, list: Sequence[Union[Expr, str, None]], negated: bool = False):
+        self.expr, self.negated = expr, negated
+        self.list = [v if isinstance(v, Expr) else Literal(v, pa.string()) for v in list]
+
+    def data_type(self, schema): return pa.bool_()
+
+    def rpn(self, schema, out):
+        raise NotImplementedError("This feature is not implemented: InListExpr has no GPU expression program (plan_string_predicates turns an "
+                                  "IN list of Utf8 literals over a string column into a mask column)")
 
 
 def col(name: str) -> Column: return Column(name)
@@ -362,10 +380,17 @@ class DictionaryDecodeExec(ExecutionPlan):
             yield pa.RecordBatch.from_arrays(cols, schema=self.schema)
 
 
+def _mask_column(e: Expr) -> Column:
+    """the string column a mask predicate of GpuLikeExec reads"""
+    return e.left if isinstance(e, BinaryExpr) else e.expr
+
+
 class GpuLikeExec(ExecutionPlan):
-    """LikeExpr over string columns -> one UINT8 mask column per LIKE (`name`, appended; NULL where the string is NULL), and the input
-    without the columns `drop`.  A Utf8 / LargeUtf8 / Utf8View column runs dfgpu_like; an INT32 column of DictionaryEncodeExec codes
-    (`dictionary_of` given) matches the dictionary's distinct values with dfgpu_like, then maps each row's code with dfgpu_like_codes."""
+    """String predicates over string columns -> one UINT8 mask column per predicate (`name`, appended; NULL where the predicate is NULL),
+    and the input without the columns `drop`.  A predicate is a LikeExpr, a BinaryExpr(Column, comparison, Utf8 Literal) or an
+    InListExpr(Column, Utf8 Literals); `likes` holds (predicate, mask name).  A Utf8 / LargeUtf8 / Utf8View column runs dfgpu_like,
+    dfgpu_string_compare or dfgpu_string_in_list; an INT32 column of DictionaryEncodeExec codes (`dictionary_of` given) evaluates the
+    predicate over the dictionary's distinct values, then maps each row's code with dfgpu_like_codes."""
 
     def __init__(self, input: ExecutionPlan, likes: Sequence[Tuple[LikeExpr, str]], drop: Sequence[str] = (), dictionary_of: Optional["callable"] = None):
         self.input, self.likes, self.drop, self.dictionary_of = input, list(likes), set(drop), dictionary_of
@@ -373,17 +398,25 @@ class GpuLikeExec(ExecutionPlan):
 
     def children(self): return [self.input]
 
-    def _mask(self, ctx: TaskContext, arr: pa.Array, e: LikeExpr) -> pa.Array:
+    @staticmethod
+    def _predicate(ctx: TaskContext, strings, e: Expr) -> "D.DeviceColumn":
+        if isinstance(e, LikeExpr):
+            return D.like(ctx.gpu, strings, e.pattern.value, e.negated)
+        if isinstance(e, BinaryExpr):
+            return D.string_compare(ctx.gpu, strings, _STRING_CMP[e.op], e.right.value)
+        return D.string_in_list(ctx.gpu, strings, [v.value for v in e.list], e.negated)
+
+    def _mask(self, ctx: TaskContext, arr: pa.Array, e: Expr) -> pa.Array:
         import numpy as np
         if isinstance(arr, pa.ChunkedArray):
             arr = arr.combine_chunks()
         if _is_string_like(arr.type):
-            m = D.like(ctx.gpu, arr, e.pattern.value, e.negated)
+            m = self._predicate(ctx, arr, e)
         else:                                              # INT32 codes of DictionaryEncodeExec
             dic = self.dictionary_of(ctx).dic
             n = dic.size()
             values = pa.array([dic.value(i) for i in range(n)], pa.binary()).cast(pa.string())
-            code_match = D.like(ctx.gpu, values, e.pattern.value, e.negated)
+            code_match = self._predicate(ctx, values, e)
             codes = D.DeviceColumn.from_host(ctx.gpu, D.HostColumn(np.asarray(arr.fill_null(0)), None if arr.null_count == 0 else np.asarray(arr.is_valid())))
             m = D.like_codes(ctx.gpu, codes, code_match, n)
         v, valid = D.device_column_numpy(m)
@@ -392,7 +425,7 @@ class GpuLikeExec(ExecutionPlan):
     def execute(self, ctx):
         isch = self.input.schema
         for rb in self.input.execute(ctx):
-            masks = [self._mask(ctx, rb.column(isch.get_field_index(e.expr.name)), e) for e, _ in self.likes]
+            masks = [self._mask(ctx, rb.column(isch.get_field_index(_mask_column(e).name)), e) for e, _ in self.likes]
             cols = [rb.column(i) for i, f in enumerate(isch) if f.name not in self.drop]
             yield pa.RecordBatch.from_arrays(cols + masks, schema=self.schema)
 
@@ -814,6 +847,8 @@ def _expr_names(e: Expr) -> set:
         return _expr_names(e.arg)
     if isinstance(e, LikeExpr):
         return _expr_names(e.expr) | _expr_names(e.pattern)
+    if isinstance(e, InListExpr):
+        return _expr_names(e.expr).union(*[_expr_names(v) for v in e.list])
     return set()
 
 
@@ -1540,40 +1575,115 @@ def fuse_full_joins(plan: ExecutionPlan) -> ExecutionPlan:
 
 
 # ---------------------------------------------------------------------------------------------
-# LIKE predicates — a mask column computed ahead of the filter (libdfgpu_strings.so)
+# string predicates — a mask column computed ahead of the filter (libdfgpu_strings.so)
 # ---------------------------------------------------------------------------------------------
+_STRING_CMP = {D.OP_EQ: "=", D.OP_NEQ: "<>", D.OP_LT: "<", D.OP_LTEQ: "<=", D.OP_GT: ">", D.OP_GTEQ: ">="}
+_MIRRORED = {D.OP_EQ: D.OP_EQ, D.OP_NEQ: D.OP_NEQ, D.OP_LT: D.OP_GT, D.OP_LTEQ: D.OP_GTEQ, D.OP_GT: D.OP_LT, D.OP_GTEQ: D.OP_LTEQ}
+
+
+def _string_column(e: Expr, schema: pa.Schema, coded: set) -> bool:
+    """a Utf8, LargeUtf8 or Utf8View column of schema (not a raw Arrow dictionary), or a column DictionaryEncodeExec coded (`coded`)"""
+    if not isinstance(e, Column):
+        return False
+    ix = schema.get_field_index(e.name)
+    return ix >= 0 and (e.name in coded or (_is_string_like(schema.field(ix).type) and not pa.types.is_dictionary(schema.field(ix).type)))
+
+
+def _utf8_literal(e: Expr) -> bool:
+    """a Utf8 literal: a str or NULL of a string type whose text encodes as UTF-8"""
+    if not isinstance(e, Literal) or not _is_string_like(e.type) or pa.types.is_dictionary(e.type):
+        return False
+    if e.value is None:
+        return True
+    try:
+        return isinstance(e.value, str) and e.value.encode("utf-8") is not None
+    except UnicodeEncodeError:
+        return False
+
+
 def _like_on_gpu(e: LikeExpr, schema: pa.Schema, coded: set) -> bool:
     """LIKE / NOT LIKE of a Utf8, LargeUtf8 or Utf8View column (or one DictionaryEncodeExec coded: `coded`) with a Utf8 literal pattern
     without `\\`; a NULL pattern too (the predicate folds to NULL)"""
-    if e.case_insensitive or not isinstance(e.expr, Column) or not isinstance(e.pattern, Literal):
+    if e.case_insensitive or not isinstance(e.pattern, Literal):
         return False
     p = e.pattern.value
     if p is not None and (not isinstance(p, str) or "\\" in p):
         return False
-    ix = schema.get_field_index(e.expr.name)
-    return ix >= 0 and (e.expr.name in coded or (_is_string_like(schema.field(ix).type) and not pa.types.is_dictionary(schema.field(ix).type)))
+    return _string_column(e.expr, schema, coded)
 
 
-def _rewrite_likes(e: Expr, schema: pa.Schema, coded: set, taken: set, likes: list) -> Optional[Expr]:
-    """e with every LIKE that runs on the GPU replaced by `mask = 1` (appended to likes as (LikeExpr, mask name)); None when a LIKE that
-    cannot run there remains"""
+def _string_comparison(e: BinaryExpr, schema: pa.Schema, coded: set) -> Optional[BinaryExpr]:
+    """a comparison of a string column with a Utf8 literal as BinaryExpr(column, op, literal), a literal on the left swapped to the right
+    with its operator mirrored; None when e is not one or the literal is longer than the library takes"""
+    l, op, r = e.left, e.op, e.right
+    if isinstance(l, Literal) and not isinstance(r, Literal):
+        l, op, r = r, _MIRRORED[op], l
+    if not (_string_column(l, schema, coded) and _utf8_literal(r)):
+        return None
+    if r.value is not None and len(r.value.encode("utf-8")) > D.STRING_MAX_LITERAL_BYTES:
+        return None
+    return e if l is e.left else BinaryExpr(l, op, r)
+
+
+def _in_list_on_gpu(e: InListExpr, schema: pa.Schema, coded: set) -> bool:
+    """an IN list of Utf8 literals and NULLs over a string column, within the library's caps on distinct values and their bytes"""
+    if not _string_column(e.expr, schema, coded) or not all(_utf8_literal(v) for v in e.list):
+        return False
+    vals = {v.value.encode("utf-8") for v in e.list if v.value is not None}
+    return len(vals) <= D.STRING_IN_MAX_VALUES and sum(len(v) for v in vals) <= D.STRING_IN_MAX_BYTES
+
+
+def _string_operand(e: Expr, schema: pa.Schema) -> bool:
+    """a column of a string type, or a literal of one: a comparison reading it must become a mask or stay off the GPU"""
+    if isinstance(e, Column):
+        ix = schema.get_field_index(e.name)
+        return ix >= 0 and _is_string_like(schema.field(ix).type)
+    return isinstance(e, Literal) and _is_string_like(e.type)
+
+
+def _mask_eq(e: Expr, prefix: str, taken: set, likes: list) -> Expr:
+    """`mask = 1` for a new mask column computing e (appended to likes as (e, mask name))"""
+    name = f"{prefix}_{len(likes)}"
+    while name in taken:
+        name = "_" + name
+    taken.add(name)
+    likes.append((e, name))
+    return BinaryExpr(Column(name), D.OP_EQ, Literal(1, pa.uint8()))
+
+
+def _rewrite_likes(e: Expr, schema: pa.Schema, coded: set, taken: set, likes: list, strings: bool = False) -> Optional[Expr]:
+    """e with every LIKE that runs on the GPU replaced by `mask = 1` (appended to likes as (predicate, mask name)); None when a LIKE that
+    cannot run there remains.  With `strings`, also every comparison of a string column with a Utf8 literal and every IN list of Utf8
+    literals over a string column; None when a comparison reading a string, or an IN list, that cannot run there remains."""
     if isinstance(e, LikeExpr):
         if not _like_on_gpu(e, schema, coded):
             return None
         if e.pattern.value is None:
             return Literal(None, pa.bool_())
-        name = f"__like_{len(likes)}"
-        while name in taken:
-            name = "_" + name
-        taken.add(name)
-        likes.append((e, name))
-        return BinaryExpr(Column(name), D.OP_EQ, Literal(1, pa.uint8()))
+        return _mask_eq(e, "__like", taken, likes)
+    if strings and isinstance(e, InListExpr):
+        if not _in_list_on_gpu(e, schema, coded):
+            return None
+        vals = [v for v in e.list if v.value is not None]
+        pred = _mask_eq(InListExpr(e.expr, vals, e.negated), "__in", taken, likes)
+        if len(vals) == len(e.list):
+            return pred
+        # a NULL in the list: a string found nowhere gives NULL.  Kleene logic adds it to the mask of the non-NULL values: IN is
+        # `found OR NULL`, NOT IN is `not found AND NULL`.  So the mask stays a plain map of each distinct string (dictionary codes too).
+        return BinaryExpr(pred, D.OP_AND if e.negated else D.OP_OR, Literal(None, pa.bool_()))
+    if strings and isinstance(e, BinaryExpr) and e.op in _STRING_CMP and (_string_operand(e.left, schema) or _string_operand(e.right, schema)):
+        c = _string_comparison(e, schema, coded)
+        if c is None:
+            return None
+        if c.right.value is None:
+            return Literal(None, pa.bool_())
+        return _mask_eq(c, "__cmp", taken, likes)
     if isinstance(e, BinaryExpr):
-        l = _rewrite_likes(e.left, schema, coded, taken, likes)
-        r = None if l is None else _rewrite_likes(e.right, schema, coded, taken, likes)
+        l = _rewrite_likes(e.left, schema, coded, taken, likes, strings)
+        r = None if l is None else _rewrite_likes(e.right, schema, coded, taken, likes, strings)
         return None if r is None else (e if (l is e.left and r is e.right) else BinaryExpr(l, e.op, r))
     if isinstance(e, (UnaryExpr, CastExpr)):
-        a = _rewrite_likes(e.arg, schema, coded, taken, likes)
+        a = _rewrite_likes(e.arg, schema, coded, taken, likes, strings)
         if a is None:
             return None
         if a is e.arg:
@@ -1602,6 +1712,27 @@ def _with_children(plan: ExecutionPlan, fn) -> ExecutionPlan:
     return out
 
 
+def _plan_masks(plan: ExecutionPlan, strings: bool) -> ExecutionPlan:
+    plan = _with_children(plan, lambda p: _plan_masks(p, strings))
+    if not isinstance(plan, GpuFilterExec):
+        return plan
+    inner = plan.input
+    isch = inner.schema
+    coded = {isch.field(i).name for i in inner.string_cols} if isinstance(inner, DictionaryEncodeExec) else set()
+    likes: list = []
+    pred = _rewrite_likes(plan.predicate, isch, coded, set(isch.names), likes, strings)
+    if pred is None or pred is plan.predicate:
+        return plan
+    out_names = [f.name for f in plan.schema]
+    raw = {_mask_column(e).name for e, _ in likes if _mask_column(e).name not in coded}
+    if raw & set(out_names):
+        return plan                                       # a string column read above the filter
+    drop = raw - _expr_names(pred)
+    below = GpuLikeExec(inner, likes, drop, inner.dictionary_of if coded else None) if likes else inner
+    projection = [below.schema.get_field_index(n) for n in out_names]
+    return GpuFilterExec(pred, below, projection, plan.fetch)
+
+
 def plan_like_predicates(plan: ExecutionPlan) -> ExecutionPlan:
     """PhysicalOptimizerRule twin (INTEGRATION.md §2c), ahead of the fusion rules: every FilterExec whose predicate holds LikeExpr(column,
     Utf8 literal) over a Utf8, LargeUtf8 or Utf8View column, or over a column DictionaryEncodeExec coded, gets a GpuLikeExec under it that
@@ -1610,24 +1741,20 @@ def plan_like_predicates(plan: ExecutionPlan) -> ExecutionPlan:
     predicate holds any other LIKE (ILIKE, a column pattern, a `\\` in the pattern) or when a Utf8 column a LIKE reads is also read
     above the filter.  A NULL literal pattern folds to a NULL predicate.  The fusion rules then treat the GpuLikeExec as the pipeline's
     source, as they treat any other node under a filter."""
-    plan = _with_children(plan, plan_like_predicates)
-    if not isinstance(plan, GpuFilterExec):
-        return plan
-    inner = plan.input
-    isch = inner.schema
-    coded = {isch.field(i).name for i in inner.string_cols} if isinstance(inner, DictionaryEncodeExec) else set()
-    likes: list = []
-    pred = _rewrite_likes(plan.predicate, isch, coded, set(isch.names), likes)
-    if pred is None or pred is plan.predicate:
-        return plan
-    out_names = [f.name for f in plan.schema]
-    raw = {e.expr.name for e, _ in likes if e.expr.name not in coded}
-    if raw & set(out_names):
-        return plan                                       # a string column read above the filter
-    drop = raw - _expr_names(pred)
-    below = GpuLikeExec(inner, likes, drop, inner.dictionary_of if coded else None) if likes else inner
-    projection = [below.schema.get_field_index(n) for n in out_names]
-    return GpuFilterExec(pred, below, projection, plan.fetch)
+    return _plan_masks(plan, strings=False)
+
+
+def plan_string_predicates(plan: ExecutionPlan) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §3b), ahead of the fusion rules, in place of plan_like_predicates: everything that rule
+    rewrites, and also, over the same string columns (Utf8, LargeUtf8, Utf8View, or coded by DictionaryEncodeExec):
+      - BinaryExpr(column, =, <>, <, <=, >, >=, Utf8 literal), a literal on the left swapped to the right with its operator mirrored;
+        a NULL literal folds to a NULL predicate;
+      - InListExpr(column, Utf8 literals and NULLs), [NOT] IN, within the library's caps (64 distinct values, 1024 bytes); a NULL in the
+        list becomes `mask OR NULL` (IN) / `mask AND NULL` (NOT IN) over the mask of the non-NULL values.
+    Each becomes a GpuLikeExec mask and `mask = 1`, and the filter keeps its schema.  A filter stays as it was when its predicate holds a
+    string predicate that cannot run on the GPU (a column compared with a column, an IN list of anything but Utf8 literals or over the
+    caps, a LIKE plan_like_predicates leaves), or when a raw string column a predicate reads is also read above the filter."""
+    return _plan_masks(plan, strings=True)
 
 
 def collect(plan: ExecutionPlan, ctx: Optional[TaskContext] = None) -> List[pa.RecordBatch]:

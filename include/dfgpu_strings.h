@@ -1,7 +1,9 @@
 /*
  * dfgpu_strings.h — C ABI of libdfgpu_strings.so: string predicates on the H100 (sm_90a) that turn a string column into a one-byte
  * mask column, for DataFusion's `LikeExpr` (reference datafusion/physical-expr/src/expressions/like.rs, whose `evaluate` calls
- * arrow-string's `like` / `nlike` kernels, arrow-string/src/like.rs).
+ * arrow-string's `like` / `nlike` kernels, arrow-string/src/like.rs), for a `BinaryExpr` comparing a string column with a Utf8 literal
+ * (expressions/binary.rs -> arrow-ord's `eq` / `neq` / `lt` / `lt_eq` / `gt` / `gt_eq`, arrow-ord/src/cmp.rs) and for an `InListExpr`
+ * of a string column over a static list of Utf8 literals (expressions/in_list.rs).
  *
  * The library stands apart from libdfgpu.so and does not link it: it includes dfgpu.h only for `dfgpu_column` and the status codes.
  * Every call enqueues its kernels on the caller's CUDA stream (a libdfgpu ctx's `dfgpu_ctx_stream(ctx)`) and returns; it makes no
@@ -21,6 +23,29 @@
  *   - a pattern longer than DFGPU_LIKE_MAX_PATTERN_BYTES bytes, or with more than DFGPU_LIKE_MAX_SEGMENTS non-empty `%`-separated pieces.
  * Rejected with DFGPU_ERR_INVALID: a pattern that is not valid UTF-8, and malformed arguments.
  * A column pattern (`a LIKE b`) and a custom ESCAPE never reach the library: the planner leaves them on the CPU.
+ *
+ * Semantics of `s op literal` (dfgpu_string_compare), op one of =, <>, <, <=, >, >=:
+ *   - Arrow's order for strings: byte-wise lexicographic over the UTF-8 bytes (which is code-point order), a proper prefix sorts first;
+ *     equal means equal length and equal bytes.  No collation, no case folding, no trimming.
+ *   - a NULL string gives NULL; on a non-NULL string the result is in {0, 1}.
+ * Semantics of `s [NOT] IN (v1, v2, ...)` (dfgpu_string_in_list), SQL's three-valued IN as InListExpr evaluates a static list:
+ *   - a NULL string gives NULL;
+ *   - a string equal to some vi gives 1 for IN and 0 for NOT IN;
+ *   - a string equal to none gives NULL when the list holds a NULL (list_has_null), else 0 for IN and 1 for NOT IN.
+ *   So a non-NULL string can give NULL.
+ * Refused with DFGPU_ERR_UNSUPPORTED (the caller keeps the CPU expression): a comparison literal longer than
+ * DFGPU_STRING_MAX_LITERAL_BYTES; a list of more than DFGPU_STRING_IN_MAX_VALUES distinct values or more than DFGPU_STRING_IN_MAX_BYTES
+ * bytes of them; a list holding a NULL over a Utf8View column of more than 240 data buffers (pass the list without its NULL and add the
+ * NULL by Kleene logic: IN is `mask OR NULL`, NOT IN is `mask AND NULL`).  Rejected with DFGPU_ERR_INVALID: a literal or list value
+ * that is not valid UTF-8, an unknown op, malformed arguments.
+ * A column compared with a column never reaches the library.
+ *
+ * How rows are settled, cheapest bytes first: a Utf8 / LargeUtf8 row's length comes from its two offsets, so `=` / `<>` against a literal
+ * of another length, and an IN row whose length is no value's length, read no string bytes; an ordering comparison stops at the first
+ * byte that differs.  A Utf8View row is settled from its 16-byte view (the length, the 4-byte prefix, the whole string when it is 12
+ * bytes or shorter); its data buffer is read only for a longer string the view leaves open.  An IN row is looked up by a hash of its
+ * bytes in a table of the values, and only the values in its probe sequence are compared byte for byte.
+ * Dictionary codes: evaluate the predicate over the dictionary's distinct values, then map each row's code with dfgpu_like_codes.
  */
 #ifndef DFGPU_STRINGS_H
 #define DFGPU_STRINGS_H
@@ -41,6 +66,18 @@ enum dfgpu_string_layout {
 #define DFGPU_LIKE_CASE_INSENSITIVE 2   /* ILIKE: always DFGPU_ERR_UNSUPPORTED */
 #define DFGPU_LIKE_MAX_PATTERN_BYTES 256
 #define DFGPU_LIKE_MAX_SEGMENTS 16
+
+enum dfgpu_string_cmp_op {
+  DFGPU_STRING_EQ = 0, /* =  */
+  DFGPU_STRING_NE = 1, /* <> */
+  DFGPU_STRING_LT = 2, /* <  */
+  DFGPU_STRING_LE = 3, /* <= */
+  DFGPU_STRING_GT = 4, /* >  */
+  DFGPU_STRING_GE = 5  /* >= */
+};
+#define DFGPU_STRING_MAX_LITERAL_BYTES 256   /* longest comparison literal */
+#define DFGPU_STRING_IN_MAX_VALUES 64        /* most distinct non-NULL values of an IN list */
+#define DFGPU_STRING_IN_MAX_BYTES 1024       /* most bytes of those values together */
 
 /* One Arrow string array resident in HBM.  The kernels read only [data + offsets[offset], data + offsets[offset + length]) of a Utf8 /
  * LargeUtf8 array, and of a Utf8View array only the views of rows [offset, offset + length) and the bytes those views point at, so
@@ -63,10 +100,23 @@ typedef struct dfgpu_string_column {
 int dfgpu_like(void* stream, const dfgpu_string_column* col, const uint8_t* pattern, int64_t pattern_len, int32_t flags,
                uint8_t* out_values, uint8_t* out_validity);
 
-/* The same predicate over dictionary codes (an INT32 dfgpu_column of codes into one dictionary, e.g. dfgpu_dictionary_remap's output):
- * code_match[0 .. n_codes) holds the predicate's value for each distinct value (dfgpu_like over the dictionary values, NOT LIKE
- * already applied).  out_values[i] = code_match[codes[i]]; a NULL code gives NULL (out_validity as in dfgpu_like); a code outside
- * [0, n_codes) gives 0. */
+/* `col op literal` (BinaryExpr with a scalar Utf8 right operand).  op: enum dfgpu_string_cmp_op.  literal: literal_len bytes of UTF-8
+ * (no terminator needed).  Outputs as in dfgpu_like. */
+int dfgpu_string_compare(void* stream, const dfgpu_string_column* col, int32_t op, const uint8_t* literal, int64_t literal_len,
+                         uint8_t* out_values, uint8_t* out_validity);
+
+/* `col [NOT] IN (values)` (InListExpr with a static list).  values: a HOST array of n_values HOST pointers to the non-NULL values, each
+ * value_lens[i] bytes of UTF-8 (duplicates allowed); list_has_null: the list also holds a NULL; negated: NOT IN.  Writes out_values[0 ..
+ * length) in {0, 1} (0 under NULL results).  out_validity (at least (length + 7) / 8 bytes) receives each result's validity rebased to
+ * bit 0; it is written when col->validity is set or list_has_null is, and may be NULL otherwise. */
+int dfgpu_string_in_list(void* stream, const dfgpu_string_column* col, const uint8_t* const* values, const int64_t* value_lens,
+                         int64_t n_values, int32_t list_has_null, int32_t negated, uint8_t* out_values, uint8_t* out_validity);
+
+/* Any of these predicates over dictionary codes (an INT32 dfgpu_column of codes into one dictionary, e.g. dfgpu_dictionary_remap's
+ * output): code_match[0 .. n_codes) holds the predicate's value for each distinct value (dfgpu_like, dfgpu_string_compare or
+ * dfgpu_string_in_list over the dictionary values, any negation already applied).  out_values[i] = code_match[codes[i]]; a NULL code
+ * gives NULL (out_validity as in dfgpu_like); a code outside [0, n_codes) gives 0.  The map carries values only: a predicate that can
+ * be NULL on a non-NULL value (an IN list holding a NULL) is mapped for its non-NULL values and combined with the NULL by the caller. */
 int dfgpu_like_codes(void* stream, const dfgpu_column* codes, const uint8_t* code_match, int64_t n_codes, uint8_t* out_values,
                      uint8_t* out_validity);
 
