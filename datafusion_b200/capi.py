@@ -1039,9 +1039,11 @@ LIKE_MAX_PATTERN_BYTES, LIKE_MAX_SEGMENTS = 256, 16
 STRING_EQ, STRING_NE, STRING_LT, STRING_LE, STRING_GT, STRING_GE = range(6)
 STRING_CMP_OPS = {"=": STRING_EQ, "<>": STRING_NE, "!=": STRING_NE, "<": STRING_LT, "<=": STRING_LE, ">": STRING_GT, ">=": STRING_GE}
 STRING_MAX_LITERAL_BYTES, STRING_IN_MAX_VALUES, STRING_IN_MAX_BYTES = 256, 64, 1024
+ERR_INVALID = -1   # DFGPU_ERR_INVALID
 
 # every symbol include/dfgpu_strings.h declares
-STRINGS_EXPORTS = ["dfgpu_like", "dfgpu_like_codes", "dfgpu_string_compare", "dfgpu_string_in_list", "dfgpu_strings_last_error"]
+STRINGS_EXPORTS = ["dfgpu_like", "dfgpu_like_codes", "dfgpu_string_compare", "dfgpu_string_in_list", "dfgpu_string_take_data",
+                   "dfgpu_string_take_offsets", "dfgpu_string_take_scratch_bytes", "dfgpu_string_take_views", "dfgpu_strings_last_error"]
 
 
 class StringColumn(C.Structure):
@@ -1071,6 +1073,14 @@ def load_strings_library() -> C.CDLL:
     lib.dfgpu_string_in_list.restype = C.c_int
     lib.dfgpu_string_in_list.argtypes = [vp, C.POINTER(StringColumn), C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.c_int64, C.c_int32,
                                          C.c_int32, vp, vp]
+    lib.dfgpu_string_take_scratch_bytes.restype = C.c_int64
+    lib.dfgpu_string_take_scratch_bytes.argtypes = [C.c_int64]
+    lib.dfgpu_string_take_offsets.restype = C.c_int
+    lib.dfgpu_string_take_offsets.argtypes = [vp, C.POINTER(StringColumn), C.c_int32, C.POINTER(Column), vp, vp, vp]
+    lib.dfgpu_string_take_data.restype = C.c_int
+    lib.dfgpu_string_take_data.argtypes = [vp, C.c_int32, C.c_int64, C.c_int64, vp, vp, vp, vp]
+    lib.dfgpu_string_take_views.restype = C.c_int
+    lib.dfgpu_string_take_views.argtypes = [vp, C.POINTER(StringColumn), C.c_int32, C.POINTER(Column), vp, vp, vp]
     lib.dfgpu_strings_last_error.restype = C.c_char_p
     lib.dfgpu_strings_last_error.argtypes = []
     _strings_lib = lib
@@ -1109,7 +1119,13 @@ class DeviceStrings:
         self.index = up(bufs[1], nel * width)                  # offsets or views of rows [0, offset + length)
         self.validity = up(bufs[0]) if bufs[0] is not None and arr.null_count > 0 else None
         self.data = [up(b) for b in bufs[2:]]
+        self.host_data = list(bufs[2:])     # the host data buffers, which string_take's Utf8View output reuses
         self._ptrs = (C.c_void_p * max(len(self.data), 1))(*[d.ptr for d in self.data])
+
+    @property
+    def nbytes(self) -> int:
+        """device bytes this array holds"""
+        return sum(b.nbytes for b in [self.index] + self.data + ([self.validity] if self.validity is not None else []))
 
     def c(self) -> StringColumn:
         s = StringColumn()
@@ -1186,6 +1202,97 @@ def like_codes(ctx: Context, codes, code_match: DeviceColumn, n_codes: int) -> D
     _strings_check(lib.dfgpu_like_codes(ctx.lib.dfgpu_ctx_stream(ctx.h), C.byref(col), C.c_void_p(code_match.values.ptr), int(n_codes),
                                         C.c_void_p(values.ptr), C.c_void_p(validity.ptr) if validity is not None else None))
     return DeviceColumn(ctx, UINT8, n, values, validity, int(col.null_count) if validity is not None else 0)
+
+
+class TakenStrings:
+    """string_take's output: a string array of the sources' layout resident in HBM.  index: the offsets (Utf8 int32, LargeUtf8 int64)
+    or the views; data: the one data buffer of a Utf8 / LargeUtf8 array, or the Utf8View output's buffer list (the sources' buffers)."""
+
+    def __init__(self, ctx: Context, layout: int, length: int, null_count: int, index: DeviceBuffer, validity: DeviceBuffer, data, host_data,
+                 keep=()):
+        self.ctx, self.layout, self.length, self.null_count = ctx, layout, length, null_count
+        self.index, self.validity, self.data, self._host_data = index, validity, data, host_data
+        self._keep = keep     # the device buffers the enqueued gather still reads (sources, ids, scratch)
+
+    def to_arrow(self):
+        """the pyarrow array of the sources' type.  Utf8View copies back the views only and reuses the sources' host data buffers."""
+        import pyarrow as pa
+        n = self.length
+        t = {STRING_UTF8: pa.string(), STRING_LARGE_UTF8: pa.large_string(), STRING_UTF8_VIEW: pa.string_view()}[self.layout]
+        validity = pa.py_buffer(self.validity.to_numpy(np.uint8)[:(n + 7) // 8]) if self.null_count and n else None
+        if self.layout == STRING_UTF8_VIEW:
+            views = pa.py_buffer(self.index.to_numpy(np.uint8)[:n * 16])
+            return pa.Array.from_buffers(t, n, [validity, views] + list(self._host_data), null_count=self.null_count)
+        w = 4 if self.layout == STRING_UTF8 else 8
+        offsets = pa.py_buffer(self.index.to_numpy(np.uint8)[:(n + 1) * w])
+        return pa.Array.from_buffers(t, n, [validity, offsets, pa.py_buffer(self.data.to_numpy(np.uint8)[:self.data.nbytes])],
+                                     null_count=self.null_count)
+
+
+def _ids_column(ctx: Context, ids):
+    """ids -> (dfgpu Column, owner): a DeviceColumn / Column as it is; a pyarrow uint32 / int64 array or numpy array uploaded"""
+    if isinstance(ids, Column):
+        return ids, None
+    if isinstance(ids, DeviceColumn):
+        return ids.c(), ids
+    import pyarrow as pa
+    if isinstance(ids, (pa.Array, pa.ChunkedArray)):
+        if isinstance(ids, pa.ChunkedArray):
+            ids = ids.combine_chunks()
+        if not (pa.types.is_uint32(ids.type) or pa.types.is_int64(ids.type)):
+            raise TypeError(f"string ids are uint32 or int64, not {ids.type}")
+        valid = None if ids.null_count == 0 else np.asarray(ids.is_valid())
+        hc = HostColumn(np.asarray(ids.fill_null(0)), valid)
+    else:
+        hc = HostColumn(np.asarray(ids))
+    if hc.type not in (UINT32, INT64):
+        raise TypeError("string ids are uint32 or int64")
+    dc = DeviceColumn.from_host(ctx, hc)
+    return dc.c(), dc
+
+
+def string_take(ctx: Context, sources, ids) -> TakenStrings:
+    """arrow-select's `take` over string arrays on the GPU (dfgpu_string_take_*): output row i is the string the id names.
+    sources: DeviceStrings or pyarrow string / large_string / string_view arrays, all of one type; ids: UINT32 rows of sources[0], or
+    INT64 ids packed as source << 32 | row (DeviceColumn, Column, pyarrow or numpy array).  A NULL id gives NULL.  DfgpuError
+    (DFGPU_ERR_INVALID) for an id outside its source, and for a Utf8 output beyond 2^31 - 1 bytes ("offset overflow")."""
+    srcs = [s if isinstance(s, DeviceStrings) else DeviceStrings(ctx, s) for s in sources]
+    if not srcs:
+        raise ValueError("string_take needs a source")
+    layout = srcs[0].layout
+    if any(s.layout != layout for s in srcs):
+        raise TypeError("string_take: the sources differ in type")
+    cols = (StringColumn * len(srcs))(*[s.c() for s in srcs])
+    idc, owner = _ids_column(ctx, ids)
+    lib = load_strings_library()
+    stream = ctx.lib.dfgpu_ctx_stream(ctx.h)
+    n = int(idc.length)
+    if layout == STRING_UTF8_VIEW:
+        views = DeviceBuffer(ctx, n * 16)
+        validity = DeviceBuffer(ctx, (n + 31) // 32 * 4)
+        status = DeviceBuffer(ctx, 16)
+        _strings_check(lib.dfgpu_string_take_views(stream, cols, len(srcs), C.byref(idc), C.c_void_p(views.ptr), C.c_void_p(validity.ptr),
+                                                   C.c_void_p(status.ptr)))
+        bad, nulls = (int(x) for x in status.to_numpy(np.int64, 2))
+        if bad:
+            raise DfgpuError(ERR_INVALID, f"string_take: {bad} ids outside their source")
+        host = [b for s in srcs for b in s.host_data]
+        return TakenStrings(ctx, layout, n, nulls, views, validity, [d for s in srcs for d in s.data], host, (srcs, owner))
+    offsets = DeviceBuffer(ctx, (n + 3) * 8)
+    scratch = DeviceBuffer(ctx, lib.dfgpu_string_take_scratch_bytes(n))
+    validity = DeviceBuffer(ctx, (n + 7) // 8)
+    _strings_check(lib.dfgpu_string_take_offsets(stream, cols, len(srcs), C.byref(idc), C.c_void_p(scratch.ptr), C.c_void_p(offsets.ptr),
+                                                 C.c_void_p(validity.ptr)))
+    total, bad, nulls = (int(x) for x in ctx.to_host(offsets.ptr + n * 8, 24).view(np.int64))
+    if bad:
+        raise DfgpuError(ERR_INVALID, f"string_take: {bad} ids outside their source")
+    if layout == STRING_UTF8 and total > 2**31 - 1:      # arrow's take refuses it the same way
+        raise DfgpuError(ERR_INVALID, f"string_take: offset overflow ({total} bytes do not fit a Utf8 array)")
+    data = DeviceBuffer(ctx, total)
+    out_offsets = DeviceBuffer(ctx, (n + 1) * 4) if layout == STRING_UTF8 else offsets
+    _strings_check(lib.dfgpu_string_take_data(stream, layout, n, total, C.c_void_p(scratch.ptr), C.c_void_p(offsets.ptr),
+                                              C.c_void_p(out_offsets.ptr), C.c_void_p(data.ptr)))
+    return TakenStrings(ctx, layout, n, nulls, out_offsets, validity, data, None, (srcs, owner, scratch, offsets))
 
 
 def device_column_numpy(col: DeviceColumn):

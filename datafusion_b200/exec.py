@@ -1528,6 +1528,8 @@ def _fuse(plan: ExecutionPlan, level: int) -> ExecutionPlan:
     join-keyed sink over a Left or an Inner join, and from _HASH_SINK on the hash sink; from _OUTPUT_SINK on, a plan none of those takes
     onto the ordered output sink.  From _JOIN_FILTERS on a probe chain's joins may carry JoinFilters, from _RIGHT_JOINS on it may
     contain Right joins, and at _FULL_JOINS a Full join.  Anything else is returned unchanged (the unfused Gpu*Exec operators run)."""
+    if isinstance(plan, GpuStringTakeExec):        # the gather of plan_string_payloads: fuse the plan of row ids under it
+        return _with_children(plan, lambda p: _fuse(p, level))
     joins = _Chain().joins | ({"Right"} if level >= _RIGHT_JOINS else set()) | ({"Full"} if level >= _FULL_JOINS else set())
     ch = _Chain(joins, filters=level >= _JOIN_FILTERS)
     fused = None
@@ -1755,6 +1757,372 @@ def plan_string_predicates(plan: ExecutionPlan) -> ExecutionPlan:
     string predicate that cannot run on the GPU (a column compared with a column, an IN list of anything but Utf8 literals or over the
     caps, a LIKE plan_like_predicates leaves), or when a raw string column a predicate reads is also read above the filter."""
     return _plan_masks(plan, strings=True)
+
+
+# ---------------------------------------------------------------------------------------------
+# string payloads — carried string columns as row ids, gathered after the operators (late materialisation, libdfgpu_strings.so)
+# ---------------------------------------------------------------------------------------------
+def _carried_type(t: pa.DataType) -> bool:
+    return pa.types.is_string(t) or pa.types.is_large_string(t) or pa.types.is_string_view(t)
+
+
+def _compact(a: pa.Array) -> pa.Array:
+    """a copy of a string array holding only its own rows' bytes: a batch sliced from a larger array shares the parent's buffers, and
+    uploading those would put the whole column on the device once per batch"""
+    if pa.types.is_string_view(a.type):
+        return a.cast(pa.large_string()).cast(pa.string_view())
+    return pa.concat_arrays([a])
+
+
+class StringPayloadStore:
+    """The device-resident strings of the sources GpuStringRowIdExec replaced, for one TaskContext.  A build-side source's batches are
+    concatenated into one array per column at its first gather (its ids are UINT32 rows of that array, as collect_left_input
+    concatenates the build); a streamed source keeps one array per column per batch (ids: batch << 32 | row).
+    Every batch is compacted to its own rows before it is uploaded.
+    Memory rule: a build-side source is held until the gather's execute ends, which is when its join's probe side has ended.  A streamed
+    source whose ids reach the gather in nondecreasing order releases every batch below the smallest id of each gathered batch: its path
+    to the gather runs through filters, projections, mask nodes and the probe side of joins that keep probe order (Inner, Left, Right,
+    Full, RightSemi, RightAnti, RightMark; the fused ordered output sink keeps it too).  Any other streamed source is held until the
+    gather's execute ends."""
+
+    def __init__(self):
+        self.sources: dict = {}     # key -> {"build": bool, "batches": {batch: [DeviceStrings]}, "host": [[pa.Array]], "whole": [DeviceStrings]}
+        self.held = self.peak = 0
+
+    def _add_bytes(self, n: int):
+        self.held += n
+        self.peak = max(self.peak, self.held)
+
+    def open(self, key, build: bool):
+        self.release(key)
+        self.sources[key] = {"build": build, "batches": {}, "host": [], "whole": None, "released": 0}
+
+    def push(self, ctx: TaskContext, key, batch: int, arrays: List[pa.Array]):
+        s = self.sources[key]
+        if s["build"]:
+            s["host"].append(arrays)                      # uploaded once, concatenated, at the first gather
+            return
+        ds = [D.DeviceStrings(ctx.gpu, _compact(a)) for a in arrays]
+        self._add_bytes(sum(d.nbytes for d in ds))
+        s["batches"][batch] = ds
+
+    def build_arrays(self, ctx: TaskContext, key) -> list:
+        s = self.sources[key]
+        if s["whole"] is None:
+            cols = list(zip(*s["host"])) if s["host"] else []
+            s["whole"] = [D.DeviceStrings(ctx.gpu, _compact(pa.concat_arrays(list(c)))) for c in cols]
+            s["host"] = []
+            self._add_bytes(sum(d.nbytes for d in s["whole"]))
+        return s["whole"]
+
+    def batches(self, key, lo: int, hi: int, col: int) -> list:
+        s = self.sources[key]
+        if lo < s["released"]:
+            raise RuntimeError(f"string payload batch {lo} of source {key} was released before its gather")
+        return [s["batches"][b][col] for b in range(lo, hi + 1)]
+
+    def release_below(self, key, batch: int):
+        s = self.sources[key]
+        for b in [b for b in s["batches"] if b < batch]:
+            self.held -= sum(d.nbytes for d in s["batches"].pop(b))
+        s["released"] = max(s["released"], batch)
+
+    def release(self, key):
+        s = self.sources.pop(key, None)
+        if s is None:
+            return
+        for ds in s["batches"].values():
+            self.held -= sum(d.nbytes for d in ds)
+        if s["whole"] is not None:
+            self.held -= sum(d.nbytes for d in s["whole"])
+
+
+def plan_string_payloads_store():
+    """a factory for the `store_of` argument: one StringPayloadStore per TaskContext, created on first use"""
+    cache = {}
+
+    def get(ctx: TaskContext) -> StringPayloadStore:
+        if id(ctx) not in cache:
+            cache[id(ctx)] = StringPayloadStore()
+        return cache[id(ctx)]
+    return get
+
+
+class GpuStringRowIdExec(ExecutionPlan):
+    """A source's carried string columns -> one row-id column (`id_name`, appended) and the strings kept on the device in the
+    StringPayloadStore; the columns `drop` (indices) leave the batch, and of them `keep` (indices) are stored.  build: UINT32 rows of
+    the concatenated source (a join's build side), else INT64 batch << 32 | row.  With no `keep` no id is made: the columns only go."""
+
+    def __init__(self, input: ExecutionPlan, drop: Sequence[int], keep: Sequence[int], id_name: str, build: bool, key, store_of):
+        self.input, self.drop, self.keep, self.id_name, self.build, self.key, self.store_of = input, list(drop), list(keep), id_name, build, key, store_of
+        fields = [f for i, f in enumerate(input.schema) if i not in self.drop]
+        if self.keep:
+            fields.append(pa.field(id_name, pa.uint32() if build else pa.int64(), False))
+        self.schema = pa.schema(fields)
+
+    def children(self): return [self.input]
+
+    def execute(self, ctx):
+        import numpy as np
+        store = self.store_of(ctx)
+        if self.keep:
+            store.open(self.key, self.build)
+        rows = 0
+        for b, rb in enumerate(self.input.execute(ctx)):
+            cols = [rb.column(i) for i in range(rb.num_columns) if i not in self.drop]
+            if self.keep:
+                store.push(ctx, self.key, b, [rb.column(i) for i in self.keep])
+                n = rb.num_rows
+                if self.build:
+                    if rows + n > 0xFFFFFFFF:
+                        raise NotImplementedError("This feature is not implemented: a build side of more than 2^32 - 1 rows carrying strings")
+                    cols.append(pa.array(np.arange(rows, rows + n, dtype=np.uint32)))
+                else:
+                    cols.append(pa.array((np.int64(b) << 32) | np.arange(n, dtype=np.int64)))
+                rows += n
+            yield pa.RecordBatch.from_arrays(cols, schema=self.schema)
+
+
+class GpuStringTakeExec(ExecutionPlan):
+    """The gather over a plan whose carried string columns travel as row ids: each output column is an input column (`('col', i)`)
+    or the strings its id column names (`('take', id column, source key, stored column)`), by dfgpu_string_take.  schema: the plan's
+    schema before plan_string_payloads.  ordered: the streamed source keys whose ids arrive nondecreasing (the store's release rule)."""
+
+    def __init__(self, input: ExecutionPlan, schema: pa.Schema, spec: Sequence[tuple], sources: dict, ordered: Sequence, store_of):
+        self.input, self.schema, self.spec, self.sources, self.ordered, self.store_of = input, schema, list(spec), dict(sources), set(ordered), store_of
+        self._metrics = {}
+
+    def children(self): return [self.input]
+
+    def _take(self, ctx, store, rb, idx: int, key, col: int) -> pa.Array:
+        import numpy as np
+        ids = rb.column(idx)
+        if ids.null_count == len(ids):                           # no id names a string (an empty batch, an unmatched outer side)
+            return pa.nulls(len(ids), self._type_of(key, col))
+        if self.sources[key]:                                    # a build side: UINT32 rows of one array
+            return D.string_take(ctx.gpu, [store.build_arrays(ctx, key)[col]], ids).to_arrow()
+        v = np.asarray(ids.fill_null(0)).astype(np.int64)
+        valid = np.asarray(ids.is_valid())
+        batch = v[valid] >> 32
+        lo, hi = int(batch.min()), int(batch.max())
+        packed = pa.array(v - (np.int64(lo) << 32), pa.int64(), mask=None if valid.all() else ~valid)
+        return D.string_take(ctx.gpu, store.batches(key, lo, hi, col), packed).to_arrow()
+
+    def _type_of(self, key, col):
+        for j, s in enumerate(self.spec):
+            if s[0] == "take" and s[2] == key and s[3] == col:
+                return self.schema.field(j).type
+
+    def execute(self, ctx):
+        import numpy as np
+        store = self.store_of(ctx)
+        store.peak = store.held
+        rows = 0
+        try:
+            for rb in self.input.execute(ctx):
+                cols = [rb.column(s[1]) if s[0] == "col" else self._take(ctx, store, rb, *s[1:]) for s in self.spec]
+                rows += rb.num_rows
+                yield pa.RecordBatch.from_arrays(cols, schema=self.schema)
+                for key in self.ordered:                         # nondecreasing ids: no later batch reaches below this one's smallest
+                    idx = next(s[1] for s in self.spec if s[0] == "take" and s[2] == key)
+                    ids = rb.column(idx).drop_null()
+                    if len(ids):
+                        store.release_below(key, int(np.asarray(ids).min()) >> 32)
+        finally:
+            for key in self.sources:
+                store.release(key)
+            self._metrics = {"output_rows": rows, "string_bytes_held": store.held, "peak_string_bytes_held": store.peak}
+
+    def metrics(self): return self._metrics
+
+
+_PAYLOAD_NODES = (GpuFilterExec, GpuHashJoinExec, GpuProjectionExec, GpuLikeExec)
+
+
+def _payload_origins(plan: ExecutionPlan, leaves: list, reads: set) -> list:
+    """the origin (leaf number, leaf column) of each output column of plan, None for a computed one; the leaves in visiting order; the
+    origins an operator reads (join keys and JoinFilter operands, predicate and mask inputs, computed projections)"""
+    def names(schema, origins, ns):
+        return {origins[i] for i, f in enumerate(schema) if f.name in ns}
+    if isinstance(plan, GpuFilterExec):
+        o = _payload_origins(plan.input, leaves, reads)
+        reads |= names(plan.input.schema, o, _expr_names(plan.predicate))
+        return o if plan.projection is None else [o[i] for i in plan.projection]
+    if isinstance(plan, GpuProjectionExec):
+        o = _payload_origins(plan.input, leaves, reads)
+        isch = plan.input.schema
+        out = []
+        for e, _ in plan.exprs:
+            if isinstance(e, Column):
+                out.append(o[isch.get_field_index(e.name)] if isch.get_field_index(e.name) >= 0 else None)
+            else:
+                reads |= names(isch, o, _expr_names(e))
+                out.append(None)
+        return out
+    if isinstance(plan, GpuLikeExec):
+        o = _payload_origins(plan.input, leaves, reads)
+        isch = plan.input.schema
+        reads |= names(isch, o, {_mask_column(e).name for e, _ in plan.likes})
+        return [o[i] for i, f in enumerate(isch) if f.name not in plan.drop] + [None] * len(plan.likes)
+    if isinstance(plan, GpuHashJoinExec):
+        lo = _payload_origins(plan.left, leaves, reads)
+        ro = _payload_origins(plan.right, leaves, reads)
+        reads |= names(plan.left.schema, lo, {l for l, _ in plan.on}) | names(plan.right.schema, ro, {r for _, r in plan.on})
+        if plan.filter is not None:
+            reads |= {(lo if sd == "left" else ro)[ix] for sd, ix in plan.filter.column_indices}
+        return [lo[i] if sd == 0 else ro[i] if sd == 1 else None for sd, i in plan.column_indices]
+    leaves.append(plan)
+    return [(len(leaves) - 1, i) for i in range(len(plan.schema))]
+
+
+_PROBE_ORDER = {"Inner", "Left", "Right", "Full", "RightSemi", "RightAnti", "RightMark"}   # joins whose output keeps probe order
+_PAYLOAD_REGIONS = iter(range(1 << 62))                                                    # store keys: (region, leaf)
+
+
+class _PayloadRewrite:
+    def __init__(self, carried: set, needed: set, store_of):
+        self.carried, self.needed, self.store_of = carried, needed, store_of
+        self.region = next(_PAYLOAD_REGIONS)
+        self.leaf = 0
+        self.kinds: dict = {}       # leaf -> build side?
+        self.ordered: set = set()   # streamed leaves whose ids reach the root in order
+
+    def id_name(self, leaf: int) -> str:
+        return f"__string_row_id_{leaf}"
+
+    def rewrite(self, plan: ExecutionPlan, build: bool, ordered: bool):
+        """-> (plan', tags): tags[i] = ('o', i of plan's output) or ('id', leaf) for each column of plan'"""
+        if isinstance(plan, GpuHashJoinExec):
+            return self.join(plan, ordered)
+        if not isinstance(plan, _PAYLOAD_NODES):
+            return self.source(plan, build, ordered)
+        new_in, it = self.rewrite(plan.input, build, ordered)
+        same = [("o", i) for i in range(len(plan.schema))]
+        if new_in is plan.input:
+            return plan, same
+        ids = [t for t in it if t[0] == "id"]
+        if isinstance(plan, GpuFilterExec):
+            if plan.projection is None:
+                return GpuFilterExec(plan.predicate, new_in, None, plan.fetch), it
+            keep = [(j, it.index(("o", i))) for j, i in enumerate(plan.projection) if ("o", i) in it]
+            proj = [p for _, p in keep] + [it.index(t) for t in ids]
+            return GpuFilterExec(plan.predicate, new_in, proj, plan.fetch), [("o", j) for j, _ in keep] + ids
+        if isinstance(plan, GpuProjectionExec):
+            isch = plan.input.schema
+            keep = [(j, e, n) for j, (e, n) in enumerate(plan.exprs)
+                    if not isinstance(e, Column) or ("o", isch.get_field_index(e.name)) in it]
+            exprs = [(e, n) for _, e, n in keep] + [(Column(self.id_name(t[1])), self.id_name(t[1])) for t in ids]
+            return GpuProjectionExec(exprs, new_in), [("o", j) for j, _, _ in keep] + ids
+        # GpuLikeExec: the input minus `drop`, then the masks
+        isch = plan.input.schema
+        out_of = {i: j for j, i in enumerate(i for i, f in enumerate(isch) if f.name not in plan.drop)}
+        tags = [("o", out_of[t[1]]) if t[0] == "o" else t for t in it if t[0] == "id" or isch.field(t[1]).name not in plan.drop]
+        n_in = len(out_of)
+        return GpuLikeExec(new_in, plan.likes, plan.drop, plan.dictionary_of), tags + [("o", n_in + k) for k in range(len(plan.likes))]
+
+    def source(self, plan: ExecutionPlan, build: bool, ordered: bool):
+        leaf = self.leaf
+        self.leaf += 1
+        inner = plan_string_payloads(plan, self.store_of)   # the operators under a node the rule does not pass through; same schema
+        drop = [i for i in range(len(plan.schema)) if (leaf, i) in self.carried]
+        if not drop:
+            return inner, [("o", i) for i in range(len(plan.schema))]
+        keep = [i for i in drop if (leaf, i) in self.needed]
+        node = GpuStringRowIdExec(inner, drop, keep, self.id_name(leaf), build, (self.region, leaf), self.store_of)
+        if keep:
+            self.kinds[leaf] = build
+            if ordered and not build:
+                self.ordered.add(leaf)
+        return node, [("o", i) for i in range(len(plan.schema)) if i not in drop] + ([("id", leaf)] if keep else [])
+
+    def join(self, plan: GpuHashJoinExec, ordered: bool):
+        nl, lt = self.rewrite(plan.left, True, False)
+        nr, rt = self.rewrite(plan.right, False, ordered and plan.join_type in _PROBE_ORDER)
+        if nl is plan.left and nr is plan.right:
+            return plan, [("o", i) for i in range(len(plan.schema))]
+        _, old_idx = build_join_schema(plan.left.schema, plan.right.schema, plan.join_type)
+        _, new_idx = build_join_schema(nl.schema, nr.schema, plan.join_type)
+        child = {0: lt, 1: rt}
+
+        def new_pos(sd, i):             # the new natural-output position of old child column (sd, i), -1 when it left
+            if sd == 2:
+                return new_idx.index((2, 0))
+            t = ("o", i)
+            return new_idx.index((sd, child[sd].index(t))) if t in child[sd] else -1
+        filt = plan.filter
+        if filt is not None:
+            filt = JoinFilter(filt.expression, [(sd, (lt if sd == "left" else rt).index(("o", ix))) for sd, ix in filt.column_indices])
+        id_pos = [p for p, (sd, i) in enumerate(new_idx) if sd != 2 and child[sd][i][0] == "id"]
+        if list(plan.column_indices) == old_idx:      # no projection
+            def tag(sd, i):
+                if sd == 2:
+                    return ("o", old_idx.index((2, 0)))
+                t = child[sd][i]
+                return ("o", old_idx.index((sd, t[1]))) if t[0] == "o" else t
+            tags = [tag(sd, i) for sd, i in new_idx]
+            return GpuHashJoinExec(nl, nr, plan.on, plan.join_type, plan.null_equality, filt, None, plan.null_aware), tags
+        keep = [(j, new_pos(sd, i)) for j, (sd, i) in enumerate(plan.column_indices)]
+        keep = [(j, p) for j, p in keep if p >= 0]
+        proj = [p for _, p in keep] + id_pos
+        tags = [("o", j) for j, _ in keep] + [child[new_idx[p][0]][new_idx[p][1]] for p in id_pos]
+        return GpuHashJoinExec(nl, nr, plan.on, plan.join_type, plan.null_equality, filt, proj, plan.null_aware), tags
+
+
+def plan_string_payloads(plan: ExecutionPlan, store_of=None) -> ExecutionPlan:
+    """PhysicalOptimizerRule twin (INTEGRATION.md §3c), after plan_string_predicates and ahead of the fusion rules: late materialisation
+    of the string columns a plan of GPU operators (GpuFilterExec, GpuHashJoinExec, GpuProjectionExec column pass-throughs, GpuLikeExec)
+    only carries.  Every Utf8, LargeUtf8 or Utf8View column of a source that no operator reads (not a join key, JoinFilter operand,
+    predicate or mask input, computed-projection input) leaves at the source: when some output needs one of a source's columns, a
+    GpuStringRowIdExec replaces them by one row-id column (UINT32 rows of the concatenated build on a join's build side, else INT64
+    batch << 32 | row) and keeps their strings on the device; else they are dropped outright.  The operators carry the ids as any
+    fixed-width column (NULL on the outer side of Left / Right / Full joins) and a GpuStringTakeExec at the plan's root gathers the
+    strings (dfgpu_string_take), emitting the plan's schema exactly.  A column an operator reads stays as it is.  Under a
+    GpuAggregateExec (not a Final mode) the operators' output is what the aggregate reads: its group and argument columns stay as they
+    are, the strings it does not read are dropped at their sources, and no gather is needed.  Any other node the rule does not pass
+    through gets the rule on its children.  A plan with no carried string column is returned as it is.  store_of: the
+    StringPayloadStore factory (plan_string_payloads_store())."""
+    store_of = store_of or plan_string_payloads_store()
+    if isinstance(plan, GpuAggregateExec) and not plan.state_input and isinstance(plan.input, _PAYLOAD_NODES):
+        read = set(plan.group_by) | {a.arg for a in plan.aggr_expr if a.arg} | {a.filter for a in plan.aggr_expr if a.filter}
+        new_in = _plan_payloads(plan.input, store_of, {i for i, f in enumerate(plan.input.schema) if f.name in read})
+        if new_in is plan.input:
+            return plan
+        return GpuAggregateExec(plan.mode, plan.group_by, plan.aggr_expr, new_in,
+                                None if plan.input_schema is plan.input.schema else plan.input_schema, plan.capacity_hint)
+    if not isinstance(plan, _PAYLOAD_NODES):
+        return _with_children(plan, lambda p: plan_string_payloads(p, store_of))
+    return _plan_payloads(plan, store_of, None)
+
+
+def _plan_payloads(plan: ExecutionPlan, store_of, read_above: Optional[set]) -> ExecutionPlan:
+    """plan_string_payloads on a plan whose root is one of its operators.  read_above: the output columns the node above reads, which
+    stay as they are while the other carried strings leave (None: the node above needs every output column as it is now)"""
+    leaves: list = []
+    reads: set = set()
+    origins = _payload_origins(plan, leaves, reads)
+    if read_above is not None:
+        reads |= {origins[j] for j in read_above if origins[j] is not None}
+    carried = {(k, i) for k, leaf in enumerate(leaves) for i, f in enumerate(leaf.schema) if _carried_type(f.type) and (k, i) not in reads}
+    wanted = range(len(origins)) if read_above is None else read_above
+    needed = {origins[j] for j in wanted if origins[j] in carried}
+    rw = _PayloadRewrite(carried, needed, store_of)
+    new, tags = rw.rewrite(plan, False, True)
+    if new is plan:
+        return plan
+    stored = {k: [i for i in range(len(leaves[k].schema)) if (k, i) in needed] for k in rw.kinds}
+    spec, fields = [], []
+    for j, o in enumerate(origins):
+        if ("o", j) in tags:
+            spec.append(("col", tags.index(("o", j))))
+        elif o in needed:
+            spec.append(("take", tags.index(("id", o[0])), (rw.region, o[0]), stored[o[0]].index(o[1])))
+        else:
+            continue                                     # a carried string nothing above reads: dropped at its source
+        fields.append(plan.schema.field(j))
+    if all(s[0] == "col" for s in spec):                 # no id was made, nothing to gather
+        return new
+    return GpuStringTakeExec(new, pa.schema(fields), spec, {(rw.region, k): b for k, b in rw.kinds.items()},
+                             {(rw.region, k) for k in rw.ordered}, store_of)
 
 
 def collect(plan: ExecutionPlan, ctx: Optional[TaskContext] = None) -> List[pa.RecordBatch]:

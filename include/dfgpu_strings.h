@@ -120,6 +120,36 @@ int dfgpu_string_in_list(void* stream, const dfgpu_string_column* col, const uin
 int dfgpu_like_codes(void* stream, const dfgpu_column* codes, const uint8_t* code_match, int64_t n_codes, uint8_t* out_values,
                      uint8_t* out_validity);
 
+/* ---- the gather: arrow-select's `take` over string arrays (late materialisation of carried string columns) ----
+ * sources: n_sources >= 1 string arrays of ONE layout, any slice offset, each at most 2^32 - 1 rows.  ids: a device dfgpu_column of
+ *   DFGPU_UINT32 rows of sources[0] (a join's build side, concatenated into one array), or of DFGPU_INT64 ids packed as
+ *   source << 32 | row (a streamed side whose output rows come from several batches), with its own offset and validity.
+ * Output row i is the string sources[src(i)][row(i)]: NULL where the id is NULL (the outer side of an outer join) or the source string
+ *   is NULL.  An id naming no source or a row outside its source is DFGPU_ERR_INVALID; the kernels cannot return it, so they count such
+ *   ids in a device word the caller reads with the output size (below), and the output row is NULL.
+ * Only the offsets / views of the rows the ids name, and those rows' bytes, are read.  Any number of sources works (64 to a launch). */
+
+/* Utf8 / LargeUtf8, phase 1.  scratch: dfgpu_string_take_scratch_bytes(ids->length) bytes of device memory, kept for phase 2.
+ * offsets: ids->length + 3 int64 of device memory.  Writes offsets[0 .. n) = the exclusive scan of the output rows' byte lengths (a
+ * NULL row takes 0 bytes), offsets[n] = the total bytes, offsets[n + 1] = the number of out-of-range ids (0 = no error),
+ * offsets[n + 2] = the number of NULL output rows; out_validity ((n + 7) / 8 bytes) receives the output validity rebased to bit 0. */
+int64_t dfgpu_string_take_scratch_bytes(int64_t n_ids);
+int dfgpu_string_take_offsets(void* stream, const dfgpu_string_column* sources, int32_t n_sources, const dfgpu_column* ids, void* scratch,
+                              int64_t* offsets, uint8_t* out_validity);
+/* Utf8 / LargeUtf8, phase 2, after the caller has read offsets[n .. n + 3) and refused out-of-range ids: layout: the sources' layout;
+ * total_bytes: offsets[n]; scratch and offsets as phase 1 left them.  Writes out_offsets (n + 1 int32 for Utf8, int64 for LargeUtf8,
+ * which may be `offsets` itself) and out_data (total_bytes bytes).  A Utf8 output beyond 2^31 - 1 bytes is DFGPU_ERR_INVALID ("offset
+ * overflow", as arrow's `take` refuses it). */
+int dfgpu_string_take_data(void* stream, int32_t layout, int64_t n_ids, int64_t total_bytes, const void* scratch, const int64_t* offsets,
+                           void* out_offsets, uint8_t* out_data);
+/* Utf8View: one phase.  Writes out_views (ids->length 16-byte views, 16-byte aligned): a view of 12 bytes or fewer as it is, a longer
+ * one with its buffer index rebased by its source's first buffer in the output's buffer list, which is the concatenation of the
+ * sources' data buffers in source order (no string byte is copied); a NULL row is a zero view.  out_validity: 4-byte aligned, room for
+ * (n + 31) / 32 32-bit words, receives the validity rebased to bit 0.  status: 2 int64 of device memory: [0] out-of-range ids, [1] NULL
+ * output rows. */
+int dfgpu_string_take_views(void* stream, const dfgpu_string_column* sources, int32_t n_sources, const dfgpu_column* ids, void* out_views,
+                            uint8_t* out_validity, int64_t* status);
+
 /* the message of this thread's last failed call ("" when none) */
 const char* dfgpu_strings_last_error(void);
 
